@@ -1,5 +1,5 @@
 #!/usr/bin/env python
-"""bench.py — trace rows/sec proven (Fibonacci, BASELINE.json metric) on N B200s of one node.
+"""bench.py — trace rows/sec proven (Fibonacci, BASELINE.json metric) on N GPUs (H100) of one node.
 
 A "step" is one full Machine::prove() of the workload (LDE + Keccak Merkle commits + LogUp perm trace
 + quotient + FRI opening), from traces to CBOR proof bytes.
@@ -11,6 +11,8 @@ A "step" is one full Machine::prove() of the workload (LDE + Keccak Merkle commi
            the N-independent-proofs figure is reported beside it under "replicas".
   --impl reference : the CPU restatement of the reference prover (oracle/, all host threads) on a
            bounded sample of the same workload; rank 0 only.
+  --dump-outputs DIR : after the timed steps, rank 0 writes what the last timed step returned (the proof bytes) to
+           DIR/proof_bytes.npy (float32, one element per byte), so that two builds can be compared output for output.
 """
 import argparse
 import ctypes as C
@@ -57,36 +59,7 @@ def peaks():
     if os.path.exists(p):
         d = json.load(open(p))
         return float(d["hbm_gbs"]), "measured (MEASURED_PEAKS.json hbm_gbs)"
-    return 6650.0, "fallback (B200_PROFILING.md)"
-
-
-def ncu_traffic_ratio(kernel):
-    """DRAM bytes moved / algorithmic bytes for one kernel class, from the committed `ncu --set full` raw pages:
-    ntt_pass_kernel: profiles/r02_ntt_v7_raw.csv (the shipping kernel: 8 launches over a 2^22 x 16 matrix, 8 B per element per launch);
-    compress_layer_kernel: profiles/r02_compress_raw.csv (the shipping kernel: tree layers of 2^24 .. 2^21 nodes, 96 B per node)."""
-    import csv
-
-    spec = {"ntt_pass_kernel": ("r02_ntt_v7_raw.csv", "ntt_pass", lambda gx, gy: 8.0 * gx * gy * (1 << 14)),      # a 2^14-element tile per CTA
-            "compress_layer_kernel": ("r02_compress_raw.csv", "compress_layer", lambda gx, gy: 96.0 * gx * 128)}  # a node per thread
-    if kernel not in spec:
-        return None, None
-    fname, tag, alg_bytes = spec[kernel]
-    path = os.path.join(ROOT, "profiles", fname)
-    try:
-        rows = list(csv.reader(open(path)))
-        hdr, units = rows[0], rows[1]
-        ir, iw, ig, ik = hdr.index("dram__bytes_read.sum"), hdr.index("dram__bytes_write.sum"), hdr.index("Grid Size"), hdr.index("Kernel Name")
-        scale = {"Mbyte": 1e6, "Gbyte": 1e9, "Kbyte": 1e3, "byte": 1.0}
-        tot, alg = 0.0, 0.0
-        for r in rows[2:]:
-            if tag not in r[ik]:
-                continue
-            tot += float(r[ir]) * scale[units[ir]] + float(r[iw]) * scale[units[iw]]
-            gx, gy = [int(v) for v in r[ig].strip("()").split(",")[:2]]
-            alg += alg_bytes(gx, gy)
-        return tot / alg, os.path.relpath(path, ROOT)
-    except Exception:
-        return None, None
+    return 3350.0, "H100 SXM data sheet (HBM3, 3.35 TB/s)"
 
 
 def aggregate_throughput(dist, rows_local, ms_local, device=None, sum_rows=True):
@@ -106,7 +79,7 @@ def aggregate_throughput(dist, rows_local, ms_local, device=None, sum_rows=True)
 class ClockSampler:
     """nvidia-smi clocks/throttle reasons during the timed region."""
 
-    Q = "clocks.sm,clocks.max.sm,power.draw,clocks_event_reasons.hw_slowdown,clocks_event_reasons.hw_thermal_slowdown,clocks_event_reasons.sw_thermal_slowdown,clocks_event_reasons.sw_power_cap"
+    Q = "clocks.sm,clocks.max.sm,power.draw,clocks_event_reasons.hw_slowdown,clocks_event_reasons.hw_thermal_slowdown,clocks_event_reasons.sw_thermal_slowdown,clocks_event_reasons.sw_power_cap,power.limit"
 
     def __init__(self, index):
         self.index, self.rows, self.stop_flag, self.th = index, [], False, None
@@ -136,7 +109,9 @@ class ClockSampler:
         for name, col in (("hw_slowdown", 3), ("hw_thermal_slowdown", 4), ("sw_thermal_slowdown", 5), ("sw_power_cap", 6)):
             if any(len(r) > col and r[col].lower().startswith("active") for r in self.rows):
                 reasons.append(name)
-        return {"sm_mhz": sm[len(sm) // 2] if sm else None, "sm_max_mhz": mx or None, "reasons": reasons, "samples": len(self.rows)}
+        limits = [r[7] for r in self.rows if len(r) > 7 and r[7].replace(".", "", 1).isdigit()]
+        return {"sm_mhz": sm[len(sm) // 2] if sm else None, "sm_max_mhz": mx or None, "power_limit_w": float(limits[0]) if limits else None,
+                "reasons": reasons, "samples": len(self.rows)}
 
 
 _HOST = None
@@ -455,6 +430,7 @@ def main():
     ap.add_argument("--cpu-baseline-log-rows", type=int, default=18)
     ap.add_argument("--no-cpu-baseline", action="store_true")
     ap.add_argument("--no-replicas", action="store_true", help="N > 1: skip the independent-proofs-per-GPU figure")
+    ap.add_argument("--dump-outputs", default=None, metavar="DIR", help="write the proof of the last timed step to DIR/proof_bytes.npy")
     ap.add_argument("--tracegen", default=None, help=argparse.SUPPRESS)
     args = ap.parse_args()
     if args.tracegen:
@@ -486,6 +462,7 @@ def main():
     if not os.path.exists(vb.lib_path):
         vbuild.build()
     torch.cuda.set_device(local_rank)
+    props = torch.cuda.get_device_properties(local_rank)
     dist = None
     if world > 1:
         import torch.distributed as dist_mod
@@ -570,6 +547,10 @@ def main():
         proof = vb.prove_machine(cfg, traces, device_resident=(dm, dp))
     ev1.record(stream)
     barrier()
+    if args.dump_outputs and rank == 0:
+        # the CBOR bytes of the last timed step, one float32 per byte (exact): the whole of what the timed call returns
+        os.makedirs(args.dump_outputs, exist_ok=True)
+        np.save(os.path.join(args.dump_outputs, "proof_bytes.npy"), np.frombuffer(proof, dtype=np.uint8).astype(np.float32))
     clocks = sampler.stop()
     ms_total = ev0.elapsed_time(ev1)
     launches = ctx.launch_count - launches0
@@ -713,47 +694,30 @@ def main():
         roofline = {"bound": "int_alu" if keccak_top else "hbm", "kernel": top[0], "achieved": achieved, "peak": peak, "unit": "GB/s", "frac": achieved / peak, "traffic": None,
                     "peak_source": peak_src, "share_of_step": top[2] / ms_instr, "ms_per_step_instrumented": ms_instr / args.steps}
         if keccak_top:
-            roofline["bound_note"] = ("the Keccak kernels run at the INT-ALU pipe's ceiling (LOP3/SHF), not at HBM's: `frac` is the HBM fraction the contract asks for, "
-                                      "`int_alu_ceiling` is the binding one (ncu: sm__inst_executed_pipe_alu 99.8 %, DRAM 0.98 x algorithmic bytes)")
-        # The Keccak kernels are bound by the INT ALU pipe, not by HBM (profiles/r01_summary.md section 4: 122 LOP3 + 58 SHF per
-        # round at 63 lanes/clk/SM = 4.32 G Keccak-f/s on this part, 4.30 measured stand-alone): report that ceiling beside the HBM one.
-        KECCAK_PEAK_GPERM = 4.43      # what the 2^24-node layer sustains at 99.8 % of the ALU pipe (profiles/r02_compress_raw.csv)
+            roofline["bound_note"] = ("the Keccak kernels are bound by the INT-ALU pipe (LOP3/SHF), not by HBM: `frac` is the HBM fraction, "
+                                      "`int_alu` gives their permutation rate")
         keccak = {}
         for name, bytes_per_perm in (("compress_layer_kernel", 96.0), ("fri_leaf_hash_kernel", 72.0)):
             kk = [k for k in kstats if k[0] == name]
             if kk and kk[0][2] > 0:
-                g = kk[0][3] / bytes_per_perm / (kk[0][2] / 1e3) / 1e9     # >= 1 permutation per `bytes_per_perm` algorithmic bytes
-                keccak[name] = {"achieved_gperm_s": g, "frac_of_alu_ceiling": g / KECCAK_PEAK_GPERM}
-        roofline["int_alu_ceiling"] = {"unit": "G Keccak-f/s", "peak": KECCAK_PEAK_GPERM, "kernels": keccak,
-                                       "note": "lower bounds: injected layers and multi-block leaves run more permutations than counted",
-                                       "ncu": "profiles/r02_compress_raw.csv: sm__inst_executed_pipe_alu 99.8 % (compress_layer_kernel of this round, 2^24 nodes in 3.79 ms = 4.43 G/s); r01_keccak_big_raw.csv: 92.8 % (leaf_hash_kernel)"}
-        ratio, ratio_src = ncu_traffic_ratio(top[0])
-        if ratio is not None:
-            # GB per launch, like `achieved`: the measured DRAM/algorithmic ratio of the committed capture applied to this
-            # run's average launch (ncu cannot run inside the timed region)
-            roofline["traffic"] = ratio * (top[3] / top[1]) / 1e9
-            roofline["algorithmic_gb_per_launch"] = (top[3] / top[1]) / 1e9
-            roofline["traffic_source"] = "%s: DRAM read+write = %.3f x algorithmic bytes" % (ratio_src, ratio)
+                keccak[name] = {"achieved_gperm_s": kk[0][3] / bytes_per_perm / (kk[0][2] / 1e3) / 1e9}     # >= 1 permutation per `bytes_per_perm` algorithmic bytes
+        roofline["int_alu"] = {"unit": "G Keccak-f/s", "kernels": keccak,
+                               "note": "lower bounds: injected layers and multi-block leaves run more permutations than counted"}
         ntt = [k for k in kstats if k[0] == "ntt_pass_kernel"]
         if ntt:
             a = (ntt[0][3] / 1e9) / (ntt[0][2] / 1e3)
             roofline["ntt_pass"] = {"achieved": a, "frac": a / peak, "unit": "GB/s", "bytes": "8 B per element per pass (read+write)"}
-            # What bounds a pass (ncu --set full of the shipping kernel, profiles/r02_ntt_v7_raw.csv + the source page): it is ISSUE bound,
-            # not HBM bound.  A radix-2 butterfly on 32-bit Montgomery words is 8 instructions (3 IMAD for the product, 3 adds, 2 min) =
-            # 4 per element-stage; a 14-stage pass executes 100.5 instructions per element (67 arithmetic — 56 butterfly floor + the
-            # inter-pass twiddle and its running product — 13.5 shared-memory accesses, 20 addressing / control) at 57-62 % issue-slot
-            # utilisation (two-way bank conflicts on the last radix-4 step, math-pipe throttle).  At the butterfly floor and full issue a
-            # pass would run at about the HBM peak; a transform is two passes, so its ALGORITHMIC rate (8 B per element per transform)
-            # is capped at half of whatever a pass reaches: 50 % of HBM at best, the north star's 70 % is not reachable in two passes.
-            sm_hz = (clocks.get("sm_mhz") or 1965) * 1e6
-            issue = 148 * 128 * sm_hz                                   # thread-instructions per second, one per lane per clock
-            roofline["ntt_pass"]["ceiling"] = {
-                "bound": "issue slots (INT32 butterflies), not HBM",
-                "gbs_per_pass_at_butterfly_floor": 8.0 * issue / (11.5 * 4) / 1e9,      # 11.5 stages per pass on average, 4 instructions per element-stage
-                "algorithmic_cap_of_a_two_pass_transform": "half of the per-pass rate",
-                "measured": {"instructions_per_element_14_stage_pass": 100.5, "of_which_arithmetic": 67, "butterfly_floor": 56, "issue_active_pct": "57-62",
-                             "gbs_per_pass_ncu": {"2^8-stage column pass": 3010, "2^10": "1580-2260", "2^14-stage row pass": "1460-1640"}},
-                "source": "profiles/r02_ntt_v7_raw.csv (ncu --set full, shipping kernel), profiles/r02_summary.md"}
+            # A pass is bound by issue slots, not by HBM: a radix-2 butterfly on 32-bit Montgomery words is 8 instructions
+            # (3 IMAD for the product, 3 adds, 2 min) = 4 per element-stage.  A transform is two passes, so its ALGORITHMIC
+            # rate (8 B per element per transform) is at most half of what a pass reaches.
+            sm_mhz = clocks.get("sm_mhz") or clocks.get("sm_max_mhz")
+            if sm_mhz:
+                issue = props.multi_processor_count * 128 * sm_mhz * 1e6    # thread-instructions per second, one per lane per clock
+                roofline["ntt_pass"]["ceiling"] = {
+                    "bound": "issue slots (INT32 butterflies), not HBM",
+                    "gbs_per_pass_at_butterfly_floor": 8.0 * issue / (11.5 * 4) / 1e9,      # 11.5 stages per pass on average, 4 instructions per element-stage
+                    "sms": props.multi_processor_count, "sm_mhz": sm_mhz,
+                    "algorithmic_cap_of_a_two_pass_transform": "half of the per-pass rate"}
 
         # ---- second headline figure: BASELINE config 2 — 2^20 x 64 BabyBear NTT + inverse, device resident ----
         ntt_line = None
@@ -801,7 +765,7 @@ def main():
                     d2.free()
                     g2 = 2 * 8.0 * hh * w2 / (ms2 / 1e3) / 1e9
                     others["2^20 x %d" % w2] = {"ms_forward_plus_inverse": ms2, "achieved": g2, "unit": "GB/s", "frac": g2 / peak, "roundtrip_bit_exact": ok2,
-                                               "l2": "working set %d MiB %s L2" % (hh * w2 * 4 >> 20, ">" if hh * w2 * 4 > 126 << 20 else "fits in")}
+                                               "l2": "working set %d MiB %s L2" % (hh * w2 * 4 >> 20, ">" if hh * w2 * 4 > props.L2_cache_size else "fits in")}
                 ntt_line["other_widths"] = others
             except Exception as exc:   # noqa: BLE001
                 ntt_line["other_widths"] = {"error": "%s: %s" % (type(exc).__name__, exc)}
@@ -826,6 +790,7 @@ def main():
             "e2e": {"value": e2e_value, "unit": "rows/s", "h2d_bytes_per_step": h2d_total, "d2h_bytes_per_step": len(proof) * G,
                     "note": "every rank copies its rows of the tall traces (1/N of them) and the short traces whole; every rank reads the proof back; `value` is from page-locked (torch pinned) buffers",
                     "other_host_memory": e2e_other},
+            "gpu": props.name,
             "gpu_launches": launches,
             "clocks": clocks,
             "roofline": roofline,

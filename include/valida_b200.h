@@ -1,4 +1,4 @@
-/* valida_b200 — C ABI of the B200-native STARK prover backend for Valida's Machine::prove().
+/* valida_b200 — C ABI of the GPU-native (H100, sm_90a) STARK prover backend for Valida's Machine::prove().
  *
  * The reference (valida-xyz/valida @ 5058de85) has NO FFI boundary (SURVEY.md §0-D8): its only seam
  * is the Rust generic `StarkConfig::Pcs: UnivariatePcsWithLde<..>` (machine/src/config.rs:7-31) plus
@@ -46,6 +46,9 @@ const char* vgpu_last_error(const vgpu_ctx* ctx);
 int32_t vgpu_ctx_synchronize(vgpu_ctx* ctx);
 /* Number of kernels this context has launched since creation (bench.py's gpu_launches). */
 uint64_t vgpu_ctx_launch_count(const vgpu_ctx* ctx);
+/* Frees the device buffers the context keeps for reuse by its next calls (otherwise held until vgpu_ctx_destroy): after a
+ * proof that filled most of the GPU's memory, this hands that memory back to other contexts and libraries. */
+int32_t vgpu_ctx_release_cached(vgpu_ctx* ctx);
 /* Optional per-kernel-class CUDA-event timing (event pairs on the context's stream around every launch).
  * vgpu_ctx_kernel_stats synchronises, drains the records and returns the number of classes written:
  * names[i] (static strings), launches, summed milliseconds and summed algorithmic bytes (DESIGN.md). */

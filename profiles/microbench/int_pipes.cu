@@ -1,5 +1,5 @@
-// Issue-rate microbenchmark for the integer instruction mix of BabyBear arithmetic and Keccak on sm_100a.
-// Each kernel runs ILP=8 independent dependency chains per thread, 1024 threads x 148*2 blocks, 4096 iterations.
+// Issue-rate microbenchmark for the integer instruction mix of BabyBear arithmetic and Keccak on sm_90a.
+// Each kernel runs ILP=8 independent dependency chains per thread, 1024 threads x 2 blocks per SM, 4096 iterations.
 #include <cstdio>
 #include <cstdint>
 #include <cuda_runtime.h>
@@ -35,16 +35,18 @@ template <int OP> __global__ void k(uint32_t* out, uint32_t seed, uint32_t c) {
     out[blockIdx.x * blockDim.x + threadIdx.x] = s;
 }
 template <int OP> void run(const char* name, int per_iter_instr) {
-    uint32_t* d; cudaMalloc(&d, 296 * 1024 * 4);
+    int sms; cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, 0);
+    const int blocks = 2 * sms;
+    uint32_t* d; cudaMalloc(&d, blocks * 1024 * 4);
     cudaEvent_t e0, e1; cudaEventCreate(&e0); cudaEventCreate(&e1);
-    k<OP><<<296, 1024>>>(d, 1, 0x12345671u);
+    k<OP><<<blocks, 1024>>>(d, 1, 0x12345671u);
     cudaEventRecord(e0);
-    k<OP><<<296, 1024>>>(d, 2, 0x12345671u);
+    k<OP><<<blocks, 1024>>>(d, 2, 0x12345671u);
     cudaEventRecord(e1); cudaEventSynchronize(e1);
     float ms; cudaEventElapsedTime(&ms, e0, e1);
-    double ops = 296.0 * 1024 * ITER * ILP;
+    double ops = (double)blocks * 1024 * ITER * ILP;
     int clk; cudaDeviceGetAttribute(&clk, cudaDevAttrClockRate, 0);
-    printf("%-28s %8.3f ms  %7.2f Gop/s  = %6.2f lane-ops/clk/SM at %d MHz (%d instr/op)\n", name, ms, ops / ms / 1e6, ops / (ms * 1e-3) / 148 / (clk * 1e3), clk / 1000, per_iter_instr);
+    printf("%-28s %8.3f ms  %7.2f Gop/s  = %6.2f lane-ops/clk/SM at %d MHz (%d instr/op)\n", name, ms, ops / ms / 1e6, ops / (ms * 1e-3) / sms / (clk * 1e3), clk / 1000, per_iter_instr);
     cudaFree(d);
 }
 int main() {

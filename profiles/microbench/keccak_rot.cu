@@ -14,7 +14,8 @@ __global__ void __launch_bounds__(128) k(uint32_t* out, uint32_t seed) {
     out[blockIdx.x * 128 + threadIdx.x] = s;
 }
 int main() {
-    const int blocks = 148 * 64;
+    int sms; cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, 0);
+    const int blocks = sms * 64;
     uint32_t* d; cudaMalloc(&d, blocks * 128 * 4);
     cudaEvent_t e0, e1; cudaEventCreate(&e0); cudaEventCreate(&e1);
     k<<<blocks, 128>>>(d, 1);

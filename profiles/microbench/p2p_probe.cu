@@ -1,6 +1,6 @@
 // Probe for the multi-GPU data path: (1) does CUDA IPC work between two PROCESSES on this box (one rank per GPU,
 // torchrun style), (2) what do kernel-issued peer stores / loads over NVLink sustain.
-// Build: nvcc -gencode arch=compute_100a,code=sm_100a -O3 -o p2p_probe p2p_probe.cu ; run with >= 2 GPUs visible.
+// Build: nvcc -gencode arch=compute_90a,code=sm_90a -O3 -o p2p_probe p2p_probe.cu ; run with >= 2 GPUs visible.
 #include <cuda_runtime.h>
 #include <cstdint>
 #include <cstdio>
@@ -52,7 +52,8 @@ int main() {
         if (e != cudaSuccess) { printf("IPC open FAILED: %s\n", cudaGetErrorString(e)); fflush(stdout); char c = 'x'; (void)!write(c2p[1], &c, 1); return 0; }
         printf("IPC open ok\n");
         void* local = nullptr; CK(cudaMalloc(&local, bytes)); CK(cudaMemset(local, 0x5a, bytes));
-        for (int blocks : {148, 592, 2368}) {
+        int sms; CK(cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, 1));
+        for (int blocks : {sms, 4 * sms, 16 * sms}) {
             float w16 = time_copy(local, peer, bytes, true, blocks), r16 = time_copy(peer, local, bytes, true, blocks);
             float w4 = time_copy(local, peer, bytes, false, blocks), r4 = time_copy(peer, local, bytes, false, blocks);
             printf("IPC blocks=%d: peer store 16B %.0f GB/s, peer load 16B %.0f GB/s, store 4B %.0f GB/s, load 4B %.0f GB/s\n", blocks,

@@ -1,4 +1,4 @@
-// Links libvalida_b200.so (built by `python -m valida_b200.build`: nvcc -gencode arch=compute_100a,code=sm_100a over
+// Links libvalida_b200.so (built by `python -m valida_b200.build`: nvcc -gencode arch=compute_90a,code=sm_90a over
 // valida_b200/csrc/**).  VALIDA_B200_LIB_DIR names the directory holding it; the default is this repository's
 // valida_b200/ directory, two levels above the crate.
 use std::env;

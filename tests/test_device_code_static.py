@@ -1,6 +1,6 @@
 """Static checks of the device code inside the built library (CPU; cuobjdump ships with the CUDA toolkit): every translation
-unit is compiled for sm_100a and nothing else, the kernels of the hot path are present, and the hot ones keep their state in
-registers (no stack frame = no spills; the figures are the ones profiles/r02_sass_mix.md was written from)."""
+unit is compiled for sm_90a (H100) and nothing else, the kernels of the hot path are present, and the hot ones keep their state in
+registers (no stack frame = no spills)."""
 import os
 import re
 import shutil
@@ -19,11 +19,11 @@ def _run(*args):
     return subprocess.run([CUOBJDUMP, *args, LIB], capture_output=True, text=True, check=True).stdout
 
 
-def test_every_cubin_is_sm_100a():
+def test_every_cubin_is_sm_90a():
     elfs = re.findall(r"ELF file\s+\d+:\s+(\S+)", _run("-lelf"))
     assert len(elfs) >= 10, elfs                                   # one per .cu translation unit
-    assert all(e.endswith(".sm_100a.cubin") for e in elfs), elfs
-    # no PTX for a JIT to fall back on: the product is sm_100a code, compiled ahead of time
+    assert all(e.endswith(".sm_90a.cubin") for e in elfs), elfs
+    # no PTX for a JIT to fall back on: the product is sm_90a code, compiled ahead of time
     ptx = subprocess.run([CUOBJDUMP, "-lptx", LIB], capture_output=True, text=True).stdout
     assert "PTX file" not in ptx, ptx
 

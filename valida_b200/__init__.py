@@ -1,4 +1,4 @@
-"""valida_b200 — B200-native STARK prover backend for Valida's Machine::prove() hot path.
+"""valida_b200 — GPU-native (H100, sm_90a) STARK prover backend for Valida's Machine::prove() hot path.
 
 Host-side mirror of the reference's prover-facing interface (StarkConfig / UnivariatePcsWithLde /
 Machine::prove) over the C ABI in include/valida_b200.h.  There is no CPU fallback: constructing a

@@ -43,6 +43,7 @@ def _load():
         "vgpu_last_error": (C.c_char_p, [vp]),
         "vgpu_ctx_synchronize": (C.c_int32, [vp]),
         "vgpu_ctx_launch_count": (u64, [vp]),
+        "vgpu_ctx_release_cached": (C.c_int32, [vp]),
         "vgpu_ctx_set_kernel_timing": (C.c_int32, [vp, C.c_int32]),
         "vgpu_ctx_kernel_stats": (C.c_uint32, [vp, C.POINTER(C.c_char_p), u32p, C.POINTER(C.c_float), C.POINTER(C.c_double), C.c_uint32]),
         "vgpu_host_register": (C.c_int32, [vp, vp, u64]),
@@ -140,6 +141,10 @@ class Context:
 
     def synchronize(self):
         self.check(lib().vgpu_ctx_synchronize(self._h))
+
+    def release_cached(self):
+        """Free the device buffers kept for reuse by later calls (e.g. after a proof that filled most of the GPU)."""
+        self.check(lib().vgpu_ctx_release_cached(self._h))
 
     @property
     def launch_count(self):

@@ -169,6 +169,13 @@ void vgpu_ctx_destroy(vgpu_ctx* ctx) {
 const char* vgpu_last_error(const vgpu_ctx* ctx) { return ctx ? ctx->err.c_str() : "null context"; }
 int32_t vgpu_ctx_synchronize(vgpu_ctx* ctx) { VG_CUDA(ctx, cudaStreamSynchronize(ctx->stream)); return 0; }
 uint64_t vgpu_ctx_launch_count(const vgpu_ctx* ctx) { return ctx->launches; }
+int32_t vgpu_ctx_release_cached(vgpu_ctx* ctx) {
+    VG_TRY(vg_enter(ctx));
+    VG_CUDA(ctx, cudaStreamSynchronize(ctx->stream));   // a cached block may still be read by queued work
+    for (auto& kv : ctx->free_bufs) cudaFree(kv.second);
+    ctx->free_bufs.clear(); ctx->cached_bytes = 0;
+    return 0;
+}
 
 int32_t vgpu_ctx_set_kernel_timing(vgpu_ctx* ctx, int32_t on) { ctx->ktiming = on != 0; return 0; }
 static const char* KCLASS_NAMES[KC_COUNT] = {"ntt_pass_kernel", "leaf_hash_kernel", "compress_layer_kernel", "fri_leaf_hash_kernel", "transpose (rm<->cm)",

@@ -1,4 +1,4 @@
-// BabyBear (p = 2^31 - 2^27 + 1) and its degree-5 binomial extension (X^5 = 2) for sm_100a.
+// BabyBear (p = 2^31 - 2^27 + 1) and its degree-5 binomial extension (X^5 = 2) for sm_90a.
 // Replaces p3-baby-bear / p3-field arithmetic used throughout the reference's proving path
 // (e.g. machine/src/chip.rs:174,194-197; machine/src/quotient.rs:199-226).
 // Device words are in MONTGOMERY form (R = 2^32), the same storage p3_baby_bear::BabyBear uses,

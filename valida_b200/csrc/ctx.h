@@ -31,7 +31,7 @@ struct vgpu_ctx {
     bool own_stream = false;
     std::string err;
     uint64_t launches = 0;
-    int sm_count = 148;
+    int sm_count = 132;
     PowTable root_table;                                        // base = two_adic_generator(27)
     uint32_t* root3 = nullptr;                                   // 3 x 512 words: w^(i), w^(512 i), w^(2^18 i) — a 6 KB, L1-resident form of the same table
     std::map<std::pair<uint32_t, uint32_t>, PowTable> shift_tables;  // (shift, scale) canonical -> table

@@ -450,8 +450,11 @@ int32_t vgpu_open(vgpu_ctx* ctx, const vgpu_prover_data* const* rounds, uint32_t
     return 0;
 }
 
-int32_t vgpu_prove_device(vgpu_ctx* ctx, const vgpu_dmat* const main[VGPU_NUM_CHIPS], const vgpu_dmat* const prep[2],
-                          uint8_t** proof_out, uint64_t* proof_len) {
+// owned_main: the caller's main traces when this call may release them once the permutation traces are built (their last
+// use), or null.  vgpu_prove passes the device copies it made itself: on an 80 GB part that is what lets a 2^24-row trace
+// (memory chip 2^26 rows, LDE 2^27) be proven on one GPU.
+static int32_t prove_device(vgpu_ctx* ctx, const vgpu_dmat* const main[VGPU_NUM_CHIPS], const vgpu_dmat* const prep[2],
+                            vgpu_dmat* const* owned_main, uint8_t** proof_out, uint64_t* proof_len) {
     if (!ctx->challenger_set) VG_FAIL(ctx, "prove: vgpu_set_challenger has not been called");
     if (!proof_out || !proof_len) VG_FAIL(ctx, "prove: null output");
     VG_TRY(vg_enter(ctx));
@@ -521,6 +524,11 @@ int32_t vgpu_prove_device(vgpu_ctx* ctx, const vgpu_dmat* const main[VGPU_NUM_CH
                     for (uint32_t r = 0; r < nt[i]; r++) a = bb::add(a, ht[((size_t)i * slots + r) * 5 + l]);
                     cumsum[i][l] = bb::from_monty(a);
                 }
+            // later work reuses the released blocks in stream order, i.e. after the permutation kernels that read them
+            for (int i = 0; owned_main && i < VGPU_NUM_CHIPS; i++) {
+                vgpu_dmat* m = owned_main[i];
+                if (m->owns && !m->symm && !m->pend_stage) { vg_free(ctx, m->d); m->d = nullptr; }
+            }
         }
         Phase ph(ctx, "commit permutation");
         VG_TRY(vgpu_commit_batches(ctx, perms.v.data(), VGPU_NUM_CHIPS, nullptr, perm_commit.data(), &perm_pd.p));
@@ -597,6 +605,11 @@ int32_t vgpu_prove_device(vgpu_ctx* ctx, const vgpu_dmat* const main[VGPU_NUM_CH
     return 0;
 }
 
+int32_t vgpu_prove_device(vgpu_ctx* ctx, const vgpu_dmat* const main[VGPU_NUM_CHIPS], const vgpu_dmat* const prep[2],
+                          uint8_t** proof_out, uint64_t* proof_len) {
+    return prove_device(ctx, main, prep, nullptr, proof_out, proof_len);
+}
+
 int32_t vgpu_prove(vgpu_ctx* ctx, const vgpu_matrix main[VGPU_NUM_CHIPS], const vgpu_matrix prep[2], int32_t repr,
                    uint8_t** proof_out, uint64_t* proof_len) {
     // Host-buffer entry: the H2D copies run on a copy stream in the order the commits consume the traces (preprocessed,
@@ -626,7 +639,7 @@ int32_t vgpu_prove(vgpu_ctx* ctx, const vgpu_matrix main[VGPU_NUM_CHIPS], const 
     struct StagerGuard { vgpu_ctx* c; ~StagerGuard() { vg_stager_finish(c); } } sg{ctx};
     VG_TRY(vg_stager_start(ctx));
     ctx->in_host_prove = true;
-    int32_t rc = vgpu_prove_device(ctx, dm.v.data(), dp.v.data(), proof_out, proof_len);
+    int32_t rc = prove_device(ctx, dm.v.data(), dp.v.data(), dm.v.data(), proof_out, proof_len);
     ctx->in_host_prove = false;
     if (rc == 0) rc = vg_stager_finish(ctx);
     return rc;

@@ -1,4 +1,4 @@
-// Keccak-f[1600] on 32-bit register pairs for sm_100a (LOP3 for theta/chi with D folded into a 3-input
+// Keccak-f[1600] on 32-bit register pairs for sm_90a (LOP3 for theta/chi with D folded into a 3-input
 // xor, SHF funnel shifts for rho; optional multiply-add rotations on the FMA pipe).
 // Replaces tiny-keccak's keccakf as used by p3-keccak::Keccak256Hash inside
 // SerializingHasher32 / CompressionFunctionFromHasher (basic/src/bin/valida.rs:367-371).
@@ -35,8 +35,8 @@ template <int M> __device__ __forceinline__ uint2 rol_small(uint2 a) {
 }
 // x = lo, y = hi
 // Rotation amounts listed in KK_FMA_ROT_MASK (bit n set = rotate-by-n uses the multiply-add form) go to the
-// FMA pipe, the rest are SHF funnel shifts on the INT ALU pipe next to the LOP3s.  Measured on B200
-// (profiles/r01_keccak_rot.md): the all-IMAD variant is 19% SLOWER than all-SHF, so the default mask is 0.
+// FMA pipe, the rest are SHF funnel shifts on the INT ALU pipe next to the LOP3s.  The default mask 0
+// keeps every rotation on SHF; profiles/microbench/keccak_rot.cu times the alternatives.
 #ifndef KK_FMA_ROT_MASK
 #define KK_FMA_ROT_MASK 0ull
 #endif

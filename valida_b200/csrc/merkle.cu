@@ -1,4 +1,4 @@
-// K3/K4 — Keccak-256 Merkle commitment over mixed-height column-major LDE matrices (sm_100a).
+// K3/K4 — Keccak-256 Merkle commitment over mixed-height column-major LDE matrices (sm_90a).
 // Replaces FieldMerkleTreeMmcs<BabyBear, SerializingHasher32<Keccak256Hash>,
 // CompressionFunctionFromHasher<_,_,2,8>, 8>::commit (basic/src/bin/valida.rs:367-374) as reached
 // from TwoAdicFriPcs::commit_shifted_batches (derive/src/lib.rs:309,330,355,372).
@@ -170,7 +170,8 @@ struct TailParams {
     uint32_t sub;             // nodes of the first fused layer per CTA (power of two <= TAIL_SUB)
     uint32_t levels;          // fused levels: level k has sub >> k nodes per CTA
 };
-__global__ void __launch_bounds__(TAIL_THREADS) tree_tail_kernel(const __grid_constant__ TailParams p) {
+// at most 80 registers (launched with TAIL_THREADS threads): left to itself ptxas takes 89 on sm_90a
+__global__ void __maxnreg__(80) tree_tail_kernel(const __grid_constant__ TailParams p) {
     __shared__ uint4 buf_a[2 * TAIL_SUB * 2];     // children of the current level: 2 * sub digests (two uint4 each)
     __shared__ uint4 buf_b[TAIL_SUB * 2];
     const uint64_t node0 = p.first_begin + (uint64_t)blockIdx.x * p.sub;

@@ -1,9 +1,9 @@
-// K1/K2 — batched BabyBear NTT / iNTT / coset-LDE over column-major device matrices (sm_100a).
+// K1/K2 — batched BabyBear NTT / iNTT / coset-LDE over column-major device matrices (sm_90a).
 // Replaces p3-dft's TwoAdicSubgroupDft::{dft_batch, idft_batch, coset_lde_batch} as reached from
 // TwoAdicFriPcs::commit_shifted_batches (reference call sites derive/src/lib.rs:309,330,355,372;
 // DFT selected at basic/src/bin/valida.rs:379).
 //
-// Design (B200-first, not the reference's row-major butterfly network):
+// Design (GPU-first, not the reference's row-major butterfly network):
 //  * a length-n column transform is split n = n1*n2 ("four-step"); each pass stages a tile of T
 //    sub-transforms of length L in shared memory and runs ALL log2(L) DIF stages there, four stages
 //    at a time in registers (radix-16 units: 16 loads, 32 butterflies, 16 stores per thread-unit, one
@@ -147,8 +147,7 @@ __device__ __forceinline__ void all_stages(uint32_t* data, const uint32_t* tw, u
 // (T = 2^(14 - LOG_LEN) sub-transforms of length L).  For that shape the per-thread sequence of 32 elements is a
 // compile-time pattern: one base address / base slot per thread, everything else immediates (bit reversals of the
 // step counter, padded-slot corrections, group pitches).  The generic index arithmetic below these helpers remains
-// for short columns and unusual shapes.  (ncu, profiles/r01_summary.md: the generic paths cost 45 - 90 executed
-// instructions per element, more than the butterflies.)
+// for short columns and unusual shapes; it executes more instructions per element than the butterflies do.
 __host__ __device__ constexpr uint32_t cbrev(uint32_t x, int bits) {
     uint32_t r = 0;
     for (int i = 0; i < bits; i++) r |= ((x >> i) & 1u) << (bits - 1 - i);
@@ -222,7 +221,7 @@ __device__ __forceinline__ void load_rows_odd_std(const PassParams& p, const uin
     const uint32_t B = bb::reverse_bits(tid, 9);
     const uint32_t sb = base_rowrev<S::LB>(B);
     const uint32_t step = root_pow(p, p.pre_r << p.pre_shift);
-#pragma unroll
+#pragma unroll 8   // fully unrolled, the 16-group tile of L = 2^10 spills a register pair on sm_90a
     for (uint32_t t = 0; t < S::T; t++) {
         const uint32_t g = (uint32_t)g0 + t;
         const uint32_t gval = p.g_bits ? bb::reverse_bits(g, (int)p.g_bits) : g;

@@ -10,8 +10,7 @@
 // the pair exchanges its ext5 value with one shuffle, and the even / odd lane writes the even / odd
 // chunk limbs.  Every trace load and every chunk store is a fully coalesced 4-byte-per-lane access
 // (the chunk matrix is left in bit-reversed row order; the quotient commit's iNTT reads it that way).
-// ncu on the first version (pair per thread, natural-order scatter): 3.2x the algorithmic DRAM reads
-// and 9x the writes; see profiles/r01_summary.md.
+// (A pair per thread with a natural-order scatter, the first version, moved several times the algorithmic bytes.)
 // alpha-folding: acc = sum_i c_i * alpha^(N-1-i) with precomputed powers — the same value as the
 // reference's Horner recurrence acc = acc*alpha + c_i, at 5 instead of 25 multiplications for the
 // base-field constraints.  The sum is accumulated LAZILY (bb::Lazy5: raw 64-bit products, one IMAD.WIDE

@@ -295,7 +295,7 @@ int32_t sort_log_by_addr(vgpu_ctx* ctx, const VgMemOp* d_mem, uint64_t n, DevBuf
     VG_TRY(vg_alloc(ctx, &bits.p, 8));
     const uint32_t init[2] = {0u, 0xffffffffu};
     VG_CUDA(ctx, cudaMemcpyAsync(bits.p, init, 8, cudaMemcpyHostToDevice, ctx->stream));
-    addr_bits_kernel<<<296, 256, 0, ctx->stream>>>(d_mem, n, bits.as<uint32_t>());
+    addr_bits_kernel<<<2 * ctx->sm_count, 256, 0, ctx->stream>>>(d_mem, n, bits.as<uint32_t>());
     VG_LAUNCH_CHECK(ctx);
     uint32_t oa[2];
     VG_CUDA(ctx, cudaMemcpyAsync(oa, bits.p, 8, cudaMemcpyDeviceToHost, ctx->stream));
