@@ -1,7 +1,8 @@
 """The product's BabyBear / ext5 arithmetic (valida_b200/csrc/bb.cuh) instantiated on the host and checked against plain Python
 integers: Montgomery form R = 2^32, X^5 = 2, Frobenius inverse, bit reversal, two-adic generators.  The same text is what every
-kernel compiles (its __CUDA_ARCH__ branches — __umulhi, the lazy 64-bit accumulators — are covered by the GPU parity tests);
-the host instantiation is what the verifier and the transcript run."""
+kernel compiles; its __CUDA_ARCH__ branches — __umulhi, __brev, the lazy 64-bit accumulators Lazy5 — are checked the same way,
+on the device and at their bounds, by test_gpu_bb_device_arith.py.  The host instantiation is what the verifier and the
+transcript run."""
 import os
 import random
 import subprocess

@@ -107,7 +107,67 @@ def test_prove_reference_test_programs_bytes_equal(ctx, oracle, name):
     assert oracle.verify(proof, t.preprocessed) == 0
 
 
-from programs import config5_program, mixed_program  # noqa: E402
+from programs import (config5_program, loads_stores_edge_program, lt_edge_operands_program, mixed_program,  # noqa: E402
+                      single_address_program)
+
+
+def _lt_edges_without_double_immediate():
+    prog = lt_edge_operands_program()
+    assert prog[-2].tolist() == [115, -104, 7, 7, 1, 1]
+    return np.concatenate([prog[:-2], prog[-1:]])
+
+
+@pytest.mark.parametrize("name", ["lt_edges", "lone_stop", "single_address"])
+def test_prove_edge_programs_bytes_equal(ctx, oracle, name):
+    """Proofs of traces at the witness builders' edges: the lt family on equal operands, on a difference in the top byte only and
+    at the sign boundaries (the lt edge program without its both-immediates instruction, see below); a lone STOP; a memory log
+    at one address.  Bytes equal to the oracle's, and the oracle verifier accepts."""
+    import valida_b200 as vb
+
+    prog = {"lt_edges": _lt_edges_without_double_immediate, "lone_stop": lambda: np.array([[8, 0, 0, 0, 0, 0]], dtype=np.int32),
+            "single_address": lambda: single_address_program(5)}[name]()
+    t = vb.run_program(prog, initial_fp=0x1000)
+    ref = oracle.prove(t.main, t.preprocessed, debug_checks=True)
+    assert ref.constraint_failures() == [-1] * 14 and ref.cumulative_sum_zero()
+    proof = gpu_prove(ctx, oracle, t)
+    assert proof == ref.cbor()
+    assert oracle.verify(proof, t.preprocessed) == 0
+
+
+@pytest.mark.parametrize("name", ["lt_edges", "loads_stores"])
+def test_edge_programs_the_cpu_air_rejects(ctx, oracle, name):
+    """The two edge programs unchanged are not provable, in the reference either.  A store32 reads the pointer at fp + b on its
+    first memory channel (cpu/src/lib.rs:615-631) where the CPU AIR asks for fp + c, and an lte32 with both operands immediate
+    reads its second operand at an address the AIR's read-address constraint does not accept.  Every stage up to the quotient is
+    still compared bit for bit with the oracle on these traces, and so are the proof bytes; both verifiers reject them."""
+    import valida_b200 as vb
+
+    prog = lt_edge_operands_program() if name == "lt_edges" else loads_stores_edge_program()
+    t = vb.run_program(prog, initial_fp=0x1000)
+    ref = oracle.prove(t.main, t.preprocessed, debug_checks=True)
+    assert ref.constraint_failures()[0] >= 0 and ref.constraint_failures()[1:] == [-1] * 13
+    tr = ref.transcript()
+    pcs = vb.TwoAdicFriPcs(ctx)
+    for chip in range(14):
+        prep = t.preprocessed[0] if chip == 1 else t.preprocessed[1] if chip == 12 else None
+        perm, cs = vb.generate_permutation_trace(ctx, chip, ctx.upload(t.main[chip]), ctx.upload(prep) if prep is not None else None,
+                                                 tr["perm_challenges"])
+        assert np.array_equal(perm.download(), ref.perm_trace(chip)), chip
+        assert np.array_equal(cs, ref.cumulative_sum(chip)), chip
+        _, main_pd = pcs.commit_batches([t.main[chip]])
+        _, perm_pd = pcs.commit_batches([perm])
+        prep_lde = None
+        if prep is not None:
+            _, prep_pd = pcs.commit_batches([prep])
+            prep_lde = pcs.get_ldes(prep_pd)[0]
+        log_degree = t.main[chip].shape[0].bit_length() - 1
+        q = vb.quotient(ctx, chip, log_degree, prep_lde, pcs.get_ldes(main_pd)[0], pcs.get_ldes(perm_pd)[0], cs, tr["perm_challenges"], tr["alpha"])
+        assert np.array_equal(q.download(), ref.quotient_chunks(chip)), chip
+    proof = gpu_prove(ctx, oracle, t)
+    assert proof == ref.cbor()
+    assert oracle.verify(proof, t.preprocessed) != 0
+    with pytest.raises(vb.VerificationError):
+        vb.verify_machine(vb.StarkConfig(ctx, oracle.rc480), proof, t.preprocessed)
 
 
 def test_prove_mixed_chip_program(ctx, oracle):

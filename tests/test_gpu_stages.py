@@ -86,16 +86,28 @@ def test_quotient_chunks_bit_exact(ctx, oracle, fib, oracle_run, chip):
     assert np.array_equal(q.download(), oracle_run.quotient_chunks(chip))
 
 
-@pytest.mark.parametrize("chip", [0, 3, 4, 5, 7, 8, 9, 10, 11, 13])
+@pytest.mark.parametrize("chip", list(range(14)))
 def test_quotient_random_traces_exercise_every_constraint(ctx, oracle, chip):
     """On random (constraint-violating) traces every constraint contributes a non-zero term, so a wrong
-    column index, sign or constraint order anywhere in the device AIR shows up as a mismatch."""
+    column index, sign or constraint order anywhere in the device AIR shows up as a mismatch.  The program and range chips
+    read a random preprocessed matrix."""
+    quotient_random_traces(ctx, oracle, chip, 4, 40 + chip)
+
+
+@pytest.mark.parametrize("chip,log_degree", [(c, d) for c in range(14) for d in (0, 1)] + [(0, 15), (10, 15)])
+def test_quotient_random_traces_one_two_and_2p15_rows(ctx, oracle, chip, log_degree):
+    """The same at one row, two rows (first and last row coincide or are neighbours), and 2^15 rows, where the domain exponents
+    of the kernel reach the low half of the two-level root table."""
+    quotient_random_traces(ctx, oracle, chip, log_degree, 40 + 100 * log_degree + chip)
+
+
+def quotient_random_traces(ctx, oracle, chip, log_degree, seed):
     import valida_b200 as vb
 
-    rng = np.random.default_rng(40 + chip)
-    log_degree = 4
+    rng = np.random.default_rng(seed)
     h = 1 << log_degree
-    w, pwid = oracle.chip_width(chip), oracle.chip_perm_width(chip)
+    w, pwid, prw = oracle.chip_width(chip), oracle.chip_perm_width(chip), oracle.chip_prep_width(chip)
+    assert (prw > 0) == (chip in (1, 12))
     main = rng.integers(0, P, size=(h, w), dtype=np.uint32)
     perm = rng.integers(0, P, size=(h, pwid), dtype=np.uint32)
     ch = rng.integers(0, P, size=15, dtype=np.uint32)
@@ -105,8 +117,12 @@ def test_quotient_random_traces_exercise_every_constraint(ctx, oracle, chip):
     _, mpd = pcs.commit_batches([main])
     _, ppd = pcs.commit_batches([perm])
     ml, pl = pcs.get_ldes(mpd)[0], pcs.get_ldes(ppd)[0]
-    exp = oracle.quotient(chip, log_degree, None, ml.download(), pl.download(), cs, ch, alpha)
-    got = vb.quotient(ctx, chip, log_degree, None, ml, pl, cs, ch, alpha).download()
+    prl = None
+    if prw:
+        _, rpd = pcs.commit_batches([rng.integers(0, P, size=(h, prw), dtype=np.uint32)])
+        prl = pcs.get_ldes(rpd)[0]
+    exp = oracle.quotient(chip, log_degree, prl.download() if prw else None, ml.download(), pl.download(), cs, ch, alpha)
+    got = vb.quotient(ctx, chip, log_degree, prl, ml, pl, cs, ch, alpha).download()
     assert np.array_equal(got, exp)
 
 

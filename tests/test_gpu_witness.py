@@ -7,7 +7,8 @@ import os
 import numpy as np
 import pytest
 
-from programs import config5_program, mixed_program, static_data_program
+from programs import (config5_program, loads_stores_edge_program, lt_edge_operands_program, mixed_program,
+                      single_address_program, static_data_program)
 
 pytestmark = pytest.mark.gpu
 GOLDEN = json.load(open(os.path.join(os.path.dirname(os.path.abspath(__file__)), "golden", "programs.json")))
@@ -64,6 +65,22 @@ def test_memory_log_sort_with_wide_addresses(ctx):
         [8, 0, 0, 0, 0, 0],
     ], dtype=np.int32)
     _check(ctx, prog)
+
+
+def test_edge_operand_programs_witness(ctx):
+    """The programs built to reach the builders' edges: equal operands and a difference in the top byte only (the device's
+    lt_rows_kernel finds the first differing byte on its own), sign boundaries, immediates on both sides, negative immediates,
+    borrows, jal / jalv frame changes (the device's CPU diff_inv is a per-row Fermat inverse, the host's a table)."""
+    _check(ctx, lt_edge_operands_program())
+    _check(ctx, loads_stores_edge_program())
+
+
+def test_degenerate_memory_logs_witness(ctx):
+    """A lone STOP (an empty memory log) and a log whose every operation has the same address (the device radix sort has
+    nothing to order)."""
+    _check(ctx, np.array([[8, 0, 0, 0, 0, 0]], dtype=np.int32))
+    _check(ctx, single_address_program(1))
+    _check(ctx, single_address_program(40))
 
 
 def test_prove_from_device_witness(ctx, oracle):

@@ -20,6 +20,8 @@ and test_quotient_restatement.py are for the LogUp and quotient code.  No GPU.""
 import numpy as np
 import pytest
 
+from programs import loads_stores_edge_program, lt_edge_operands_program, single_address_program
+
 P = 2013265921
 LOAD32, STORE32, JAL, JALV, BEQ, BNE, IMM32, STOP, LOADFP, ADD32, SUB32 = 1, 2, 3, 4, 5, 6, 7, 8, 10, 100, 101
 LT32, AND32, OR32, XOR32, LTE32, SLT32, SLE32 = 104, 107, 108, 109, 115, 117, 118
@@ -386,30 +388,19 @@ def _ins(op, a=0, b=0, c=0, d=0, e=0):
 
 
 def test_loads_stores_loadfp_sub_and_signed_immediates(built):
-    # every instruction of the restated subset that the Fibonacci program does not reach: load32 / store32 through pointers,
-    # loadfp, sub32 with and without an immediate (incl. a NEGATIVE immediate: operand c is replaced by the reduced bytes of
-    # c as u32, cpu/src/lib.rs:364-371), bne on an immediate, a backwards jal with a frame change and back with jalv
-    prog = [
-        _ins(IMM32, -4, 0, 0, 1, 44),            # [fp-4] = 300
-        _ins(IMM32, -8, 0, 0, 0, 7),             # [fp-8] = 7
-        _ins(LOADFP, -12, -8),                   # [fp-12] = fp-8  (a pointer)
-        _ins(LOAD32, -16, 0, -12),               # [fp-16] = [[fp-12]] = 7
-        _ins(SUB32, -20, -4, -8),                # 300 - 7 = 293
-        _ins(SUB32, -24, -20, 38, 0, 1),         # 293 - 38 = 255 : borrow pattern in the low byte
-        _ins(ADD32, -28, -24, -1, 0, 1),         # 255 + 0xFFFFFFFF = 254 (wraps): immediate operand -1
-        _ins(LOADFP, -32, -36),                  # pointer to fp-36
-        _ins(STORE32, 0, -32, -28),              # [[fp-32]] = [fp-28] -> [fp-36] = 254
-        _ins(BNE, 12 * 24, -36, 254, 0, 1),      # equal: falls through
-        _ins(BEQ, 12 * 24, -36, -28),            # equal: taken, skips the next instruction
-        _ins(IMM32, -4, 9, 9, 9, 9),             # skipped
-        _ins(JAL, -40, 14 * 24, -64),            # call: return address at [fp-40], fp -= 64, to pc 14
-        _ins(STOP),
-        _ins(IMM32, 4, 0, 0, 0, 64),             # callee: [fp+4] = 64 (the frame offset back)
-        _ins(JALV, -4, 24, 4),                   # back to [fp+24] = [old fp-40] = 13*24, fp += [fp+4] = 64
-    ]
-    vm, got = check(np.array(prog, dtype=np.int32))
+    # every instruction of the restated subset that the Fibonacci program does not reach (tests/programs.py; the device witness
+    # and the GPU proof are checked on the same program in test_gpu_witness.py / test_gpu_prove.py)
+    vm, got = check(loads_stores_edge_program())
     assert vm.cells[(0x1000 - 36) & M32] == word(254) and vm.pc == 13 and vm.fp == 0x1000
     assert len(vm.subs) == 2 and len(vm.adds) == 1
+
+
+def test_degenerate_memory_logs(built):
+    # a lone STOP (no memory operation at all) and a log whose every operation is at one address
+    vm, got = check(np.array([_ins(STOP)], dtype=np.int32))
+    assert vm.clock == 1 and not vm.mem_ops
+    vm, got = check(single_address_program(5))
+    assert {addr for ops in vm.mem_ops.values() for _, addr, _ in ops} == {(0x1000 - 4) & M32}
 
 
 def test_the_references_other_test_programs_and_the_multi_chip_mixes(built):
@@ -437,22 +428,7 @@ def test_the_references_other_test_programs_and_the_multi_chip_mixes(built):
 def test_lt_family_edge_operands(built):
     # equal operands (no differing byte: flags, bits and diff_inv stay zero), operands that differ in the TOP byte only, sign
     # boundaries, both immediates at once (the recorded immediate is the right one, written through the LEFT-immediate path)
-    rows = []
-    vals = [0, 1, 0x7FFFFFFF, 0x80000000, 0xFFFFFFFF, 0x01000000, 0x00FFFFFF]
-    prog = []
-    for i, v in enumerate(vals):
-        w = word(v)
-        prog.append(_ins(IMM32, -4 * (i + 1), *w))
-    k = 0
-    for i in range(len(vals)):
-        for j in range(len(vals)):
-            op = (LT32, LTE32, SLT32, SLE32)[(i + j) % 4]
-            prog.append(_ins(op, -64 - 4 * (k % 8), -4 * (i + 1), -4 * (j + 1)))
-            k += 1
-    prog.append(_ins(SLT32, -100, -5, -4, 1, 0))            # left immediate -5 against [fp-4] = 0
-    prog.append(_ins(LTE32, -104, 7, 7, 1, 1))              # both immediates
-    prog.append(_ins(STOP))
-    vm, _ = check(np.array(prog, dtype=np.int32))
+    vm, _ = check(lt_edge_operands_program())
     assert u32(vm.cells[(0x1000 - 100) & M32]) == 1 and u32(vm.cells[(0x1000 - 104) & M32]) == 1
 
 
