@@ -145,6 +145,16 @@ int32_t vgpu_quotient(vgpu_ctx* ctx, const vgpu_chip_desc* chip, uint32_t log_de
                       const vgpu_dmat* main_lde, const vgpu_dmat* perm_lde, const uint32_t cumulative_sum[5],
                       const uint32_t perm_challenges[15], const uint32_t alpha[5], vgpu_dmat** out_chunks);
 
+/* ---- check_constraints (machine/src/check_constraints.rs:14-84; debug builds of the reference) ----
+ * Every constraint of the chip's Air::eval and of eval_permutation_constraints on every row i of the TRACE (with row (i+1) mod h),
+ * selectors is_first_row = [i == 0], is_last_row = [i == h-1], is_transition = 1 - is_last_row.  main / prep: as for vgpu_perm_trace;
+ * perm: the chip's flattened permutation trace (h x 5(k+1), as vgpu_perm_trace returns it); its last element is the cumulative sum.
+ * Writes the first failing row (-1: every constraint vanishes on every row), the index in eval order of the first constraint that does
+ * not vanish on it, and the number of rows with at least one failure.  Synchronises.  Whole matrices only (not row shards). */
+int32_t vgpu_check_constraints(vgpu_ctx* ctx, const vgpu_chip_desc* chip, const vgpu_dmat* main, const vgpu_dmat* prep_or_null,
+                               const vgpu_dmat* perm, const uint32_t challenges[15],
+                               int64_t* first_row, uint32_t* first_constraint, uint64_t* failing_rows);
+
 /* ---- Fiat-Shamir transcript owned by the context (DuplexChallenger; config.challenger() clone) ------
  * reset() restores the initial sponge of vgpu_set_challenger; values are canonical words. */
 int32_t vgpu_challenger_reset(vgpu_ctx* ctx);
@@ -167,6 +177,10 @@ int32_t vgpu_open(vgpu_ctx* ctx, const vgpu_prover_data* const* rounds, uint32_t
  * released with vgpu_free_bytes.  vgpu_set_challenger must have been called. */
 int32_t vgpu_prove(vgpu_ctx* ctx, const vgpu_matrix main[VGPU_NUM_CHIPS], const vgpu_matrix prep[2], int32_t repr,
                    uint8_t** proof_out, uint64_t* proof_len);
+/* Debug mode of vgpu_prove / vgpu_prove_device (off by default): after the permutation traces, check_constraints on every chip and
+ * check_cumulative_sums; on any failure the call returns an error naming every failing chip, its first row and constraint and its count
+ * of failing rows, and / or that the cumulative sums do not cancel, and writes no proof.  Refused on a context that splits proofs. */
+int32_t vgpu_ctx_set_debug_checks(vgpu_ctx* ctx, int32_t on);
 /* Same with the traces already resident in HBM (bench.py's device-resident timing). */
 int32_t vgpu_prove_device(vgpu_ctx* ctx, const vgpu_dmat* const main[VGPU_NUM_CHIPS], const vgpu_dmat* const prep[2],
                           uint8_t** proof_out, uint64_t* proof_len);

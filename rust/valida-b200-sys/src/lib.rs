@@ -121,6 +121,7 @@ extern "C" {
     pub fn vgpu_basic_machine_chip(chip_id: u32) -> *const vgpu_chip_desc;
     pub fn vgpu_perm_trace(ctx: *mut vgpu_ctx, chip: *const vgpu_chip_desc, main: *const vgpu_dmat, prep_or_null: *const vgpu_dmat, challenges: *const u32, out_perm: *mut *mut vgpu_dmat, cumulative_sum_out: *mut u32) -> i32;
     pub fn vgpu_quotient(ctx: *mut vgpu_ctx, chip: *const vgpu_chip_desc, log_degree: u32, prep_lde_or_null: *const vgpu_dmat, main_lde: *const vgpu_dmat, perm_lde: *const vgpu_dmat, cumulative_sum: *const u32, perm_challenges: *const u32, alpha: *const u32, out_chunks: *mut *mut vgpu_dmat) -> i32;
+    pub fn vgpu_check_constraints(ctx: *mut vgpu_ctx, chip: *const vgpu_chip_desc, main: *const vgpu_dmat, prep_or_null: *const vgpu_dmat, perm: *const vgpu_dmat, challenges: *const u32, first_row: *mut i64, first_constraint: *mut u32, failing_rows: *mut u64) -> i32;
 
     // ---- transcript ----
     pub fn vgpu_challenger_reset(ctx: *mut vgpu_ctx) -> i32;
@@ -132,6 +133,7 @@ extern "C" {
 
     // ---- Machine::prove ----
     pub fn vgpu_prove(ctx: *mut vgpu_ctx, main: *const vgpu_matrix, prep: *const vgpu_matrix, repr: i32, proof_out: *mut *mut u8, proof_len: *mut u64) -> i32;
+    pub fn vgpu_ctx_set_debug_checks(ctx: *mut vgpu_ctx, on: i32) -> i32;
     pub fn vgpu_prove_device(ctx: *mut vgpu_ctx, main: *const *const vgpu_dmat, prep: *const *const vgpu_dmat, proof_out: *mut *mut u8, proof_len: *mut u64) -> i32;
     pub fn vgpu_free_bytes(p: *mut u8);
     pub fn vgpu_last_prove_phases(ctx: *const vgpu_ctx, names: *mut *const c_char, ms: *mut f32, cap: u32) -> u32;

@@ -128,6 +128,13 @@ impl Context {
         self.check(unsafe { sys::vgpu_set_challenger(self.raw, round_constants.as_ptr(), mds_ptr) })
     }
 
+    /// Debug mode of [`Context::prove_bytes`] (off by default): every chip's constraints on every trace row and the cumulative sums
+    /// are checked before the commitments, as the reference's `prove` does in debug builds; a bad witness is an error naming each
+    /// failing chip, row and constraint.  `Machine::prove` passes `cfg!(debug_assertions)`.
+    pub fn set_debug_checks(&mut self, on: bool) -> Result<()> {
+        self.check(unsafe { sys::vgpu_ctx_set_debug_checks(self.raw, on as i32) })
+    }
+
     /// Page-locks a caller buffer in place so that the uploads of [`Context::prove_bytes`] overlap its commits.
     pub fn host_register(&mut self, words: &[u32]) -> Result<()> {
         self.check(unsafe { sys::vgpu_host_register(self.raw, words.as_ptr() as *const c_void, (words.len() * 4) as u64) })

@@ -21,6 +21,7 @@ from .api import (  # noqa: F401
     fib_program,
     generate_permutation_trace,
     quotient,
+    check_constraints,
     lib,
     lib_path,
     run_program,

@@ -64,6 +64,8 @@ def _load():
         "vgpu_basic_machine_chip": (vp, [C.c_uint32]),
         "vgpu_perm_trace": (C.c_int32, [vp, vp, vp, vp, u32p, C.POINTER(vp), u32p]),
         "vgpu_quotient": (C.c_int32, [vp, vp, C.c_uint32, vp, vp, vp, u32p, u32p, u32p, C.POINTER(vp)]),
+        "vgpu_check_constraints": (C.c_int32, [vp, vp, vp, vp, vp, u32p, C.POINTER(C.c_int64), u32p, C.POINTER(u64)]),
+        "vgpu_ctx_set_debug_checks": (C.c_int32, [vp, C.c_int32]),
         "vgpu_set_challenger": (C.c_int32, [vp, u32p, u32p]),
         "vgpu_challenger_reset": (C.c_int32, [vp]),
         "vgpu_challenger_observe": (C.c_int32, [vp, u32p, C.c_uint32]),
@@ -152,6 +154,11 @@ class Context:
 
     def set_kernel_timing(self, on):
         lib().vgpu_ctx_set_kernel_timing(self._h, 1 if on else 0)
+
+    def set_debug_checks(self, on):
+        """Debug mode of prove_machine (the reference's debug builds): check_constraints on every chip and the cumulative sums
+        before committing to a proof; a bad witness raises VgpuError naming each failing chip, row and constraint."""
+        self.check(lib().vgpu_ctx_set_debug_checks(self._h, 1 if on else 0))
 
     def kernel_stats(self):
         """[(kernel class, launches, total ms, algorithmic bytes)] since the last call (synchronises)."""
@@ -380,6 +387,16 @@ def quotient(ctx, chip_id, log_degree, prep_lde, main_lde, perm_lde, cumulative_
     ctx.check(lib().vgpu_quotient(ctx._h, chip, log_degree, prep_lde._h if prep_lde is not None else None, main_lde._h, perm_lde._h,
                                   _u32arr(cumulative_sum, 5), _u32arr(perm_challenges, 15), _u32arr(alpha, 5), C.byref(out)))
     return DeviceMatrix(ctx, out)
+
+
+def check_constraints(ctx, chip_id, main, prep, perm, perm_challenges):
+    """machine/src/check_constraints.rs:14-84 on whole device traces (perm: the flattened permutation trace) — returns
+    (first failing row or -1, index in eval order of its first failing constraint, number of rows with a failure)."""
+    chip = lib().vgpu_basic_machine_chip(chip_id)
+    row, con, n = C.c_int64(), C.c_uint32(), C.c_uint64()
+    ctx.check(lib().vgpu_check_constraints(ctx._h, chip, main._h, prep._h if prep is not None else None, perm._h,
+                                           _u32arr(perm_challenges, 15), C.byref(row), C.byref(con), C.byref(n)))
+    return int(row.value), int(con.value), int(n.value)
 
 
 class StarkConfig:

@@ -29,3 +29,7 @@ int32_t vg_ext_batch_inverse(vgpu_ctx* ctx, uint32_t* data, uint64_t cs, uint64_
 int32_t vg_perm_trace_enqueue(vgpu_ctx* ctx, const vgpu_chip_desc* chip, const vgpu_dmat* main, const vgpu_dmat* prep_or_null,
                               const uint32_t challenges[15], vgpu_dmat** out_perm, uint32_t* d_totals, uint32_t* n_totals);
 uint32_t vg_perm_totals_ranks(const vgpu_ctx* ctx);
+// check.cu — check_constraints of one chip on whole traces; d_first / d_count must hold ~0 / 0 before the sweep
+int32_t vg_check_enqueue(vgpu_ctx* ctx, const vgpu_chip_desc* chip, const vgpu_dmat* main, const vgpu_dmat* prep_or_null, const vgpu_dmat* perm,
+                         const uint32_t challenges[15], unsigned long long* d_first, unsigned long long* d_count);
+void vg_check_decode(const unsigned long long first_count[2], int64_t* row, uint32_t* constraint, uint64_t* failing_rows);

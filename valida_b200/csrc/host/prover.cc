@@ -383,6 +383,40 @@ struct PdGuard { vgpu_prover_data* p = nullptr; ~PdGuard() { if (p) vgpu_prover_
 struct BufGuard { vgpu_ctx* ctx; void* p = nullptr; explicit BufGuard(vgpu_ctx* c) : ctx(c) {} ~BufGuard() { vg_free(ctx, p); } };
 struct MatGuard { std::vector<vgpu_dmat*> v; ~MatGuard() { for (auto* m : v) vgpu_dmat_free(m); } };
 
+// The debug mode checks whole traces; a split proof holds row shards, whose last row's "next" row lives on another rank.  Every rank
+// refuses alike, before any collective.
+int32_t debug_mode_allowed(vgpu_ctx* ctx) {
+    if (ctx->debug_checks && vg_sharded(ctx))
+        VG_FAIL(ctx, "prove: the debug checks run on whole traces only; turn them off or call vgpu_comm_set_sharding(ctx, 0)");
+    return 0;
+}
+
+// check_constraints of every chip (first keys [14], then failing-row counts [14]) and check_cumulative_sums
+// (machine/src/check_constraints.rs:87-93): an error naming every failure, or 0.
+int32_t debug_verdict(vgpu_ctx* ctx, const unsigned long long* chk, const uint32_t cumsum[VGPU_NUM_CHIPS][5]) {
+    static const char* NAMES[VGPU_NUM_CHIPS] = {"cpu", "program", "mem", "add", "sub", "mul", "div", "shift", "lt", "com", "bitwise", "output", "range", "static_data"};
+    std::string msg;
+    for (int i = 0; i < VGPU_NUM_CHIPS; i++) {
+        const unsigned long long fc[2] = {chk[i], chk[VGPU_NUM_CHIPS + i]};
+        int64_t row; uint32_t c; uint64_t n;
+        vg_check_decode(fc, &row, &c, &n);
+        if (row < 0) continue;
+        char b[160];
+        snprintf(b, sizeof b, "chip %d (%s): constraint %u does not vanish on row %lld (%llu rows fail)", i, NAMES[i], c, (long long)row, (unsigned long long)n);
+        msg += (msg.empty() ? "" : "; ") + std::string(b);
+    }
+    bool cancel = true;
+    for (int l = 0; l < 5; l++) {
+        uint64_t s = 0;
+        for (int i = 0; i < VGPU_NUM_CHIPS; i++) s += cumsum[i][l];
+        cancel = cancel && s % bb::P == 0;
+    }
+    if (!cancel) msg += (msg.empty() ? "" : "; ") + std::string("cumulative sums do not cancel");
+    if (msg.empty()) return 0;
+    ctx->err = "prove: debug checks failed: " + msg;
+    return -1;
+}
+
 }  // namespace
 
 void vg_host_state_free(vgpu_ctx* ctx) {
@@ -455,6 +489,9 @@ int32_t vgpu_open(vgpu_ctx* ctx, const vgpu_prover_data* const* rounds, uint32_t
 // (memory chip 2^26 rows, LDE 2^27) be proven on one GPU.
 static int32_t prove_device(vgpu_ctx* ctx, const vgpu_dmat* const main[VGPU_NUM_CHIPS], const vgpu_dmat* const prep[2],
                             vgpu_dmat* const* owned_main, uint8_t** proof_out, uint64_t* proof_len) {
+    VG_TRY(debug_mode_allowed(ctx));
+    const bool debug = ctx->debug_checks;
+    auto prep_for = [&](int i) -> const vgpu_dmat* { return i == 1 ? prep[0] : i == 12 ? prep[1] : nullptr; };
     if (!ctx->challenger_set) VG_FAIL(ctx, "prove: vgpu_set_challenger has not been called");
     if (!proof_out || !proof_len) VG_FAIL(ctx, "prove: null output");
     VG_TRY(vg_enter(ctx));
@@ -505,17 +542,26 @@ static int32_t prove_device(vgpu_ctx* ctx, const vgpu_dmat* const main[VGPU_NUM_
         {
             Phase ph(ctx, "permutation traces");
             // the cumulative sums of all chips come back with ONE copy: per chip the per-rank sums of its running sum
+            // (debug mode: the check results of the 14 chips, first keys then failing-row counts, ride in the same buffer and copy)
             const uint32_t slots = vg_perm_totals_ranks(ctx);
+            const size_t tot_words = (size_t)VGPU_NUM_CHIPS * slots * 5, chk_words = debug ? 4 * VGPU_NUM_CHIPS : 0;
             BufGuard tot(ctx);
-            VG_TRY(vg_alloc(ctx, (void**)&tot.p, (size_t)VGPU_NUM_CHIPS * slots * 5 * 4));
+            VG_TRY(vg_alloc(ctx, (void**)&tot.p, (tot_words + chk_words) * 4));
             uint32_t nt[VGPU_NUM_CHIPS];
             for (int i = 0; i < VGPU_NUM_CHIPS; i++) {
-                const vgpu_dmat* p = i == 1 ? prep[0] : i == 12 ? prep[1] : nullptr;
                 vgpu_dmat* pm = nullptr;
-                VG_TRY(vg_perm_trace_enqueue(ctx, chips[i], main[i], p, perm_challenges, &pm, (uint32_t*)tot.p + (size_t)i * slots * 5, &nt[i]));
+                VG_TRY(vg_perm_trace_enqueue(ctx, chips[i], main[i], prep_for(i), perm_challenges, &pm, (uint32_t*)tot.p + (size_t)i * slots * 5, &nt[i]));
                 perms.v.push_back(pm);
             }
-            std::vector<uint32_t> ht((size_t)VGPU_NUM_CHIPS * slots * 5);
+            if (debug) {   // check_constraints (derive/src/lib.rs:246-253) while the main traces are still held
+                Phase pc(ctx, "check constraints");
+                unsigned long long* d_chk = (unsigned long long*)((uint32_t*)tot.p + tot_words);   // tot_words is even: 8-byte aligned
+                VG_CUDA(ctx, cudaMemsetAsync(d_chk, 0xff, VGPU_NUM_CHIPS * 8, ctx->stream));
+                VG_CUDA(ctx, cudaMemsetAsync(d_chk + VGPU_NUM_CHIPS, 0, VGPU_NUM_CHIPS * 8, ctx->stream));
+                for (int i = 0; i < VGPU_NUM_CHIPS; i++)
+                    VG_TRY(vg_check_enqueue(ctx, chips[i], main[i], prep_for(i), perms.v[i], perm_challenges, d_chk + i, d_chk + VGPU_NUM_CHIPS + i));
+            }
+            std::vector<uint32_t> ht(tot_words + chk_words);
             VG_CUDA(ctx, cudaMemcpyAsync(ht.data(), tot.p, ht.size() * 4, cudaMemcpyDeviceToHost, ctx->stream));
             VG_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
             for (int i = 0; i < VGPU_NUM_CHIPS; i++)
@@ -524,6 +570,7 @@ static int32_t prove_device(vgpu_ctx* ctx, const vgpu_dmat* const main[VGPU_NUM_
                     for (uint32_t r = 0; r < nt[i]; r++) a = bb::add(a, ht[((size_t)i * slots + r) * 5 + l]);
                     cumsum[i][l] = bb::from_monty(a);
                 }
+            if (debug) VG_TRY(debug_verdict(ctx, (const unsigned long long*)(ht.data() + tot_words), cumsum));
             // later work reuses the released blocks in stream order, i.e. after the permutation kernels that read them
             for (int i = 0; owned_main && i < VGPU_NUM_CHIPS; i++) {
                 vgpu_dmat* m = owned_main[i];
@@ -617,6 +664,7 @@ int32_t vgpu_prove(vgpu_ctx* ctx, const vgpu_matrix main[VGPU_NUM_CHIPS], const 
     // only when a tree layer of their height is reached), each transpose is deferred to the matrix's first use, so
     // copies of later matrices overlap the LDE / Keccak kernels of earlier ones.
     // Split proof: of a trace tall enough to be split a rank uploads ITS run of rows only (1 / comm_size of the bytes).
+    VG_TRY(debug_mode_allowed(ctx));
     VG_TRY(vg_enter(ctx));
     MatGuard dm, dp;
     phases_reset(ctx);
@@ -644,6 +692,8 @@ int32_t vgpu_prove(vgpu_ctx* ctx, const vgpu_matrix main[VGPU_NUM_CHIPS], const 
     if (rc == 0) rc = vg_stager_finish(ctx);
     return rc;
 }
+
+int32_t vgpu_ctx_set_debug_checks(vgpu_ctx* ctx, int32_t on) { ctx->debug_checks = on != 0; return 0; }
 
 void vgpu_free_bytes(uint8_t* p) { std::free(p); }
 

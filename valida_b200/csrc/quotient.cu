@@ -22,6 +22,7 @@
 #include "ctx.h"
 #include "devchip.h"
 #include "airs.cuh"
+#include "logup.cuh"
 #include <cstring>
 #include <cstdlib>
 #include <memory>
@@ -73,21 +74,6 @@ __device__ __forceinline__ uint32_t qroot_pow(const QParams& p, uint64_t e) {
     e &= ((1ull << VG_LOG_NMAX) - 1);
     return bb::mul(__ldg(p.root_lo + (e & (VG_POW_LO - 1))), __ldg(p.root_hi + (e >> VG_POW_LO_BITS)));
 }
-__device__ __forceinline__ uint32_t dev_pair_col(const DevPairCol& pc, const uint32_t* mrow, uint64_t mcs, const uint32_t* prow, uint64_t pcs) {
-    uint32_t v = pc.constant;
-    for (uint32_t t = 0; t < pc.n_terms; t++) {
-        uint32_t x = pc.is_prep[t] ? __ldg(prow + (uint64_t)pc.column[t] * pcs) : __ldg(mrow + (uint64_t)pc.column[t] * mcs);
-        v = bb::add(v, bb::mul(x, pc.weight[t]));
-    }
-    return v;
-}
-__device__ __forceinline__ E5 load_e5(const uint32_t* row, uint64_t cs, uint32_t m) {
-    E5 r;
-#pragma unroll
-    for (int l = 0; l < 5; l++) r.c[l] = __ldg(row + (uint64_t)(5 * m + l) * cs);
-    return r;
-}
-
 // MINB: resident-CTA target (register cap) of the variant.  The sweep is latency bound (ncu r1b: issue slots 43-57 % busy at
 // 5 CTAs per SM), so more resident warps beat fewer spills: measured 11.4 / 8.9 / 8.6 ms per proof at 2-4 / 6 / 8 CTAs per SM.
 template <int CHIP, int MINB>
@@ -118,7 +104,6 @@ __global__ void __launch_bounds__(128, MINB) quotient_kernel(const __grid_consta
         inv_last = e ? bb::mul(i23, d2) : bb::mul(i01, d0);
     }
     const DevChip& chip = p.chip;
-    const uint32_t k = chip.n_interactions;
     const uint32_t parity = (uint32_t)(((uint64_t)j + (e ? h : 0)) & 1);
     const uint32_t zh = p.zh[parity];
     DevBuilder b;
@@ -128,27 +113,8 @@ __global__ void __launch_bounds__(128, MINB) quotient_kernel(const __grid_consta
     b.trans = F{bb::sub(x, p.glast)};
     b.apow = p.apow; b.idx = 0; b.acc.init();
     air::eval_chip<CHIP>(b);
-    {   // eval_permutation_constraints
-        const uint32_t* ql = p.perm + rho; const uint32_t* qn = p.perm_n + nrow;
-        const uint32_t* pl = p.prep ? p.prep + rho : nullptr; const uint32_t* pn = p.prep ? p.prep_n + nrow : nullptr;
-        const E5 phi_local = load_e5(ql, p.qcs, k), phi_next = load_e5(qn, p.qcs, k);
-        E5 rhs = bb::e5_zero(), phi0 = bb::e5_zero();
-        for (uint32_t m = 0; m < k; m++) {
-            const DevInteraction& it = chip.interactions[m];
-            bb::Lazy5 ra; ra.init();
-            for (uint32_t f = 0; f < it.n_fields; f++) ra.fma_base(chip.betas[f], dev_pair_col(it.fields[f], b.lrow, p.mcs, pl, p.pcs));
-            const E5 rlc = bb::e5_add(it.alpha, ra.value());
-            const E5 pm_l = load_e5(ql, p.qcs, m), pm_n = load_e5(qn, p.qcs, m);
-            b.z_ext(bb::e5_sub_base(bb::e5_mul(rlc, pm_l), bb::R1));
-            const uint32_t mult_l = dev_pair_col(it.count, b.lrow, p.mcs, pl, p.pcs), mult_n = dev_pair_col(it.count, b.nrow, p.mcs, pn, p.pcs);
-            const E5 tl = bb::e5_mul_base(pm_l, mult_l), tn = bb::e5_mul_base(pm_n, mult_n);
-            if (it.is_send) { phi0 = bb::e5_add(phi0, tl); rhs = bb::e5_add(rhs, tn); }
-            else { phi0 = bb::e5_sub(phi0, tl); rhs = bb::e5_sub(rhs, tn); }
-        }
-        b.z_ext(bb::e5_mul_base(bb::e5_sub(bb::e5_sub(phi_next, phi_local), rhs), b.trans.v));
-        b.z_ext(bb::e5_mul_base(bb::e5_sub(phi_local, phi0), b.first.v));
-        b.z_ext(bb::e5_mul_base(bb::e5_sub(phi_local, p.cumsum), b.last.v));
-    }
+    logup::eval_constraints(b, chip, b.lrow, b.nrow, p.mcs, p.prep ? p.prep + rho : nullptr, p.prep ? p.prep_n + nrow : nullptr, p.pcs,
+                            p.perm + rho, p.perm_n + nrow, p.qcs, p.cumsum);
     const E5 q = bb::e5_mul_base(b.acc.value(), p.zinv[parity]);
     // decompose_and_flatten across the lane pair: even = (q(x) + q(-x))/2, odd = (q(x) - q(-x)) / (2 s g^j)
     E5 other;
