@@ -77,6 +77,36 @@ __global__ void __launch_bounds__(128) leaf_hash_kernel(const uint32_t* const* _
     o[1] = make_uint4(wrap_mod_p(d[4]), wrap_mod_p(d[5]), wrap_mod_p(d[6]), wrap_mod_p(d[7]));
 }
 
+// Rows of at most LEAF_NB_MAX sponge blocks (nwords / RATE_WORDS + 1 blocks with the padding: up to 67 words) take
+// leaf_hash_kernel_blocks<NB>, whose absorption is unrolled for exactly NB blocks: the slots of every block but the last are all
+// row words, the first block runs the round-0-peeled permutation (its capacity lanes are zero) and the last the round-23-peeled
+// one, and the column pointers come from the kernel's parameter space rather than a table in global memory.
+constexpr int LEAF_NB_MAX = 2;
+struct LeafCols { const uint32_t* col[LEAF_NB_MAX * RATE_WORDS]; };
+template <int NB>
+__global__ void __launch_bounds__(128) leaf_hash_kernel_blocks(const __grid_constant__ LeafCols c, uint32_t nwords, uint64_t row0, uint64_t nrows, uint32_t* __restrict__ digests) {
+    uint64_t r = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
+    if (r >= nrows) return;
+    r += row0;
+    uint2 A[25];
+#pragma unroll
+    for (int i = 0; i < 25; i++) A[i] = make_uint2(0, 0);
+#pragma unroll
+    for (int b = 0; b < NB; b++) {
+#pragma unroll
+        for (int i = 0; i < RATE_WORDS; i++) {
+            const uint32_t g = b * RATE_WORDS + i;
+            uint32_t w = (b < NB - 1 || g < nwords) ? bb::from_monty(__ldg(c.col[g] + r)) : (g == nwords ? 1u : 0u);
+            if (b == NB - 1 && i == RATE_WORDS - 1) w ^= 0x80000000u;
+            if (i & 1) A[i / 2].y ^= w; else A[i / 2].x ^= w;
+        }
+        if (b == 0) kk::keccak_f_peeled<true, NB == 1>(A); else kk::keccak_f_peeled<false, true>(A);
+    }
+    uint4* o = reinterpret_cast<uint4*>(digests + r * 8);
+    o[0] = make_uint4(wrap_mod_p(A[0].x), wrap_mod_p(A[0].y), wrap_mod_p(A[1].x), wrap_mod_p(A[1].y));
+    o[1] = make_uint4(wrap_mod_p(A[2].x), wrap_mod_p(A[2].y), wrap_mod_p(A[3].x), wrap_mod_p(A[3].y));
+}
+
 __device__ __forceinline__ void compress_pair(const uint32_t l[8], const uint32_t r[8], uint32_t out[8]) {
     uint32_t d[8];
     keccak256_words<true>(16, [&](uint32_t i) { return i < 8 ? l[i] : r[i - 8]; }, d);
@@ -180,44 +210,51 @@ __global__ void __maxnreg__(80) tree_tail_kernel(const __grid_constant__ TailPar
         for (uint32_t i = threadIdx.x; i < 4 * p.sub; i += TAIL_THREADS) buf_a[i] = __ldg(src + i);
     }
     __syncthreads();
-    WarpKeccak wk;
-    wk.init(threadIdx.x & 31);
     uint4* cur = buf_a; uint4* nxt = buf_b;
-    for (uint32_t k = 0; k < p.levels; k++) {
+    // n halves every level, so the wide levels all come first.  Two loops rather than one branch: the WarpKeccak set-up is then
+    // not live across the thread-per-node rounds, which fit in 80 registers only without it.
+    uint32_t k = 0;
+    for (; k < p.levels && (p.sub >> k) > TAIL_WARP_NODES; k++) {      // a thread per node
         const uint32_t n = p.sub >> k;
         const uint64_t base = node0 >> k;
-        if (n > TAIL_WARP_NODES) {
-            for (uint32_t t = threadIdx.x; t < n; t += TAIL_THREADS) {
-                const uint4 a = cur[4 * t], b = cur[4 * t + 1], c = cur[4 * t + 2], d = cur[4 * t + 3];
-                uint32_t l[8] = {a.x, a.y, a.z, a.w, b.x, b.y, b.z, b.w}, r[8] = {c.x, c.y, c.z, c.w, d.x, d.y, d.z, d.w}, o[8];
-                compress_pair(l, r, o);
-                if (p.inj_v[k]) {
-                    const uint4* q = reinterpret_cast<const uint4*>(p.inj_v[k] + (base + t) * 8);
-                    const uint4 e = __ldg(q), f = __ldg(q + 1);
-                    uint32_t tt[8] = {e.x, e.y, e.z, e.w, f.x, f.y, f.z, f.w}, o2[8];
-                    compress_pair(o, tt, o2);
+        for (uint32_t t = threadIdx.x; t < n; t += TAIL_THREADS) {
+            const uint4 a = cur[4 * t], b = cur[4 * t + 1], c = cur[4 * t + 2], d = cur[4 * t + 3];
+            uint32_t l[8] = {a.x, a.y, a.z, a.w, b.x, b.y, b.z, b.w}, r[8] = {c.x, c.y, c.z, c.w, d.x, d.y, d.z, d.w}, o[8];
+            compress_pair(l, r, o);
+            if (p.inj_v[k]) {
+                const uint4* q = reinterpret_cast<const uint4*>(p.inj_v[k] + (base + t) * 8);
+                const uint4 e = __ldg(q), f = __ldg(q + 1);
+                uint32_t tt[8] = {e.x, e.y, e.z, e.w, f.x, f.y, f.z, f.w}, o2[8];
+                compress_pair(o, tt, o2);
 #pragma unroll
-                    for (int i = 0; i < 8; i++) o[i] = o2[i];
-                }
-                const uint4 w0 = make_uint4(o[0], o[1], o[2], o[3]), w1 = make_uint4(o[4], o[5], o[6], o[7]);
-                nxt[2 * t] = w0; nxt[2 * t + 1] = w1;
-                uint4* g = reinterpret_cast<uint4*>(p.next_v[k] + (base + t) * 8);
-                g[0] = w0; g[1] = w1;
+                for (int i = 0; i < 8; i++) o[i] = o2[i];
             }
-        } else {
-            const uint32_t lane = threadIdx.x & 31;
-            for (uint32_t t = threadIdx.x >> 5; t < n; t += TAIL_THREADS / 32) {      // a warp per node
-                const uint2* in = reinterpret_cast<const uint2*>(cur + 4 * t);         // 16 words = 8 uint2
-                uint2 dg = wk.compress(lane < 8 ? in[lane] : make_uint2(0, 0));        // lanes 0..3: the digest
-                if (p.inj_v[k]) {
-                    const uint2* q = reinterpret_cast<const uint2*>(p.inj_v[k] + (base + t) * 8);
-                    const uint2 w = lane < 4 ? dg : (lane < 8 ? __ldg(q + (lane - 4)) : make_uint2(0, 0));
-                    dg = wk.compress(w);
-                }
-                if (lane < 4) {
-                    reinterpret_cast<uint2*>(nxt + 2 * t)[lane] = dg;
-                    reinterpret_cast<uint2*>(p.next_v[k] + (base + t) * 8)[lane] = dg;
-                }
+            const uint4 w0 = make_uint4(o[0], o[1], o[2], o[3]), w1 = make_uint4(o[4], o[5], o[6], o[7]);
+            nxt[2 * t] = w0; nxt[2 * t + 1] = w1;
+            uint4* g = reinterpret_cast<uint4*>(p.next_v[k] + (base + t) * 8);
+            g[0] = w0; g[1] = w1;
+        }
+        __syncthreads();
+        uint4* tmp = cur; cur = nxt; nxt = tmp;
+    }
+    if (k == p.levels) return;
+    const uint32_t lane = threadIdx.x & 31;
+    WarpKeccak wk;
+    wk.init(lane);
+    for (; k < p.levels; k++) {      // a warp per node
+        const uint32_t n = p.sub >> k;
+        const uint64_t base = node0 >> k;
+        for (uint32_t t = threadIdx.x >> 5; t < n; t += TAIL_THREADS / 32) {
+            const uint2* in = reinterpret_cast<const uint2*>(cur + 4 * t);         // 16 words = 8 uint2
+            uint2 dg = wk.compress(lane < 8 ? in[lane] : make_uint2(0, 0));        // lanes 0..3: the digest
+            if (p.inj_v[k]) {
+                const uint2* q = reinterpret_cast<const uint2*>(p.inj_v[k] + (base + t) * 8);
+                const uint2 w = lane < 4 ? dg : (lane < 8 ? __ldg(q + (lane - 4)) : make_uint2(0, 0));
+                dg = wk.compress(w);
+            }
+            if (lane < 4) {
+                reinterpret_cast<uint2*>(nxt + 2 * t)[lane] = dg;
+                reinterpret_cast<uint2*>(p.next_v[k] + (base + t) * 8)[lane] = dg;
             }
         }
         __syncthreads();
@@ -282,13 +319,25 @@ static int32_t hash_rows(vgpu_ctx* ctx, const std::vector<const vgpu_dmat*>& mat
         if (m->dist == VG_ROWS && (row0 < m->row0 || row0 + nrows > m->row0 + m->h)) VG_FAIL(ctx, "commit: rows [%llu, +%llu) are not in this rank's shard", (unsigned long long)row0, (unsigned long long)nrows);
         for (uint64_t c = 0; c < m->w; c++) cols.push_back(m->d + c * m->col_stride - m->row0);
     }
+    const uint32_t nwords = (uint32_t)cols.size(), nblocks = nwords / RATE_WORDS + 1, grid = (uint32_t)((nrows + 127) / 128);
+    if (nblocks <= LEAF_NB_MAX) {
+        LeafCols lc{};
+        std::copy(cols.begin(), cols.end(), lc.col);
+        {
+            KScope ks(ctx, KC_LEAF_HASH, (double)nrows * (4.0 * nwords + 32.0));
+            if (nblocks == 1) leaf_hash_kernel_blocks<1><<<grid, 128, 0, ctx->stream>>>(lc, nwords, row0, nrows, digests_v);
+            else leaf_hash_kernel_blocks<2><<<grid, 128, 0, ctx->stream>>>(lc, nwords, row0, nrows, digests_v);
+        }
+        VG_LAUNCH_CHECK(ctx);
+        return 0;
+    }
     const uint32_t** dcols = nullptr;
     VG_TRY(vg_alloc(ctx, (void**)&dcols, cols.size() * sizeof(void*)));
     // cudaMemcpyAsync from pageable memory stages synchronously: `cols` may go once the call returns
     VG_CUDA(ctx, cudaMemcpyAsync(dcols, cols.data(), cols.size() * sizeof(void*), cudaMemcpyHostToDevice, ctx->stream));
     {
-        KScope ks(ctx, KC_LEAF_HASH, (double)nrows * (4.0 * cols.size() + 32.0));
-        leaf_hash_kernel<<<(unsigned)((nrows + 127) / 128), 128, 0, ctx->stream>>>(dcols, (uint32_t)cols.size(), row0, nrows, digests_v);
+        KScope ks(ctx, KC_LEAF_HASH, (double)nrows * (4.0 * nwords + 32.0));
+        leaf_hash_kernel<<<grid, 128, 0, ctx->stream>>>(dcols, nwords, row0, nrows, digests_v);
     }
     VG_LAUNCH_CHECK(ctx);
     vg_free(ctx, dcols);
