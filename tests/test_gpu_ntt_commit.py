@@ -10,7 +10,7 @@ def rand_mat(rng, h, w):
     return rng.integers(0, P, size=(h, w), dtype=np.uint32)
 
 
-@pytest.mark.parametrize("log_h,w", [(0, 1), (1, 3), (2, 2), (5, 7), (8, 51), (10, 16), (12, 5), (13, 3), (14, 2), (16, 4), (17, 3), (18, 2), (22, 2), (23, 1)])
+@pytest.mark.parametrize("log_h,w", [(0, 1), (1, 3), (2, 2), (5, 7), (8, 51), (10, 16), (12, 5), (13, 3), (14, 2), (15, 3), (16, 4), (17, 3), (18, 2), (19, 2), (21, 2), (22, 2), (23, 1), (24, 1)])
 def test_ntt_forward_inverse_bit_exact(ctx, oracle, log_h, w):
     import valida_b200 as vb
 
@@ -45,7 +45,7 @@ def test_ntt_monty_repr_and_host_entry(ctx, oracle):
     assert np.array_equal(buf, oracle.dft(m))
 
 
-@pytest.mark.parametrize("log_h,w,shift", [(0, 2, 31), (1, 1, 31), (3, 4, 31), (9, 14, 31), (12, 3, 31), (13, 5, 31), (15, 2, 7), (16, 2, pow(31, P - 2, P)), (18, 3, 31), (20, 2, 31), (22, 2, 31), (23, 1, 961)])
+@pytest.mark.parametrize("log_h,w,shift", [(0, 2, 31), (1, 1, 31), (3, 4, 31), (9, 14, 31), (12, 3, 31), (13, 5, 31), (15, 2, 7), (16, 2, pow(31, P - 2, P)), (17, 2, 31), (18, 3, 31), (19, 2, 31), (20, 2, 31), (21, 2, 31), (22, 2, 31), (23, 1, 961), (24, 1, 31)])
 def test_coset_lde_bit_exact(ctx, oracle, log_h, w, shift):
     import valida_b200 as vb
 
@@ -158,7 +158,7 @@ def test_coset_lde_larger_blowups_natural_order(ctx, oracle):
     rng = np.random.default_rng(77)
     x = rng.integers(0, P, (1 << 9, 3), dtype=np.uint32)
     dft = vb.Radix2Dft(ctx)
-    for added_bits in (2, 3):
+    for added_bits in (1, 2, 3, 4):
         got = dft.coset_lde_batch(ctx.upload(x), added_bits, 31).download()
         assert np.array_equal(got, oracle.coset_lde(x, added_bits, 31, False))
     with pytest.raises(vb.VgpuError, match="log_blowup = 1 only"):

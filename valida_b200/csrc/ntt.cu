@@ -582,8 +582,7 @@ __global__ void zero_pad_kernel(const uint32_t* src, uint64_t src_cs, uint32_t* 
 // split for the passes that have one strided and one contiguous sub-transform
 void split_col_row(int log_n, int* l_col, int* l_row) {
     if (log_n <= LOG_ROW_MAX) { *l_col = 0; *l_row = log_n; return; }
-    static const int row_split = [] { const char* e = getenv("VGPU_NTT_LOG_ROW"); int v = e ? atoi(e) : LOG_ROW_MAX; return v < 8 || v > LOG_ROW_MAX ? LOG_ROW_MAX : v; }();   // tuning knob (profiles/)
-    int lc = log_n - row_split;
+    int lc = log_n - LOG_ROW_MAX;
     if (lc > LOG_COL_MAX) lc = LOG_COL_MAX;          // then the contiguous part takes the rest (<= LOG_ROW_MAX for log_n <= 26)
     if (lc < 4) lc = 4;
     *l_col = lc; *l_row = log_n - lc;
@@ -713,8 +712,9 @@ int32_t vg_coset_lde(vgpu_ctx* ctx, const uint32_t* src, uint64_t src_cs, uint64
     int log_n = 0;
     while ((1ull << log_n) < h) log_n++;
     if ((1ull << log_n) != h) VG_FAIL(ctx, "coset_lde: height %llu is not a power of two", (unsigned long long)h);
-    if (log_n + (int)log_blowup > VG_LOG_NMAX) VG_FAIL(ctx, "coset_lde: LDE height 2^%d exceeds BabyBear two-adicity", log_n + (int)log_blowup);
+    // the height limit first: with log_blowup >= 1 the two-adicity check below would otherwise shadow it
     if (log_n > LOG_ROW_MAX + LOG_COL_MAX) VG_FAIL(ctx, "coset_lde: heights above 2^%d are not built", LOG_ROW_MAX + LOG_COL_MAX);
+    if (log_n + (int)log_blowup > VG_LOG_NMAX) VG_FAIL(ctx, "coset_lde: LDE height 2^%d exceeds BabyBear two-adicity", log_n + (int)log_blowup);
     if (h == 1) {
         const uint64_t H = 1ull << log_blowup;
         repeat_row_kernel<<<(unsigned)((H * w + 127) / 128), 128, 0, ctx->stream>>>(src, src_cs, dst, dst_cs, H, w);
