@@ -11,6 +11,8 @@
 // Sources: cpu/src/stark.rs:22-305, alu_u32/src/{add,sub,mul,shift,lt,com,bitwise}/stark.rs,
 // output/src/stark.rs:21-39, static_data/src/stark.rs:25-37; memory/range/program/div are empty.
 #pragma once
+#include <type_traits>
+#include "../../include/valida_b200.h"
 #include "bb.cuh"
 
 namespace air {
@@ -311,6 +313,15 @@ template <int CHIP, class B> BB_HD void eval_chip(B& b) {
     else if (CHIP == 11) eval_output(b);
     else if (CHIP == 13) eval_static_data(b);
     // 1 program, 2 memory, 6 div, 12 range: empty eval
+}
+
+// f(std::integral_constant<int, CHIP>{}) for CHIP == chip_id: the per-chip instantiation behind a run-time chip id
+// (ids >= VGPU_NUM_CHIPS call nothing)
+template <int CHIP = 0, class Fn> void with_chip(uint32_t chip_id, Fn&& f) {
+    if constexpr (CHIP < VGPU_NUM_CHIPS) {
+        if (chip_id == CHIP) f(std::integral_constant<int, CHIP>{});
+        else with_chip<CHIP + 1>(chip_id, f);
+    }
 }
 
 }  // namespace air

@@ -72,10 +72,6 @@ __global__ void __launch_bounds__(128) check_kernel(const __grid_constant__ CPar
     }
 }
 
-template <int CHIP> void launch(const CParams& p, cudaStream_t st) {
-    check_kernel<CHIP><<<(unsigned)((p.h + 127) / 128), 128, 0, st>>>(p);
-}
-
 }  // namespace
 
 // Validates the arguments (before anything is enqueued) and enqueues the sweep of one chip.  d_first / d_count must hold ~0 / 0.
@@ -107,15 +103,7 @@ int32_t vg_check_enqueue(vgpu_ctx* ctx, const vgpu_chip_desc* chip, const vgpu_d
     p.perm = perm->d; p.qcs = perm->col_stride;
     p.h = h; p.first = d_first; p.count = d_count;
     KScope ks(ctx, KC_CHECK, 4.0 * (double)h * (double)(main->gw + perm->gw + (prep ? prep->gw : 0)));
-    switch (chip->chip_id) {
-        case 0: launch<0>(p, ctx->stream); break;   case 1: launch<1>(p, ctx->stream); break;
-        case 2: launch<2>(p, ctx->stream); break;   case 3: launch<3>(p, ctx->stream); break;
-        case 4: launch<4>(p, ctx->stream); break;   case 5: launch<5>(p, ctx->stream); break;
-        case 6: launch<6>(p, ctx->stream); break;   case 7: launch<7>(p, ctx->stream); break;
-        case 8: launch<8>(p, ctx->stream); break;   case 9: launch<9>(p, ctx->stream); break;
-        case 10: launch<10>(p, ctx->stream); break; case 11: launch<11>(p, ctx->stream); break;
-        case 12: launch<12>(p, ctx->stream); break; case 13: launch<13>(p, ctx->stream); break;
-    }
+    air::with_chip(chip->chip_id, [&](auto c) { check_kernel<decltype(c)::value><<<(unsigned)((h + 127) / 128), 128, 0, ctx->stream>>>(p); });
     VG_LAUNCH_CHECK(ctx);
     return 0;
 }

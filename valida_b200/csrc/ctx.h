@@ -20,6 +20,10 @@ struct PowTable {            // device tables of Montgomery words
     uint32_t hi_len = 0;
     uint32_t base = 0;       // the base itself (Montgomery), without the scale
 };
+// base^e (times the scale) from a PowTable's lo / hi tables, e < 4096 * hi_len
+__device__ __forceinline__ uint32_t vg_pow_lookup(const uint32_t* lo, const uint32_t* hi, uint64_t e) {
+    return bb::mul(__ldg(lo + (e & (VG_POW_LO - 1))), __ldg(hi + (e >> VG_POW_LO_BITS)));
+}
 
 // kernel classes for the optional per-launch CUDA-event timing (bench.py's roofline line)
 enum KClass { KC_NTT = 0, KC_LEAF_HASH, KC_COMPRESS, KC_FRI_LEAF, KC_TRANSPOSE, KC_PERM, KC_QUOTIENT, KC_INVDEN, KC_BARY, KC_REDUCED_OPENING, KC_FRI_FOLD, KC_EXCHANGE, KC_COLLECTIVE, KC_OTHER, KC_CHECK, KC_COUNT };
@@ -35,7 +39,6 @@ struct vgpu_ctx {
     PowTable root_table;                                        // base = two_adic_generator(27)
     uint32_t* root3 = nullptr;                                   // 3 x 512 words: w^(i), w^(512 i), w^(2^18 i) — a 6 KB, L1-resident form of the same table
     std::map<std::pair<uint32_t, uint32_t>, PowTable> shift_tables;  // (shift, scale) canonical -> table
-    std::vector<void*> owned;                                   // freed at destroy
     // Poseidon challenger instance (host side; the transcript is sequential and tiny)
     uint32_t poseidon_rc[480];
     uint32_t poseidon_mds[256];
@@ -108,16 +111,22 @@ struct vgpu_dmat {
 #define VG_TRY(expr) do { int32_t _r = (expr); if (_r != 0) return _r; } while (0)
 #define VG_LAUNCH_CHECK(ctx) do { (ctx)->launches++; cudaError_t _e = cudaGetLastError(); if (_e != cudaSuccess) { VG_FAIL(ctx, "kernel launch failed at %s:%d: %s", __FILE__, __LINE__, cudaGetErrorString(_e)); } } while (0)
 
+// an event from ctx->event_pool (where its users return the ones they are done with), or a new one
+inline cudaError_t vg_take_event(vgpu_ctx* ctx, cudaEvent_t* e) {
+    if (ctx->event_pool.empty()) return cudaEventCreate(e);
+    *e = ctx->event_pool.back();
+    ctx->event_pool.pop_back();
+    return cudaSuccess;
+}
+
 // RAII scope: when ctx->ktiming is on, brackets the launches inside it with a CUDA event pair on ctx->stream.
 struct KScope {
     vgpu_ctx* ctx; bool on; size_t idx = 0;      // scopes nest (a collective inside a sweep): each closes ITS pair
     KScope(vgpu_ctx* c, int cls, double bytes) : ctx(c), on(c->ktiming) {
         if (!on) return;
         KTimer t; t.cls = cls; t.bytes = bytes;
-        for (cudaEvent_t* e : {&t.a, &t.b}) {
-            if (!c->event_pool.empty()) { *e = c->event_pool.back(); c->event_pool.pop_back(); }
-            else cudaEventCreate(e);
-        }
+        vg_take_event(c, &t.a);
+        vg_take_event(c, &t.b);
         cudaEventRecord(t.a, c->stream);
         c->ktimers.push_back(t);
         idx = c->ktimers.size() - 1;

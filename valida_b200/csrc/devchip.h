@@ -23,7 +23,6 @@ struct DevChip {
 };
 
 int32_t vg_build_devchip(vgpu_ctx* ctx, const vgpu_chip_desc* chip, const uint32_t challenges_canonical[15], DevChip* out);
-int32_t vg_upload_devchip(vgpu_ctx* ctx, const vgpu_chip_desc* chip, const uint32_t challenges_canonical[15], DevChip** out_device);
 int32_t vg_prefix_sum_columns(vgpu_ctx* ctx, uint32_t* data, uint64_t cs, uint64_t n, uint32_t ncols);
 int32_t vg_ext_batch_inverse(vgpu_ctx* ctx, uint32_t* data, uint64_t cs, uint64_t h, uint32_t groups);
 int32_t vg_perm_trace_enqueue(vgpu_ctx* ctx, const vgpu_chip_desc* chip, const vgpu_dmat* main, const vgpu_dmat* prep_or_null,

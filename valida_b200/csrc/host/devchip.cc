@@ -31,14 +31,3 @@ int32_t vg_build_devchip(vgpu_ctx* ctx, const vgpu_chip_desc* chip, const uint32
     }
     return 0;
 }
-
-int32_t vg_upload_devchip(vgpu_ctx* ctx, const vgpu_chip_desc* chip, const uint32_t ch[15], DevChip** out_device) {
-    DevChip host;
-    VG_TRY(vg_build_devchip(ctx, chip, ch, &host));
-    DevChip* d = nullptr;
-    VG_TRY(vg_alloc(ctx, (void**)&d, sizeof(DevChip)));
-    VG_CUDA(ctx, cudaMemcpyAsync(d, &host, sizeof(DevChip), cudaMemcpyHostToDevice, ctx->stream));
-    VG_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
-    *out_device = d;
-    return 0;
-}

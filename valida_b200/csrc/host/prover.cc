@@ -9,8 +9,8 @@
 #include "../open.h"
 #include "../devchip.h"
 #include "challenger.h"
+#include "fri_config.h"
 #include <algorithm>
-#include <array>
 #include <chrono>
 #include <cstring>
 #include <map>
@@ -20,9 +20,6 @@ using bb::E5;
 
 namespace {
 
-constexpr int LOG_BLOWUP = 1, NUM_QUERIES = 40, POW_BITS = 8;   // basic/src/bin/valida.rs:385-390
-
-using Digest = std::array<uint32_t, 8>;   // canonical words
 struct ExtC { uint32_t c[5]; };           // canonical
 ExtC canon(const E5& e) { ExtC r; for (int i = 0; i < 5; i++) r.c[i] = bb::from_monty(e.c[i]); return r; }
 
@@ -41,13 +38,10 @@ struct OpenRound { const vgpu_prover_data* pd; std::vector<std::vector<E5>> poin
 // synchronisation inside the proof.
 struct Phase {
     vgpu_ctx* ctx;
-    static cudaEvent_t ev(vgpu_ctx* c) {
-        cudaEvent_t e = nullptr;
-        if (!c->event_pool.empty()) { e = c->event_pool.back(); c->event_pool.pop_back(); } else cudaEventCreate(&e);
-        return e;
-    }
     Phase(vgpu_ctx* c, const char* n) : ctx(c) {
-        vgpu_ctx::PhaseMark m; m.name = n; m.a = ev(c); m.b = ev(c);
+        vgpu_ctx::PhaseMark m{n, nullptr, nullptr};
+        vg_take_event(c, &m.a);
+        vg_take_event(c, &m.b);
         cudaEventRecord(m.a, c->stream);
         c->phase_marks.push_back(m);
         idx = c->phase_marks.size() - 1;

@@ -24,7 +24,6 @@
 #include <memory>
 #include <new>
 #include <exception>
-#include <chrono>
 #include <cstdio>
 #include <omp.h>
 #include "../../../include/valida_b200.h"
@@ -514,18 +513,13 @@ static int vm_run_impl(const int32_t* program_words, uint64_t n_instr, uint32_t 
 
 // Chip::generate_trace x14 on the host
 static vgpu_traces* build_traces_host(Vm& vm) {
-    // VGPU_TRACEGEN_TIMING=1 prints the time of each stage to stderr (development aid)
-    auto T0 = std::chrono::steady_clock::now();
-    auto lap = [&](const char* what) { if (getenv("VGPU_TRACEGEN_TIMING")) { auto t = std::chrono::steady_clock::now(); fprintf(stderr, "tracegen %-12s %.3f s\n", what, std::chrono::duration<double>(t - T0).count()); T0 = t; } };
     const int32_t* program_words = vm.prog;
     const uint64_t n_instr = vm.n_instr;
     std::unique_ptr<vgpu_traces> tr(new vgpu_traces());      // released to the caller at the end; freed if an allocation below throws
     Traces& t = tr->t;
     t.clock = vm.clock; t.n_mem_ops = (uint32_t)vm.mem_ops.size(); t.n_add_ops = (uint32_t)vm.adds.size(); t.n_sub_ops = (uint32_t)vm.subs.size();
     build_cpu(vm, t);
-    lap("cpu");
     build_mem(vm, t);
-    lap("mem");
     {  // program: 1 main column (counts) + 7 preprocessed
         size_t h = next_pow2(n_instr);
         t.store[1].zeros(h);
@@ -541,7 +535,6 @@ static vgpu_traces* build_traces_host(Vm& vm) {
     }
     build_addsub(vm.adds, true, t.store[3], t.main[3]);
     build_addsub(vm.subs, false, t.store[4], t.main[4]);
-    lap("prog+addsub");
     {  // mul: 2^10 counter rows
         t.store[5].zeros(1024 * 18);
         for (size_t i = 0; i < 1024; i++) t.store[5][i * 18 + 17] = (uint32_t)i + 1;
@@ -569,7 +562,6 @@ static vgpu_traces* build_traces_host(Vm& vm) {
         t.main[13] = {t.store[13].data(), h, 6};
     }
     t.cells = vm.cells;
-    lap("rest");
     return tr.release();
 }
 

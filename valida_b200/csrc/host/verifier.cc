@@ -9,7 +9,7 @@
 #include "../ctx.h"
 #include "../verify.h"
 #include "challenger.h"
-#include <array>
+#include "fri_config.h"
 #include <cstring>
 #include <string>
 
@@ -17,10 +17,7 @@ using bb::E5;
 
 namespace {
 
-constexpr int LOG_BLOWUP = 1, NUM_QUERIES = 40, POW_BITS = 8;   // basic/src/bin/valida.rs:385-390
 constexpr int MAX_LOG_DEGREE = 26;
-
-using Digest = std::array<uint32_t, 8>;   // canonical words
 
 // ---- Keccak-256 on the host (original 0x01 padding: p3-keccak wraps tiny-keccak's Keccak::v256) -------
 const uint64_t RC[24] = {0x0000000000000001ull, 0x0000000000008082ull, 0x800000000000808aull, 0x8000000080008000ull, 0x000000000000808bull,

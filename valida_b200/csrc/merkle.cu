@@ -15,7 +15,6 @@
 #include "keccak.cuh"
 #include "merkle.h"
 #include <algorithm>
-#include <cstdlib>
 #include <numeric>
 
 namespace {
@@ -352,12 +351,11 @@ constexpr uint64_t TAIL_FUSE = 1u << 15;
 template <class Inject>
 static int32_t build_upper_layers(vgpu_ctx* ctx, const std::vector<LayerPlan>& plan, VgTree* t, uint32_t* inject_buf, Inject inject) {
     if (plan[0].gather) VG_TRY(vg_comm_allgather_inplace(ctx, t->layer_ptr[0], 8));
-    static const bool fuse = [] { const char* e = getenv("VGPU_TREE_TAIL"); return !e || atoi(e) != 0; }();   // tuning knob (profiles/)
     size_t lvl = 1;
     while (lvl < plan.size()) {
         const LayerPlan& p = plan[lvl];
         const uint32_t* prev_v = t->layer_ptr[lvl - 1] - plan[lvl - 1].sbegin * 8;
-        if (fuse && p.ccount <= TAIL_FUSE) {
+        if (p.ccount <= TAIL_FUSE) {
             // one launch: levels lvl .. lvl + n - 1, each half the one below; stop after a gather layer and at the root
             TailParams tp{};
             tp.prev_v = prev_v; tp.first_begin = p.cbegin;

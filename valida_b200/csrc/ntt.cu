@@ -20,7 +20,6 @@
 //  * twiddles: a two-level power table of w_(2^27) in global memory (L2-resident) feeds a per-CTA
 //    shared table of w_L^j.
 #include "ctx.h"
-#include <cstdlib>
 
 namespace {
 
@@ -42,7 +41,7 @@ struct PassParams {
     uint32_t pre_mode; uint32_t pre_r, pre_g, pre_shift;   // exponent = (rnat*pre_r + gval*pre_g) << pre_shift  (< 2^27)
     // post-multiplier on natural output k: mode 1: w_NMAX^(+-(gval*k) * post_unit) ; mode 2: table[gval*post_g + k*post_k] ; mode 3: constant
     uint32_t post_mode; uint32_t post_shift, post_g, post_k; uint32_t post_scale;   // mode 1 exponent = (gval*k) << post_shift
-    const uint32_t* root_lo; const uint32_t* root_hi;   // w_NMAX tables (two-level: 4096 + 32768 entries)
+    const uint32_t* root_hi;                            // w_NMAX two-level table, hi part: w^(4096 j)
     const uint32_t* root3;                              // w_NMAX three-level table (3 x 512 entries, stays in L1)
     const uint32_t* tab_lo; const uint32_t* tab_hi;     // shift tables (mode 2)
     uint32_t tab_base;                                  // the table's base (shift) in Montgomery form
@@ -246,8 +245,7 @@ __device__ __forceinline__ void post_begin(const PassParams& p, uint32_t gval, u
         if (p.inverse) { e0 = 0u - e0; es = 0u - es; }
         *m = root_pow(p, e0); *step = root_pow(p, es);
     } else if (p.post_mode == 2) {
-        const uint32_t e0 = gval * p.post_g + k_start * p.post_k;
-        *m = mul(__ldg(p.tab_lo + (e0 & (VG_POW_LO - 1))), __ldg(p.tab_hi + (e0 >> VG_POW_LO_BITS)));
+        *m = vg_pow_lookup(p.tab_lo, p.tab_hi, gval * p.post_g + k_start * p.post_k);
         *step = p.tab_step;
     } else { *m = p.post_mode == 3 ? p.post_scale : bb::R1; *step = bb::R1; }
 }
@@ -469,15 +467,7 @@ __global__ void __launch_bounds__(512) ntt_pass_kernel(PassParams p) {
                 const uint32_t k_start = p.dst_natural ? p0 : (bb::reverse_bits(p0, (int)lowbits) << ibits);
                 const uint32_t k_stride = p.dst_natural ? (1u << lowbits) : 1u;
                 uint32_t m, step;
-                if (p.post_mode == 1) {
-                    uint32_t e0 = (gval * k_start) << p.post_shift, es = (gval * k_stride) << p.post_shift;
-                    if (p.inverse) { e0 = 0u - e0; es = 0u - es; }
-                    m = root_pow(p, e0); step = root_pow(p, es);
-                } else {
-                    const uint32_t e0 = gval * p.post_g + k_start * p.post_k;
-                    m = mul(__ldg(p.tab_lo + (e0 & (VG_POW_LO - 1))), __ldg(p.tab_hi + (e0 >> VG_POW_LO_BITS)));
-                    step = p.tab_step;
-                }
+                post_begin(p, gval, k_start, k_stride, &m, &step);
                 uint32_t* dcol = dst + (uint64_t)g * p.dst_gs;
                 const uint32_t* drow = data + t * LS;
                 for (uint32_t i = 0; i < I; i++) {
@@ -504,8 +494,7 @@ __global__ void __launch_bounds__(512) ntt_pass_kernel(PassParams p) {
                         if (p.inverse) e = (0u - e);                      // root_pow masks to 27 bits: w^(-e) = w^(2^27 - e)
                         v = mul(v, root_pow(p, e));
                     } else if (p.post_mode == 2) {
-                        const uint32_t e = gval * p.post_g + k * p.post_k;
-                        v = mul(v, mul(__ldg(p.tab_lo + (e & (VG_POW_LO - 1))), __ldg(p.tab_hi + (e >> VG_POW_LO_BITS))));
+                        v = mul(v, vg_pow_lookup(p.tab_lo, p.tab_hi, gval * p.post_g + k * p.post_k));
                     } else {
                         v = mul(v, p.post_scale);
                     }
@@ -530,7 +519,7 @@ uint32_t choose_tile(int log_len, uint64_t groups) {
 }
 
 int32_t launch_pass(vgpu_ctx* ctx, PassParams p, uint64_t w) {
-    p.root_lo = ctx->root_table.lo; p.root_hi = ctx->root_table.hi; p.root3 = ctx->root3;
+    p.root_hi = ctx->root_table.hi; p.root3 = ctx->root3;
     const uint32_t L = 1u << p.log_len;
     p.tile = choose_tile((int)p.log_len, p.groups);
     const uint64_t tiles = p.groups / p.tile;

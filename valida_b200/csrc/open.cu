@@ -10,7 +10,6 @@
 #include "devchip.h"
 #include "open.h"
 #include <algorithm>
-#include <cstdlib>
 #include <memory>
 
 namespace {
@@ -18,8 +17,7 @@ namespace {
 using bb::E5;
 
 __device__ __forceinline__ uint32_t oroot_pow(const uint32_t* lo, const uint32_t* hi, uint64_t e) {
-    e &= ((1ull << VG_LOG_NMAX) - 1);
-    return bb::mul(__ldg(lo + (e & (VG_POW_LO - 1))), __ldg(hi + (e >> VG_POW_LO_BITS)));
+    return vg_pow_lookup(lo, hi, e & ((1ull << VG_LOG_NMAX) - 1));
 }
 __device__ __forceinline__ E5 ld5(const uint32_t* v, uint64_t cs, uint64_t i) {
     E5 r;
@@ -305,8 +303,8 @@ struct InvdenParams {
     uint32_t qc[4][5];       // Q(x) = x^4 + sum_j qc[j] x^j   (qc[j] ext5, limb l at qc[j][l])
     const uint32_t* lo; const uint32_t* hi;
 };
-template <int INVDEN_BATCH, int MINB>
-__global__ void __launch_bounds__(128, MINB) invden_norm_kernel(const __grid_constant__ InvdenParams p) {
+constexpr int INVDEN_BATCH = 8, INVDEN_MINB = 8;
+__global__ void __launch_bounds__(128, INVDEN_MINB) invden_norm_kernel(const __grid_constant__ InvdenParams p) {
     const uint64_t stride = (p.count + INVDEN_BATCH - 1) / INVDEN_BATCH;
     const uint64_t t = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
     if (t >= stride) return;
@@ -384,14 +382,8 @@ int32_t vg_inverse_denominators(vgpu_ctx* ctx, uint32_t log_H, const E5& z, uint
         }
         for (int j = 0; j < 4; j++) for (int l = 0; l < 5; l++) p.qc[j][l] = q[j].c[l];
     }
-    static const int batch = [] { const char* e = getenv("VGPU_INVDEN_BATCH"); return e ? atoi(e) : 8; }();   // tuning knob (profiles/)
-    if (batch == 8) {
-        const uint64_t stride = (count + 7) / 8;
-        invden_norm_kernel<8, 8><<<(unsigned)((stride + 127) / 128), 128, 0, ctx->stream>>>(p);
-    } else {
-        const uint64_t stride = (count + 15) / 16;
-        invden_norm_kernel<16, 4><<<(unsigned)((stride + 127) / 128), 128, 0, ctx->stream>>>(p);
-    }
+    const uint64_t stride = (count + INVDEN_BATCH - 1) / INVDEN_BATCH;
+    invden_norm_kernel<<<(unsigned)((stride + 127) / 128), 128, 0, ctx->stream>>>(p);
     VG_LAUNCH_CHECK(ctx);
     return 0;
 }

@@ -11,7 +11,6 @@
 // Output layout = RowMajorMatrix<Challenge>::flatten_to_base, column-major on device: column 5m+l.
 #include "ctx.h"
 #include "devchip.h"
-#include <cstdlib>
 #include <memory>
 
 namespace {
@@ -44,9 +43,9 @@ __global__ void __launch_bounds__(256) perm_denominators_kernel(const __grid_con
 }
 
 constexpr int INV_BATCH = 8;
+constexpr int INV_MINB = 5;   // resident CTAs per SM: the register cap of 8 spills (88-byte stack frame)
 // In-place inverse of `count` ext5 columns (column group g uses base columns 5g..5g+4); zero stays zero.
-template <int MINB>
-__global__ void __launch_bounds__(128, MINB) ext_batch_inverse_kernel(uint32_t* __restrict__ data, uint64_t cs, uint64_t h, uint32_t groups) {
+__global__ void __launch_bounds__(128, INV_MINB) ext_batch_inverse_kernel(uint32_t* __restrict__ data, uint64_t cs, uint64_t h, uint32_t groups) {
     uint64_t stride = (h + INV_BATCH - 1) / INV_BATCH;
     uint64_t t = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
     if (t >= stride) return;
@@ -216,10 +215,7 @@ int32_t vg_prefix_sum_columns(vgpu_ctx* ctx, uint32_t* data, uint64_t cs, uint64
 int32_t vg_ext_batch_inverse(vgpu_ctx* ctx, uint32_t* data, uint64_t cs, uint64_t h, uint32_t groups) {
     if (!groups || !h) return 0;
     uint64_t stride = (h + INV_BATCH - 1) / INV_BATCH;
-    static const int minb = [] { const char* e = getenv("VGPU_EXTINV_MINB"); return e ? atoi(e) : 5; }();   // tuning knob (profiles/)
-    if (minb == 8) ext_batch_inverse_kernel<8><<<(unsigned)((stride + 127) / 128), 128, 0, ctx->stream>>>(data, cs, h, groups);
-    else if (minb == 6) ext_batch_inverse_kernel<6><<<(unsigned)((stride + 127) / 128), 128, 0, ctx->stream>>>(data, cs, h, groups);
-    else ext_batch_inverse_kernel<5><<<(unsigned)((stride + 127) / 128), 128, 0, ctx->stream>>>(data, cs, h, groups);
+    ext_batch_inverse_kernel<<<(unsigned)((stride + 127) / 128), 128, 0, ctx->stream>>>(data, cs, h, groups);
     VG_LAUNCH_CHECK(ctx);
     return 0;
 }

@@ -24,7 +24,6 @@
 #include "airs.cuh"
 #include "logup.cuh"
 #include <cstring>
-#include <cstdlib>
 #include <memory>
 
 namespace {
@@ -71,13 +70,13 @@ struct DevBuilder {
 };
 
 __device__ __forceinline__ uint32_t qroot_pow(const QParams& p, uint64_t e) {
-    e &= ((1ull << VG_LOG_NMAX) - 1);
-    return bb::mul(__ldg(p.root_lo + (e & (VG_POW_LO - 1))), __ldg(p.root_hi + (e >> VG_POW_LO_BITS)));
+    return vg_pow_lookup(p.root_lo, p.root_hi, e & ((1ull << VG_LOG_NMAX) - 1));
 }
-// MINB: resident-CTA target (register cap) of the variant.  The sweep is latency bound (ncu r1b: issue slots 43-57 % busy at
-// 5 CTAs per SM), so more resident warps beat fewer spills: measured 11.4 / 8.9 / 8.6 ms per proof at 2-4 / 6 / 8 CTAs per SM.
-template <int CHIP, int MINB>
-__global__ void __launch_bounds__(128, MINB) quotient_kernel(const __grid_constant__ QParams p) {
+// Resident-CTA target (register cap) of the sweep.  It is latency bound (ncu r1b: issue slots 43-57 % busy at 5 CTAs per
+// SM), so more resident warps beat fewer spills: measured 11.4 / 8.9 / 8.6 ms per proof at 2-4 / 6 / 8 CTAs per SM.
+constexpr int QUOTIENT_MINB = 8;
+template <int CHIP>
+__global__ void __launch_bounds__(128, QUOTIENT_MINB) quotient_kernel(const __grid_constant__ QParams p) {
     const uint64_t h = 1ull << p.log_h, H = 2 * h;
     const uint64_t rho_raw = p.row_begin + (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;     // storage row of the committed LDEs
     const bool active = rho_raw < p.row_end;
@@ -151,8 +150,8 @@ __global__ void __launch_bounds__(256) selector_inverse_kernel(uint32_t* __restr
         v[i] = bb::R1;
         if (t + (uint64_t)i * stride < count) {
             const uint32_t j = bb::reverse_bits((uint32_t)r, (int)log_h);
-            uint64_t e = ((uint64_t)j << (VG_LOG_NMAX - log_h - 1)) & ((1ull << VG_LOG_NMAX) - 1);
-            const uint32_t x0 = bb::mul(s, bb::mul(__ldg(root_lo + (e & (VG_POW_LO - 1))), __ldg(root_hi + (e >> VG_POW_LO_BITS))));
+            const uint64_t e = ((uint64_t)j << (VG_LOG_NMAX - log_h - 1)) & ((1ull << VG_LOG_NMAX) - 1);
+            const uint32_t x0 = bb::mul(s, vg_pow_lookup(root_lo, root_hi, e));
             const uint32_t nx0 = bb::neg(x0);
             v[i] = bb::mul(bb::mul(bb::sub(x0, bb::R1), bb::sub(x0, glast)), bb::mul(bb::sub(nx0, bb::R1), bb::sub(nx0, glast)));
         }
@@ -175,24 +174,13 @@ struct CountBuilder {
     BB_HD F N(int) const { return F{0}; }
     BB_HD void z(F) { n++; }
 };
-template <int CHIP> uint32_t count_base() { CountBuilder c; air::eval_chip<CHIP>(c); return c.n; }
-
-template <int CHIP> void launch(const QParams& p, uint64_t h, cudaStream_t st) {
-    (void)h;
-    static const int minb = [] { const char* e = getenv("VGPU_QUOTIENT_MINB"); return e ? atoi(e) : 8; }();   // tuning knob (profiles/)
-    const unsigned grid = (unsigned)((p.row_end - p.row_begin + 127) / 128);
-    if (minb == 6) quotient_kernel<CHIP, 6><<<grid, 128, 0, st>>>(p);
-    else quotient_kernel<CHIP, 8><<<grid, 128, 0, st>>>(p);
-}
 
 }  // namespace
 
 uint32_t vg_chip_base_constraints(uint32_t chip_id) {
-    switch (chip_id) {
-        case 0: return count_base<0>(); case 3: return count_base<3>(); case 4: return count_base<4>(); case 5: return count_base<5>();
-        case 7: return count_base<7>(); case 8: return count_base<8>(); case 9: return count_base<9>(); case 10: return count_base<10>();
-        case 11: return count_base<11>(); case 13: return count_base<13>(); default: return 0;
-    }
+    CountBuilder c;
+    air::with_chip(chip_id, [&](auto chip) { air::eval_chip<decltype(chip)::value>(c); });
+    return c.n;
 }
 
 extern "C" int32_t vgpu_quotient(vgpu_ctx* ctx, const vgpu_chip_desc* chip, uint32_t log_degree, const vgpu_dmat* prep_lde,
@@ -264,15 +252,9 @@ extern "C" int32_t vgpu_quotient(vgpu_ctx* ctx, const vgpu_chip_desc* chip, uint
         selector_inverse_kernel<<<(unsigned)((stride + 255) / 256), 256, 0, ctx->stream>>>(selinv - pb, pb, pc, log_degree, p.s, p.glast, p.root_lo, p.root_hi);
         ctx->launches++;
     }
-    switch (chip->chip_id) {
-        case 0: launch<0>(p, h, ctx->stream); break;   case 1: launch<1>(p, h, ctx->stream); break;
-        case 2: launch<2>(p, h, ctx->stream); break;   case 3: launch<3>(p, h, ctx->stream); break;
-        case 4: launch<4>(p, h, ctx->stream); break;   case 5: launch<5>(p, h, ctx->stream); break;
-        case 6: launch<6>(p, h, ctx->stream); break;   case 7: launch<7>(p, h, ctx->stream); break;
-        case 8: launch<8>(p, h, ctx->stream); break;   case 9: launch<9>(p, h, ctx->stream); break;
-        case 10: launch<10>(p, h, ctx->stream); break; case 11: launch<11>(p, h, ctx->stream); break;
-        case 12: launch<12>(p, h, ctx->stream); break; case 13: launch<13>(p, h, ctx->stream); break;
-    }
+    air::with_chip(chip->chip_id, [&](auto c) {
+        quotient_kernel<decltype(c)::value><<<(unsigned)((p.row_end - p.row_begin + 127) / 128), 128, 0, ctx->stream>>>(p);
+    });
     delete ks;
     vg_free(ctx, selinv);
     VG_LAUNCH_CHECK(ctx);

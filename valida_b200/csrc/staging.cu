@@ -169,14 +169,12 @@ int32_t vg_upload_begin(vgpu_ctx* ctx, const uint32_t* host, uint64_t h, uint64_
     VG_TRY(vg_alloc(ctx, (void**)&dst->pend_stage, h * w * 4));
     {   // the staging block may be a cached one whose last user is still queued on the compute stream
         cudaEvent_t fence;
-        if (!ctx->event_pool.empty()) { fence = ctx->event_pool.back(); ctx->event_pool.pop_back(); }
-        else VG_CUDA(ctx, cudaEventCreate(&fence));
+        VG_CUDA(ctx, vg_take_event(ctx, &fence));
         VG_CUDA(ctx, cudaEventRecord(fence, ctx->stream));
         VG_CUDA(ctx, cudaStreamWaitEvent(ctx->copy_stream, fence, 0));
         ctx->event_pool.push_back(fence);
     }
-    if (!ctx->event_pool.empty()) { dst->pend_ev = ctx->event_pool.back(); ctx->event_pool.pop_back(); }
-    else VG_CUDA(ctx, cudaEventCreate(&dst->pend_ev));
+    VG_CUDA(ctx, vg_take_event(ctx, &dst->pend_ev));
     dst->pend_repr = repr;
     const size_t bytes = h * w * 4;
     if (bytes >= STAGE_MIN && is_pageable(host)) {

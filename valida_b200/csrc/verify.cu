@@ -26,17 +26,6 @@ struct VerifierFolder {
     void z_ext(const E5& x) { acc = bb::e5_add(bb::e5_mul(acc, alpha), x); }
 };
 
-template <int CHIP> void eval_one(VerifierFolder& f) { air::eval_chip<CHIP>(f); }
-
-void eval_air(uint32_t chip_id, VerifierFolder& f) {
-    switch (chip_id) {
-        case 0: eval_one<0>(f); break;   case 3: eval_one<3>(f); break;   case 4: eval_one<4>(f); break;
-        case 5: eval_one<5>(f); break;   case 7: eval_one<7>(f); break;   case 8: eval_one<8>(f); break;
-        case 9: eval_one<9>(f); break;   case 10: eval_one<10>(f); break; case 11: eval_one<11>(f); break;
-        case 13: eval_one<13>(f); break; default: break;   // program, memory, div, range: empty eval
-    }
-}
-
 // VirtualPairCol::apply over extension-valued rows (p3_air::VirtualPairCol; machine/src/chip.rs:76-80)
 bool pair_col_ext(const DevPairCol& pc, const E5* main_row, E5* out) {
     E5 v = bb::e5_from_base(pc.constant);
@@ -79,7 +68,7 @@ int32_t vg_verify_chip_constraints(vgpu_ctx* ctx, const vgpu_chip_desc* chip, ui
     f.last = X{bb::e5_mul(z_h, bb::e5_inv(zmg))};
     f.trans = X{zmg};
     f.alpha = alpha; f.acc = bb::e5_zero();
-    eval_air(chip->chip_id, f);
+    air::with_chip(chip->chip_id, [&](auto c) { air::eval_chip<decltype(c)::value>(f); });
     {   // eval_permutation_constraints
         std::vector<E5> pl(pw), pn(pw);
         for (uint32_t m = 0; m < pw; m++) { pl[m] = unflatten(ov.perm_local.data(), m); pn[m] = unflatten(ov.perm_next.data(), m); }
