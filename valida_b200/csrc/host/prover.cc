@@ -10,6 +10,7 @@
 #include "../devchip.h"
 #include "challenger.h"
 #include "fri_config.h"
+#include "proof.h"
 #include <algorithm>
 #include <chrono>
 #include <cstring>
@@ -20,18 +21,6 @@ using bb::E5;
 
 namespace {
 
-struct ExtC { uint32_t c[5]; };           // canonical
-ExtC canon(const E5& e) { ExtC r; for (int i = 0; i < 5; i++) r.c[i] = bb::from_monty(e.c[i]); return r; }
-
-struct BatchOpeningH { std::vector<std::vector<uint32_t>> opened_values; std::vector<Digest> opening_proof; };
-struct CommitPhaseStepH { ExtC sibling_value; std::vector<Digest> opening_proof; };
-struct QueryProofH { std::vector<CommitPhaseStepH> steps; };
-struct FriProofH { std::vector<Digest> commit_phase_commits; std::vector<QueryProofH> query_proofs; ExtC final_poly; uint32_t pow_witness; };
-struct OpeningH {
-    std::vector<std::vector<std::vector<std::vector<ExtC>>>> values;   // [round][matrix][point][column]
-    FriProofH fri;
-    std::vector<std::vector<BatchOpeningH>> query_openings;             // [query][round]
-};
 struct OpenRound { const vgpu_prover_data* pd; std::vector<std::vector<E5>> points; };
 
 // Device time of a phase: an event pair on the context's stream, read back by vgpu_last_prove_phases — no host
@@ -106,7 +95,7 @@ struct OpenScratch {
     }
 };
 
-int32_t open_multi_batches(vgpu_ctx* ctx, const std::vector<OpenRound>& rounds, vgh::Challenger& ch, OpeningH* out) {
+int32_t open_multi_batches(vgpu_ctx* ctx, const std::vector<OpenRound>& rounds, vgh::Challenger& ch, vgh::OpenedValues* values, vgh::PcsProof* out) {
     const E5 alpha = ch.sample_ext();
     // alpha^c table (host; the reduced-opening kernel takes its powers through the kernel parameters)
     uint32_t max_w = 1;
@@ -154,25 +143,24 @@ int32_t open_multi_batches(vgpu_ctx* ctx, const std::vector<OpenRound>& rounds, 
     VG_CUDA(ctx, cudaMemcpyAsync(sums.data(), S.d_sums, sums_words * 4, cudaMemcpyDeviceToHost, ctx->stream));
     VG_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
     // Pass 2 — opened values on the host, then the reduced openings of every matrix (again without waiting)
-    out->values.clear();
+    values->clear();
     {
         size_t ji = 0;
         std::vector<E5> apow_off(max_w);
         for (const OpenRound& rd : rounds) {
-            out->values.emplace_back();
+            values->emplace_back();
             for (size_t mi = 0; mi < rd.pd->ldes.size(); mi++, ji++) {
                 const Job& j = jobs[ji];
                 const uint32_t w = j.w, np = (uint32_t)j.pts->size();
                 std::vector<E5> ys;
                 vg_eval_columns_finish(sums.data() + j.sums_at, j.lde->gh, w, np, j.pts->data(), &ys, j.lde->dist == VG_ROWS ? vg_eval_columns_first_coset(w) : w);
                 E5 sum_y[2];
-                out->values.back().emplace_back();
+                values->back().emplace_back();
                 for (uint32_t q = 0; q < np; q++) {
                     E5 s = bb::e5_zero();
-                    std::vector<ExtC> yc(w);
-                    for (uint32_t c = 0; c < w; c++) { s = bb::e5_add(s, bb::e5_mul(apow[c], ys[q * w + c])); yc[c] = canon(ys[q * w + c]); }
+                    for (uint32_t c = 0; c < w; c++) s = bb::e5_add(s, bb::e5_mul(apow[c], ys[q * w + c]));
                     sum_y[q] = s;
-                    out->values.back().back().push_back(std::move(yc));
+                    values->back().back().emplace_back(ys.begin() + q * w, ys.begin() + (q + 1) * w);
                 }
                 // point q's terms carry alpha^(num_reduced + q * w): the power table is shifted by the first offset
                 const E5 a_off = bb::e5_pow(alpha, num_reduced[j.log_H]);
@@ -202,7 +190,7 @@ int32_t open_multi_batches(vgpu_ctx* ctx, const std::vector<OpenRound>& rounds, 
         Digest root;
         VG_TRY(vg_fri_layer_commit(ctx, cur.d, cur.count, npairs, cur.shard(), &L.tree, root.data()));
         ch.observe_digest_canonical(root.data());
-        out->fri.commit_phase_commits.push_back(root);
+        out->commit_phase_commits.push_back(root);
         E5 beta = ch.sample_ext();
         RowVec next;
         VG_TRY(rowvec_alloc(ctx, npairs, &next));
@@ -229,13 +217,11 @@ int32_t open_multi_batches(vgpu_ctx* ctx, const std::vector<OpenRound>& rounds, 
         for (uint64_t i = 1; i < cur.n; i++)
             for (int l = 0; l < 5; l++)
                 if (fin[l * cur.n + i] != f0.c[l]) VG_FAIL(ctx, "FRI: final layer is not constant (the committed functions are not low degree)");
-        out->fri.final_poly = canon(f0);
+        out->final_poly = f0;
     }
     {
         HostPhase hp(ctx, "proof-of-work grind (device search + host check)");
-        uint32_t wm = 0;
-        VG_TRY(vg_pow_grind(ctx, ch, POW_BITS, &wm));
-        out->fri.pow_witness = bb::from_monty(wm);
+        VG_TRY(vg_pow_grind(ctx, ch, POW_BITS, &out->pow_witness));
     }
     std::vector<uint64_t> indices;
     for (int q = 0; q < NUM_QUERIES; q++) indices.push_back(ch.sample_bits(log_max));
@@ -273,29 +259,28 @@ int32_t open_multi_batches(vgpu_ctx* ctx, const std::vector<OpenRound>& rounds, 
     }
     std::vector<uint32_t> words;
     VG_TRY(vg_gather_words(ctx, ptrs, &words));
-    out->fri.query_proofs.assign((size_t)nq, QueryProofH());
-    out->query_openings.assign((size_t)nq, std::vector<BatchOpeningH>());
+    out->query_proofs.assign((size_t)nq, std::vector<vgh::CommitPhaseStep>());
+    out->query_openings.assign((size_t)nq, std::vector<vgh::BatchOpening>());
 #pragma omp parallel for schedule(static) num_threads(8)
     for (long qi = 0; qi < nq; qi++) {
         size_t pos = per_query * (size_t)qi;
         auto take_digest = [&]() { Digest d; for (int k = 0; k < 8; k++) d[k] = words[pos++]; return d; };
-        QueryProofH& qp = out->fri.query_proofs[qi];
-        qp.steps.reserve(S.layers.size());
+        std::vector<vgh::CommitPhaseStep>& steps = out->query_proofs[qi];
+        steps.reserve(S.layers.size());
         for (size_t i = 0; i < S.layers.size(); i++) {
-            CommitPhaseStepH st;
-            for (int l = 0; l < 5; l++) st.sibling_value.c[l] = bb::from_monty(words[pos++]);
+            vgh::CommitPhaseStep st;
+            for (int l = 0; l < 5; l++) st.sibling_value.c[l] = words[pos++];
             const size_t depth = S.layers[i].tree.layer_ptr.size() - 1;
             st.opening_proof.reserve(depth);
             for (size_t lvl = 0; lvl < depth; lvl++) st.opening_proof.push_back(take_digest());
-            qp.steps.push_back(std::move(st));
+            steps.push_back(std::move(st));
         }
         for (const OpenRound& rd : rounds) {
-            BatchOpeningH bo;
+            vgh::BatchOpening bo;
             int lg = log2u(rd.pd->max_height);
             for (auto* m : rd.pd->ldes) {
-                std::vector<uint32_t> row(m->w);
-                for (uint64_t c = 0; c < m->w; c++) row[c] = bb::from_monty(words[pos++]);
-                bo.opened_values.push_back(std::move(row));
+                bo.opened_values.emplace_back(words.begin() + pos, words.begin() + pos + m->w);
+                pos += m->w;
             }
             for (int lvl = 0; lvl < lg; lvl++) bo.opening_proof.push_back(take_digest());
             out->query_openings[qi].push_back(std::move(bo));
@@ -304,64 +289,13 @@ int32_t open_multi_batches(vgpu_ctx* ctx, const std::vector<OpenRound>& rounds, 
     return 0;
 }
 
-// ---- CBOR (serde/ciborium image of MachineProof; machine/src/proof.rs:13-44) -------------------------
-struct Cbor {
-    // append-only byte buffer with a raw cursor: the ~150 k field elements of a proof are 12-byte stores, not push_backs
-    std::vector<uint8_t> b; size_t n = 0;
-    uint8_t* room(size_t k) { if (n + k > b.size()) b.resize(std::max(2 * b.size(), n + k + (1u << 20))); return b.data() + n; }
-    void finish() { b.resize(n); }
-    void head(uint8_t major, uint64_t v) {
-        uint8_t* o = room(9);
-        const uint8_t m = (uint8_t)(major << 5);
-        if (v < 24) { o[0] = m | (uint8_t)v; n += 1; }
-        else if (v <= 0xff) { o[0] = m | 24; o[1] = (uint8_t)v; n += 2; }
-        else if (v <= 0xffff) { o[0] = m | 25; o[1] = (uint8_t)(v >> 8); o[2] = (uint8_t)v; n += 3; }
-        else if (v <= 0xffffffffull) { o[0] = m | 26; for (int i = 0; i < 4; i++) o[1 + i] = (uint8_t)(v >> (24 - 8 * i)); n += 5; }
-        else { o[0] = m | 27; for (int i = 0; i < 8; i++) o[1 + i] = (uint8_t)(v >> (56 - 8 * i)); n += 9; }
-    }
-    void key(const char* s) { size_t k = std::strlen(s); head(3, k); std::memcpy(room(k), s, k); n += k; }
-    void map(uint64_t k) { head(5, k); }
-    void arr(uint64_t k) { head(4, k); }
-    // BabyBear { value } holds the Montgomery word: {"value": u32}
-    void felt(uint32_t canonical) {
-        static const uint8_t pre[7] = {0xa1, 0x65, 'v', 'a', 'l', 'u', 'e'};
-        const uint32_t v = bb::to_monty(canonical);
-        uint8_t* o = room(12);
-        std::memcpy(o, pre, 7);
-        if (v < 24) { o[7] = (uint8_t)v; n += 8; }
-        else if (v <= 0xff) { o[7] = 24; o[8] = (uint8_t)v; n += 9; }
-        else if (v <= 0xffff) { o[7] = 25; o[8] = (uint8_t)(v >> 8); o[9] = (uint8_t)v; n += 10; }
-        else { o[7] = 26; o[8] = (uint8_t)(v >> 24); o[9] = (uint8_t)(v >> 16); o[10] = (uint8_t)(v >> 8); o[11] = (uint8_t)v; n += 12; }
-    }
-    void ext(const ExtC& e) { map(1); key("value"); arr(5); for (int i = 0; i < 5; i++) felt(e.c[i]); }
-    void digest(const Digest& d) { arr(8); for (int i = 0; i < 8; i++) felt(d[i]); }
-    void digests(const std::vector<Digest>& v) { arr(v.size()); for (auto& d : v) digest(d); }
-    void exts(const std::vector<ExtC>& v) { arr(v.size()); for (auto& e : v) ext(e); }
-};
-
-// TwoAdicFriPcsProof { fri_proof, query_openings } as serde/ciborium writes it
-void write_opening_proof(Cbor& w, const OpeningH& op) {
-    // (encoding the per-query parts on several host threads into buffers of their own was measured: 0.88 ms against 0.64 ms serial)
-    w.map(2);
-    w.key("fri_proof"); w.map(4);
-    w.key("commit_phase_commits"); w.digests(op.fri.commit_phase_commits);
-    w.key("query_proofs"); w.arr(op.fri.query_proofs.size());
-    for (auto& q : op.fri.query_proofs) {
-        w.map(1); w.key("commit_phase_openings"); w.arr(q.steps.size());
-        for (auto& s : q.steps) { w.map(2); w.key("sibling_value"); w.ext(s.sibling_value); w.key("opening_proof"); w.digests(s.opening_proof); }
-    }
-    w.key("final_poly"); w.ext(op.fri.final_poly);
-    w.key("pow_witness"); w.felt(op.fri.pow_witness);
-    w.key("query_openings"); w.arr(op.query_openings.size());
-    for (auto& q : op.query_openings) {
-        w.arr(q.size());
-        for (auto& bo : q) {
-            w.map(2);
-            w.key("opened_values"); w.arr(bo.opened_values.size());
-            for (auto& row : bo.opened_values) { w.arr(row.size()); for (uint32_t x : row) w.felt(x); }
-            w.key("opening_proof"); w.digests(bo.opening_proof);
-        }
-    }
+// The encoded bytes in a buffer of their own, released by vgpu_free_bytes.
+int32_t hand_off(vgpu_ctx* ctx, const std::vector<uint8_t>& bytes, uint8_t** out, uint64_t* out_len) {
+    uint8_t* buf = (uint8_t*)std::malloc(bytes.size());
+    if (!buf) VG_FAIL(ctx, "out of host memory");
+    std::memcpy(buf, bytes.data(), bytes.size());
+    *out = buf; *out_len = bytes.size();
+    return 0;
 }
 
 vgh::Poseidon16* poseidon_of(vgpu_ctx* ctx) {
@@ -460,22 +394,10 @@ int32_t vgpu_open(vgpu_ctx* ctx, const vgpu_prover_data* const* rounds, uint32_t
             rds[r].points.push_back(std::move(pts));
         }
     }
-    OpeningH op;
-    VG_TRY(open_multi_batches(ctx, rds, *(vgh::Challenger*)ctx->challenger, &op));
-    Cbor w;
-    w.arr(2);
-    w.arr(op.values.size());
-    for (auto& round : op.values) {
-        w.arr(round.size());
-        for (auto& mat : round) { w.arr(mat.size()); for (auto& at_point : mat) w.exts(at_point); }
-    }
-    write_opening_proof(w, op);
-    w.finish();
-    uint8_t* buf = (uint8_t*)std::malloc(w.b.size());
-    if (!buf) VG_FAIL(ctx, "out of host memory");
-    std::memcpy(buf, w.b.data(), w.b.size());
-    *out_cbor = buf; *out_len = w.b.size();
-    return 0;
+    vgh::OpenedValues values;
+    vgh::PcsProof proof;
+    VG_TRY(open_multi_batches(ctx, rds, *(vgh::Challenger*)ctx->challenger, &values, &proof));
+    return hand_off(ctx, vgh::encode_opening(values, proof), out_cbor, out_len);
 }
 
 // owned_main: the caller's main traces when this call may release them once the permutation traces are built (their last
@@ -522,11 +444,12 @@ static int32_t prove_device(vgpu_ctx* ctx, const vgpu_dmat* const main[VGPU_NUM_
         VG_TRY(vgpu_commit_batches(ctx, prep, 2, nullptr, digest, &prep_pd.p));
         ch.observe_digest_canonical(digest);
     }
-    Digest main_commit, perm_commit, quot_commit;
+    vgh::MachineProof mp;
+    mp.chip_proofs.resize(VGPU_NUM_CHIPS);
     {   // main commit (313-332)
         Phase ph(ctx, "commit main");
-        VG_TRY(vgpu_commit_batches(ctx, main, VGPU_NUM_CHIPS, nullptr, main_commit.data(), &main_pd.p));
-        ch.observe_digest_canonical(main_commit.data());
+        VG_TRY(vgpu_commit_batches(ctx, main, VGPU_NUM_CHIPS, nullptr, mp.main_trace.data(), &main_pd.p));
+        ch.observe_digest_canonical(mp.main_trace.data());
     }
     uint32_t perm_challenges[15];
     for (int i = 0; i < 3; i++) { E5 e = ch.sample_ext(); for (int l = 0; l < 5; l++) perm_challenges[5 * i + l] = bb::from_monty(e.c[l]); }
@@ -562,6 +485,7 @@ static int32_t prove_device(vgpu_ctx* ctx, const vgpu_dmat* const main[VGPU_NUM_
                 for (int l = 0; l < 5; l++) {
                     uint32_t a = 0;
                     for (uint32_t r = 0; r < nt[i]; r++) a = bb::add(a, ht[((size_t)i * slots + r) * 5 + l]);
+                    mp.chip_proofs[i].cumulative_sum.c[l] = a;
                     cumsum[i][l] = bb::from_monty(a);
                 }
             if (debug) VG_TRY(debug_verdict(ctx, (const unsigned long long*)(ht.data() + tot_words), cumsum));
@@ -572,8 +496,8 @@ static int32_t prove_device(vgpu_ctx* ctx, const vgpu_dmat* const main[VGPU_NUM_
             }
         }
         Phase ph(ctx, "commit permutation");
-        VG_TRY(vgpu_commit_batches(ctx, perms.v.data(), VGPU_NUM_CHIPS, nullptr, perm_commit.data(), &perm_pd.p));
-        ch.observe_digest_canonical(perm_commit.data());
+        VG_TRY(vgpu_commit_batches(ctx, perms.v.data(), VGPU_NUM_CHIPS, nullptr, mp.perm_trace.data(), &perm_pd.p));
+        ch.observe_digest_canonical(mp.perm_trace.data());
     }
     E5 alpha = ch.sample_ext();
     uint32_t alpha_c[5];
@@ -593,8 +517,8 @@ static int32_t prove_device(vgpu_ctx* ctx, const vgpu_dmat* const main[VGPU_NUM_
         Phase ph(ctx, "commit quotient");
         uint32_t shifts[VGPU_NUM_CHIPS];
         for (int i = 0; i < VGPU_NUM_CHIPS; i++) shifts[i] = (uint32_t)(((uint64_t)bb::GEN_CANON * bb::GEN_CANON) % bb::P);   // coset_shift^(2^log_quotient_degree)
-        VG_TRY(vgpu_commit_batches(ctx, quots.v.data(), VGPU_NUM_CHIPS, shifts, quot_commit.data(), &quot_pd.p));
-        ch.observe_digest_canonical(quot_commit.data());
+        VG_TRY(vgpu_commit_batches(ctx, quots.v.data(), VGPU_NUM_CHIPS, shifts, mp.quotient_chunks.data(), &quot_pd.p));
+        ch.observe_digest_canonical(mp.quotient_chunks.data());
     }
     E5 zeta = ch.sample_ext();
     // openings (379-392): main & perm at [zeta, zeta*g_i], quotient at [zeta^2]; preprocessed is NOT opened
@@ -606,44 +530,20 @@ static int32_t prove_device(vgpu_ctx* ctx, const vgpu_dmat* const main[VGPU_NUM_
         rounds[1].points.push_back({zeta, zg});
         rounds[2].points.push_back({bb::e5_sqr(zeta)});
     }
-    OpeningH op;
+    vgh::OpenedValues values;
     {
         Phase ph(ctx, "open (evaluate + FRI)");
-        VG_TRY(open_multi_batches(ctx, rounds, ch, &op));
+        VG_TRY(open_multi_batches(ctx, rounds, ch, &values, &mp.opening_proof));
     }
-    // MachineProof -> CBOR
     HostPhase hc(ctx, "host: MachineProof -> CBOR");
-    Cbor w;
-    w.b.resize(4u << 20);
-    w.map(3);
-    w.key("commitments"); w.map(3);
-    w.key("main_trace"); w.digest(main_commit);
-    w.key("perm_trace"); w.digest(perm_commit);
-    w.key("quotient_chunks"); w.digest(quot_commit);
-    w.key("opening_proof"); write_opening_proof(w, op);
-    w.key("chip_proofs"); w.arr(VGPU_NUM_CHIPS);
-    const std::vector<ExtC> none;
     for (int i = 0; i < VGPU_NUM_CHIPS; i++) {
-        w.map(3);
-        w.key("log_degree"); w.head(0, (uint64_t)log_degrees[i]);
-        w.key("opened_values"); w.map(7);
-        w.key("preprocessed_local"); w.exts(none);
-        w.key("preprocessed_next"); w.exts(none);
-        w.key("trace_local"); w.exts(op.values[0][i][0]);
-        w.key("trace_next"); w.exts(op.values[0][i][1]);
-        w.key("permutation_local"); w.exts(op.values[1][i][0]);
-        w.key("permutation_next"); w.exts(op.values[1][i][1]);
-        w.key("quotient_chunks"); w.exts(op.values[2][i][0]);
-        w.key("cumulative_sum");
-        ExtC cs; for (int l = 0; l < 5; l++) cs.c[l] = cumsum[i][l];
-        w.ext(cs);
+        vgh::ChipProof& c = mp.chip_proofs[i];
+        c.log_degree = (uint32_t)log_degrees[i];
+        c.trace_local = std::move(values[0][i][0]); c.trace_next = std::move(values[0][i][1]);
+        c.permutation_local = std::move(values[1][i][0]); c.permutation_next = std::move(values[1][i][1]);
+        c.quotient_chunks = std::move(values[2][i][0]);
     }
-    w.finish();
-    uint8_t* buf = (uint8_t*)std::malloc(w.b.size());
-    if (!buf) VG_FAIL(ctx, "out of host memory");
-    std::memcpy(buf, w.b.data(), w.b.size());
-    *proof_out = buf; *proof_len = w.b.size();
-    return 0;
+    return hand_off(ctx, vgh::encode(mp), proof_out, proof_len);
 }
 
 int32_t vgpu_prove_device(vgpu_ctx* ctx, const vgpu_dmat* const main[VGPU_NUM_CHIPS], const vgpu_dmat* const prep[2],

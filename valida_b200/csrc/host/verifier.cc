@@ -10,6 +10,7 @@
 #include "../verify.h"
 #include "challenger.h"
 #include "fri_config.h"
+#include "proof.h"
 #include <cstring>
 #include <string>
 
@@ -101,121 +102,16 @@ bool merkle_verify_batch(const Digest& commit, const std::vector<Dim>& dims, uin
     return pos == order.size() && node == commit;
 }
 
-// ---- CBOR reader for exactly the shape vgpu_prove / the reference's ciborium writer emit ----------------
-struct Reader {
-    const uint8_t* p; const uint8_t* end; bool ok = true;
-    uint64_t head(int major) {
-        if (!ok || p >= end) { ok = false; return 0; }
-        uint8_t b = *p++;
-        if ((b >> 5) != major) { ok = false; return 0; }
-        uint8_t info = b & 31;
-        if (info < 24) return info;
-        int n = info == 24 ? 1 : info == 25 ? 2 : info == 26 ? 4 : info == 27 ? 8 : -1;
-        if (n < 0 || end - p < n) { ok = false; return 0; }
-        uint64_t v = 0;
-        for (int i = 0; i < n; i++) v = (v << 8) | *p++;
-        return v;
-    }
-    void key(const char* s) {
-        uint64_t n = head(3), want = std::strlen(s);
-        if (!ok || n != want || (uint64_t)(end - p) < n || std::memcmp(p, s, n) != 0) { ok = false; return; }
-        p += n;
-    }
-    void map(uint64_t n) { if (head(5) != n) ok = false; }
-    // bounded array length: every element costs at least one byte, so a hostile length cannot make us allocate
-    uint64_t arr() { uint64_t n = head(4); if (n > (uint64_t)(end - p)) { ok = false; return 0; } return n; }
-    uint32_t felt() {   // BabyBear { value: Montgomery word }
-        map(1); key("value");
-        uint64_t v = head(0);
-        if (v >= bb::P) ok = false;
-        return (uint32_t)v;
-    }
-    E5 ext() { E5 e = bb::e5_zero(); map(1); key("value"); if (arr() != 5) ok = false; for (int i = 0; i < 5 && ok; i++) e.c[i] = felt(); return e; }
-    Digest digest() { Digest d{}; if (arr() != 8) ok = false; for (int i = 0; i < 8 && ok; i++) d[i] = bb::from_monty(felt()); return d; }
-    std::vector<Digest> digests() { std::vector<Digest> v; uint64_t n = arr(); for (uint64_t i = 0; i < n && ok; i++) v.push_back(digest()); return v; }
-    std::vector<E5> exts() { std::vector<E5> v; uint64_t n = arr(); for (uint64_t i = 0; i < n && ok; i++) v.push_back(ext()); return v; }
-};
-
-struct BatchOpeningV { std::vector<std::vector<uint32_t>> rows_monty; std::vector<Digest> path; };
-struct FriStepV { E5 sibling; std::vector<Digest> path; };
-struct ProofV {
-    Digest main_commit, perm_commit, quot_commit;
-    std::vector<Digest> fri_commits;
-    std::vector<std::vector<FriStepV>> fri_queries;
-    E5 final_poly; uint32_t pow_witness_monty = 0;
-    std::vector<std::vector<BatchOpeningV>> query_openings;   // [query][round]
-    struct Chip { uint32_t log_degree = 0; VgChipOpening ov; size_t n_prep_local = 0, n_prep_next = 0; E5 cumulative_sum; };
-    std::vector<Chip> chips;
-};
-
-bool decode(const uint8_t* data, uint64_t len, ProofV* out) {
-    Reader r{data, data + len};
-    r.map(3);
-    r.key("commitments"); r.map(3);
-    r.key("main_trace"); out->main_commit = r.digest();
-    r.key("perm_trace"); out->perm_commit = r.digest();
-    r.key("quotient_chunks"); out->quot_commit = r.digest();
-    r.key("opening_proof"); r.map(2);
-    r.key("fri_proof"); r.map(4);
-    r.key("commit_phase_commits"); out->fri_commits = r.digests();
-    r.key("query_proofs");
-    for (uint64_t q = 0, nq = r.arr(); q < nq && r.ok; q++) {
-        r.map(1); r.key("commit_phase_openings");
-        std::vector<FriStepV> steps;
-        for (uint64_t s = 0, ns = r.arr(); s < ns && r.ok; s++) {
-            FriStepV st;
-            r.map(2); r.key("sibling_value"); st.sibling = r.ext(); r.key("opening_proof"); st.path = r.digests();
-            steps.push_back(std::move(st));
-        }
-        out->fri_queries.push_back(std::move(steps));
-    }
-    r.key("final_poly"); out->final_poly = r.ext();
-    r.key("pow_witness"); out->pow_witness_monty = r.felt();
-    r.key("query_openings");
-    for (uint64_t q = 0, nq = r.arr(); q < nq && r.ok; q++) {
-        std::vector<BatchOpeningV> per_round;
-        for (uint64_t b = 0, nb = r.arr(); b < nb && r.ok; b++) {
-            BatchOpeningV bo;
-            r.map(2); r.key("opened_values");
-            for (uint64_t m = 0, nm = r.arr(); m < nm && r.ok; m++) {
-                std::vector<uint32_t> row;
-                for (uint64_t c = 0, nc = r.arr(); c < nc && r.ok; c++) row.push_back(r.felt());
-                bo.rows_monty.push_back(std::move(row));
-            }
-            r.key("opening_proof"); bo.path = r.digests();
-            per_round.push_back(std::move(bo));
-        }
-        out->query_openings.push_back(std::move(per_round));
-    }
-    r.key("chip_proofs");
-    for (uint64_t i = 0, n = r.arr(); i < n && r.ok; i++) {
-        ProofV::Chip c;
-        r.map(3);
-        r.key("log_degree"); c.log_degree = (uint32_t)r.head(0);
-        r.key("opened_values"); r.map(7);
-        r.key("preprocessed_local"); c.n_prep_local = r.exts().size();
-        r.key("preprocessed_next"); c.n_prep_next = r.exts().size();
-        r.key("trace_local"); c.ov.trace_local = r.exts();
-        r.key("trace_next"); c.ov.trace_next = r.exts();
-        r.key("permutation_local"); c.ov.perm_local = r.exts();
-        r.key("permutation_next"); c.ov.perm_next = r.exts();
-        r.key("quotient_chunks"); c.ov.quotient_chunks = r.exts();
-        r.key("cumulative_sum"); c.cumulative_sum = r.ext();
-        out->chips.push_back(std::move(c));
-    }
-    return r.ok && r.p == r.end;
-}
-
 struct RoundV { Digest commit; std::vector<Dim> dims; std::vector<std::vector<E5>> points; std::vector<std::vector<const std::vector<E5>*>> values; };
 
 // TwoAdicFriPcs::verify_multi_batches + p3-fri verifier; 0 = accept, otherwise the verdict code of include/valida_b200.h
-int32_t verify_openings(const std::vector<RoundV>& rounds, const ProofV& pf, vgh::Challenger& ch) {
+int32_t verify_openings(const std::vector<RoundV>& rounds, const vgh::PcsProof& pf, vgh::Challenger& ch) {
     const E5 alpha = ch.sample_ext();
     std::vector<E5> betas;
-    for (const Digest& c : pf.fri_commits) { ch.observe_digest_canonical(c.data()); betas.push_back(ch.sample_ext()); }
-    if (pf.fri_queries.size() != (size_t)NUM_QUERIES || pf.query_openings.size() != (size_t)NUM_QUERIES) return VGPU_REJECT_SHAPE;
-    if (!ch.check_witness(POW_BITS, pf.pow_witness_monty)) return VGPU_REJECT_POW;
-    const int log_max_height = (int)pf.fri_commits.size() + LOG_BLOWUP;
+    for (const Digest& c : pf.commit_phase_commits) { ch.observe_digest_canonical(c.data()); betas.push_back(ch.sample_ext()); }
+    if (pf.query_proofs.size() != (size_t)NUM_QUERIES || pf.query_openings.size() != (size_t)NUM_QUERIES) return VGPU_REJECT_SHAPE;
+    if (!ch.check_witness(POW_BITS, pf.pow_witness)) return VGPU_REJECT_POW;
+    const int log_max_height = (int)pf.commit_phase_commits.size() + LOG_BLOWUP;
     if (log_max_height > MAX_LOG_DEGREE + LOG_BLOWUP) return VGPU_REJECT_SHAPE;
     for (auto& rd : rounds)
         for (auto& d : rd.dims) if (log2_ceil(d.h) + LOG_BLOWUP > log_max_height) return VGPU_REJECT_SHAPE;
@@ -229,27 +125,27 @@ int32_t verify_openings(const std::vector<RoundV>& rounds, const ProofV& pf, vgh
         if (pf.query_openings[q].size() != rounds.size()) return VGPU_REJECT_SHAPE;
         for (size_t r = 0; r < rounds.size(); r++) {
             const RoundV& rd = rounds[r];
-            const BatchOpeningV& bo = pf.query_openings[q][r];
-            if (bo.rows_monty.size() != rd.dims.size()) return VGPU_REJECT_SHAPE;
+            const vgh::BatchOpening& bo = pf.query_openings[q][r];
+            if (bo.opened_values.size() != rd.dims.size()) return VGPU_REJECT_SHAPE;
             std::vector<Dim> lde_dims;
             uint64_t max_h = 0;
             for (auto& d : rd.dims) { lde_dims.push_back({d.w, d.h << LOG_BLOWUP}); max_h = std::max(max_h, d.h << LOG_BLOWUP); }
             std::vector<std::vector<uint32_t>> canon_rows;
-            for (auto& row : bo.rows_monty) { std::vector<uint32_t> c; for (uint32_t x : row) c.push_back(bb::from_monty(x)); canon_rows.push_back(std::move(c)); }
+            for (auto& row : bo.opened_values) { std::vector<uint32_t> c; for (uint32_t x : row) c.push_back(bb::from_monty(x)); canon_rows.push_back(std::move(c)); }
             const uint64_t batch_index = index >> (log_max_height - log2_ceil(max_h));
-            if (!merkle_verify_batch(rd.commit, lde_dims, batch_index, canon_rows, bo.path)) return VGPU_REJECT_INPUT_MERKLE;
+            if (!merkle_verify_batch(rd.commit, lde_dims, batch_index, canon_rows, bo.opening_proof)) return VGPU_REJECT_INPUT_MERKLE;
             for (size_t mi = 0; mi < rd.dims.size(); mi++) {
                 const int lh = log2_ceil(rd.dims[mi].h) + LOG_BLOWUP;
                 const uint32_t rev = bb::reverse_bits((uint32_t)(index >> (log_max_height - lh)), lh);
                 const uint32_t x = bb::mul(gen, bb::pow(bb::two_adic_generator_monty(lh), rev));
                 for (size_t pi = 0; pi < rd.points[mi].size(); pi++) {
                     const std::vector<E5>& at_z = *rd.values[mi][pi];
-                    if (at_z.size() != bo.rows_monty[mi].size()) return VGPU_REJECT_SHAPE;
+                    if (at_z.size() != bo.opened_values[mi].size()) return VGPU_REJECT_SHAPE;
                     const E5 den = bb::e5_add_base(bb::e5_neg(rd.points[mi][pi]), x);   // x - z
                     if (bb::e5_is_zero(den)) return VGPU_REJECT_SHAPE;
                     const E5 dinv = bb::e5_inv(den);
                     for (size_t c = 0; c < at_z.size(); c++) {
-                        const E5 quotient = bb::e5_mul(bb::e5_add_base(bb::e5_neg(at_z[c]), bo.rows_monty[mi][c]), dinv);   // (p(x) - p(z)) / (x - z)
+                        const E5 quotient = bb::e5_mul(bb::e5_add_base(bb::e5_neg(at_z[c]), bo.opened_values[mi][c]), dinv);   // (p(x) - p(z)) / (x - z)
                         ro[lh] = bb::e5_add(ro[lh], bb::e5_mul(apw[lh], quotient));
                         apw[lh] = bb::e5_mul(apw[lh], alpha);
                     }
@@ -257,8 +153,8 @@ int32_t verify_openings(const std::vector<RoundV>& rounds, const ProofV& pf, vgh
             }
         }
         // p3-fri verify_query
-        const std::vector<FriStepV>& steps = pf.fri_queries[q];
-        if (steps.size() != pf.fri_commits.size()) return VGPU_REJECT_SHAPE;
+        const std::vector<vgh::CommitPhaseStep>& steps = pf.query_proofs[q];
+        if (steps.size() != pf.commit_phase_commits.size()) return VGPU_REJECT_SHAPE;
         E5 folded = bb::e5_zero();
         uint32_t x = bb::pow(bb::two_adic_generator_monty(log_max_height), bb::reverse_bits((uint32_t)index, log_max_height));
         const uint32_t minus_one = bb::two_adic_generator_monty(1);
@@ -267,10 +163,10 @@ int32_t verify_openings(const std::vector<RoundV>& rounds, const ProofV& pf, vgh
             folded = bb::e5_add(folded, ro[lfh + 1]);
             const uint64_t sib = (index ^ 1) & 1, pair = index >> 1;
             E5 evals[2] = {folded, folded};
-            evals[sib] = steps[si].sibling;
+            evals[sib] = steps[si].sibling_value;
             std::vector<uint32_t> row(10);
             for (int e = 0; e < 2; e++) for (int l = 0; l < 5; l++) row[5 * e + l] = bb::from_monty(evals[e].c[l]);
-            if (!merkle_verify_batch(pf.fri_commits[si], {{10, 1ull << lfh}}, pair, {row}, steps[si].path)) return VGPU_REJECT_FRI_MERKLE;
+            if (!merkle_verify_batch(pf.commit_phase_commits[si], {{10, 1ull << lfh}}, pair, {row}, steps[si].opening_proof)) return VGPU_REJECT_FRI_MERKLE;
             uint32_t xs[2] = {x, x};
             xs[sib] = bb::mul(xs[sib], minus_one);
             // line through (xs[0], evals[0]), (xs[1], evals[1]) evaluated at beta; xs[1] - xs[0] = -2 xs[0]
@@ -297,13 +193,14 @@ extern "C" int32_t vgpu_verify(vgpu_ctx* ctx, const uint8_t* proof, uint64_t pro
     if (!ctx->challenger_set) VG_FAIL(ctx, "verify: vgpu_set_challenger has not been called");
     VG_TRY(vg_enter(ctx));
     *verdict = VGPU_REJECT_MALFORMED;
-    ProofV pf;
-    if (!decode(proof, proof_len, &pf)) return 0;
-    if (pf.chips.size() != (size_t)VGPU_NUM_CHIPS) { *verdict = VGPU_REJECT_SHAPE; return 0; }
-    for (auto& c : pf.chips) if (c.log_degree > (uint32_t)MAX_LOG_DEGREE || c.n_prep_local || c.n_prep_next) { *verdict = VGPU_REJECT_SHAPE; return 0; }
+    vgh::MachineProof pf;
+    if (!vgh::decode(proof, proof_len, &pf)) return 0;
+    const std::vector<vgh::ChipProof>& chips = pf.chip_proofs;
+    if (chips.size() != (size_t)VGPU_NUM_CHIPS) { *verdict = VGPU_REJECT_SHAPE; return 0; }
+    for (auto& c : chips) if (c.log_degree > (uint32_t)MAX_LOG_DEGREE || c.preprocessed_local.size() || c.preprocessed_next.size()) { *verdict = VGPU_REJECT_SHAPE; return 0; }
     // the two chips with preprocessed columns have the height of those columns (program ROM, range table): a proof may not
     // shrink them (an all-one-row proof has no FRI layers at all)
-    if ((1ull << pf.chips[1].log_degree) != prep[0].height || (1ull << pf.chips[12].log_degree) != prep[1].height) { *verdict = VGPU_REJECT_SHAPE; return 0; }
+    if ((1ull << chips[1].log_degree) != prep[0].height || (1ull << chips[12].log_degree) != prep[1].height) { *verdict = VGPU_REJECT_SHAPE; return 0; }
 
     vgh::Poseidon16 perm;
     perm.set(ctx->poseidon_rc, ctx->poseidon_has_mds ? ctx->poseidon_mds : nullptr);
@@ -321,38 +218,37 @@ extern "C" int32_t vgpu_verify(vgpu_ctx* ctx, const uint8_t* proof, uint64_t pro
         vgpu_prover_data_free(pd);
         ch.observe_digest_canonical(digest);
     }
-    ch.observe_digest_canonical(pf.main_commit.data());
+    ch.observe_digest_canonical(pf.main_trace.data());
     uint32_t perm_challenges[15];
     for (int i = 0; i < 3; i++) { E5 e = ch.sample_ext(); for (int l = 0; l < 5; l++) perm_challenges[5 * i + l] = bb::from_monty(e.c[l]); }
-    ch.observe_digest_canonical(pf.perm_commit.data());
+    ch.observe_digest_canonical(pf.perm_trace.data());
     const E5 alpha = ch.sample_ext();
-    ch.observe_digest_canonical(pf.quot_commit.data());
+    ch.observe_digest_canonical(pf.quotient_chunks.data());
     const E5 zeta = ch.sample_ext();
 
     std::vector<RoundV> rounds(3);
-    rounds[0].commit = pf.main_commit; rounds[1].commit = pf.perm_commit; rounds[2].commit = pf.quot_commit;
+    rounds[0].commit = pf.main_trace; rounds[1].commit = pf.perm_trace; rounds[2].commit = pf.quotient_chunks;
     for (int i = 0; i < VGPU_NUM_CHIPS; i++) {
         const vgpu_chip_desc* chip = vgpu_basic_machine_chip(i);
-        const ProofV::Chip& c = pf.chips[i];
+        const vgh::ChipProof& c = chips[i];
         const uint64_t h = 1ull << c.log_degree;
         const E5 zg = bb::e5_mul_base(zeta, bb::two_adic_generator_monty((int)c.log_degree));
         rounds[0].dims.push_back({chip->width, h});
         rounds[1].dims.push_back({5ull * (chip->n_interactions + 1), h});
         rounds[2].dims.push_back({10, h});
-        rounds[0].points.push_back({zeta, zg}); rounds[0].values.push_back({&c.ov.trace_local, &c.ov.trace_next});
-        rounds[1].points.push_back({zeta, zg}); rounds[1].values.push_back({&c.ov.perm_local, &c.ov.perm_next});
-        rounds[2].points.push_back({bb::e5_sqr(zeta)}); rounds[2].values.push_back({&c.ov.quotient_chunks});
+        rounds[0].points.push_back({zeta, zg}); rounds[0].values.push_back({&c.trace_local, &c.trace_next});
+        rounds[1].points.push_back({zeta, zg}); rounds[1].values.push_back({&c.permutation_local, &c.permutation_next});
+        rounds[2].points.push_back({bb::e5_sqr(zeta)}); rounds[2].values.push_back({&c.quotient_chunks});
     }
-    int32_t v = verify_openings(rounds, pf, ch);
+    int32_t v = verify_openings(rounds, pf.opening_proof, ch);
     if (v != VGPU_ACCEPT) { *verdict = v; return 0; }
     for (int i = 0; i < VGPU_NUM_CHIPS; i++) {
         bool ok = false;
-        VG_TRY(vg_verify_chip_constraints(ctx, vgpu_basic_machine_chip(i), pf.chips[i].log_degree, pf.chips[i].ov, pf.chips[i].cumulative_sum,
-                                          zeta, alpha, perm_challenges, &ok));
+        VG_TRY(vg_verify_chip_constraints(ctx, vgpu_basic_machine_chip(i), chips[i], zeta, alpha, perm_challenges, &ok));
         if (!ok) { *verdict = VGPU_REJECT_CONSTRAINTS_CHIP0 - i; return 0; }
     }
     E5 sum = bb::e5_zero();
-    for (auto& c : pf.chips) sum = bb::e5_add(sum, c.cumulative_sum);
+    for (auto& c : chips) sum = bb::e5_add(sum, c.cumulative_sum);
     if (!bb::e5_is_zero(sum)) { *verdict = VGPU_REJECT_CUMULATIVE_SUM; return 0; }
     *verdict = VGPU_ACCEPT;
     return 0;

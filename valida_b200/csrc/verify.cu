@@ -50,12 +50,13 @@ E5 unflatten(const E5* v, uint32_t m) {
 
 }  // namespace
 
-int32_t vg_verify_chip_constraints(vgpu_ctx* ctx, const vgpu_chip_desc* chip, uint32_t log_degree, const VgChipOpening& ov,
-                                   const E5& cumulative_sum, const E5& zeta, const E5& alpha, const uint32_t perm_challenges[15], bool* ok) {
+int32_t vg_verify_chip_constraints(vgpu_ctx* ctx, const vgpu_chip_desc* chip, const vgh::ChipProof& cp, const E5& zeta,
+                                   const E5& alpha, const uint32_t perm_challenges[15], bool* ok) {
     *ok = false;
+    const uint32_t log_degree = cp.log_degree;
     const uint32_t k = chip->n_interactions, pw = k + 1;
-    if (ov.trace_local.size() != chip->width || ov.trace_next.size() != chip->width) return 0;
-    if (ov.perm_local.size() != 5 * pw || ov.perm_next.size() != 5 * pw || ov.quotient_chunks.size() != 10) return 0;
+    if (cp.trace_local.size() != chip->width || cp.trace_next.size() != chip->width) return 0;
+    if (cp.permutation_local.size() != 5 * pw || cp.permutation_next.size() != 5 * pw || cp.quotient_chunks.size() != 10) return 0;
     DevChip dc;
     VG_TRY(vg_build_devchip(ctx, chip, perm_challenges, &dc));
     const uint32_t g_inv = bb::inv(bb::two_adic_generator_monty((int)log_degree));
@@ -63,7 +64,7 @@ int32_t vg_verify_chip_constraints(vgpu_ctx* ctx, const vgpu_chip_desc* chip, ui
     const E5 zm1 = bb::e5_sub_base(zeta, bb::R1), zmg = bb::e5_sub_base(zeta, g_inv);
     if (bb::e5_is_zero(zm1) || bb::e5_is_zero(zmg)) return 0;
     VerifierFolder f;
-    f.lrow = ov.trace_local.data(); f.nrow = ov.trace_next.data();
+    f.lrow = cp.trace_local.data(); f.nrow = cp.trace_next.data();
     f.first = X{bb::e5_mul(z_h, bb::e5_inv(zm1))};
     f.last = X{bb::e5_mul(z_h, bb::e5_inv(zmg))};
     f.trans = X{zmg};
@@ -71,7 +72,7 @@ int32_t vg_verify_chip_constraints(vgpu_ctx* ctx, const vgpu_chip_desc* chip, ui
     air::with_chip(chip->chip_id, [&](auto c) { air::eval_chip<decltype(c)::value>(f); });
     {   // eval_permutation_constraints
         std::vector<E5> pl(pw), pn(pw);
-        for (uint32_t m = 0; m < pw; m++) { pl[m] = unflatten(ov.perm_local.data(), m); pn[m] = unflatten(ov.perm_next.data(), m); }
+        for (uint32_t m = 0; m < pw; m++) { pl[m] = unflatten(cp.permutation_local.data(), m); pn[m] = unflatten(cp.permutation_next.data(), m); }
         E5 rhs = bb::e5_zero(), phi0 = bb::e5_zero();
         for (uint32_t m = 0; m < k; m++) {
             const DevInteraction& it = dc.interactions[m];
@@ -90,10 +91,10 @@ int32_t vg_verify_chip_constraints(vgpu_ctx* ctx, const vgpu_chip_desc* chip, ui
         }
         f.z_ext(bb::e5_mul(f.trans.e, bb::e5_sub(bb::e5_sub(pn[k], pl[k]), rhs)));
         f.z_ext(bb::e5_mul(f.first.e, bb::e5_sub(pl[k], phi0)));
-        f.z_ext(bb::e5_mul(f.last.e, bb::e5_sub(pl[k], cumulative_sum)));
+        f.z_ext(bb::e5_mul(f.last.e, bb::e5_sub(pl[k], cp.cumulative_sum)));
     }
     // quotient(zeta) = chunk_0(zeta^2) + zeta * chunk_1(zeta^2)   (log_quotient_degree = 1)
-    const E5 quot = bb::e5_add(unflatten(ov.quotient_chunks.data(), 0), bb::e5_mul(unflatten(ov.quotient_chunks.data(), 1), zeta));
+    const E5 quot = bb::e5_add(unflatten(cp.quotient_chunks.data(), 0), bb::e5_mul(unflatten(cp.quotient_chunks.data(), 1), zeta));
     const E5 want = bb::e5_mul(z_h, quot);
     bool same = true;
     for (int l = 0; l < 5; l++) same = same && (want.c[l] == f.acc.c[l]);

@@ -2,13 +2,8 @@
 // out-of-domain constraint check (verify.cu).
 #pragma once
 #include "ctx.h"
-#include <vector>
-
-struct VgChipOpening {   // OpenedValues of one ChipProof (machine/src/proof.rs:27-37), Montgomery limbs
-    std::vector<bb::E5> trace_local, trace_next, perm_local, perm_next, quotient_chunks;
-};
+#include "host/proof.h"
 
 // *ok = the folded constraints at zeta equal Z_H(zeta) * quotient(zeta).  Returns non-zero only on API errors.
-int32_t vg_verify_chip_constraints(vgpu_ctx* ctx, const vgpu_chip_desc* chip, uint32_t log_degree, const VgChipOpening& ov,
-                                   const bb::E5& cumulative_sum, const bb::E5& zeta, const bb::E5& alpha,
-                                   const uint32_t perm_challenges_canonical[15], bool* ok);
+int32_t vg_verify_chip_constraints(vgpu_ctx* ctx, const vgpu_chip_desc* chip, const vgh::ChipProof& cp, const bb::E5& zeta,
+                                   const bb::E5& alpha, const uint32_t perm_challenges_canonical[15], bool* ok);
