@@ -49,6 +49,10 @@ uint64_t vgpu_ctx_launch_count(const vgpu_ctx* ctx);
 /* Frees the device buffers the context keeps for reuse by its next calls (otherwise held until vgpu_ctx_destroy): after a
  * proof that filled most of the GPU's memory, this hands that memory back to other contexts and libraries. */
 int32_t vgpu_ctx_release_cached(vgpu_ctx* ctx);
+/* Device memory of the context, in bytes: out[0] = live (buffers in use), out[1] = peak live since the context was created or
+ * the last reset, out[2] = cached (freed buffers kept for reuse; vgpu_ctx_release_cached empties it), out[3] = peak live bytes
+ * of the symmetric heap of a split proof (0 without one).  reset != 0: the peaks restart from the current live bytes. */
+int32_t vgpu_ctx_memory_stats(vgpu_ctx* ctx, uint64_t out[4], int32_t reset);
 /* Optional per-kernel-class CUDA-event timing (event pairs on the context's stream around every launch).
  * vgpu_ctx_kernel_stats synchronises, drains the records and returns the number of classes written:
  * names[i] (static strings), launches, summed milliseconds and summed algorithmic bytes (DESIGN.md). */

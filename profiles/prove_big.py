@@ -16,11 +16,15 @@ print("tracegen %.1f s, heights" % (time.perf_counter() - t0), [m.shape[0] for m
 dm = [ctx.upload(m) for m in t.main]; dp = [ctx.upload(m) for m in t.preprocessed]
 ctx.synchronize()
 for i in range(3):
+    ctx.memory_stats(reset=True)
     t0 = time.perf_counter()
     proof = vb.prove_machine(cfg, t, device_resident=(dm, dp))
     dt = time.perf_counter() - t0
     print("prove %d: %.1f ms  %.2f Mrows/s  proof %d bytes" % (i, dt * 1e3, (1 << log_rows) / dt / 1e6, len(proof)), flush=True)
     print("  phases:", ["%s %.1f" % p for p in vb.last_prove_phases(ctx)], flush=True)
+    ms = ctx.memory_stats()
+    print("  memory (GB): live %.2f  peak live %.2f  cached %.2f  symmetric-heap peak %.2f"
+          % tuple(ms[k] / 1e9 for k in ("live", "peak", "cached", "symm_peak")), flush=True)
 t0 = time.perf_counter()
 vb.verify_machine(cfg, proof, t.preprocessed)
 print("verified in %.1f ms" % ((time.perf_counter() - t0) * 1e3))

@@ -90,6 +90,7 @@ extern "C" {
     pub fn vgpu_ctx_synchronize(ctx: *mut vgpu_ctx) -> i32;
     pub fn vgpu_ctx_launch_count(ctx: *const vgpu_ctx) -> u64;
     pub fn vgpu_ctx_release_cached(ctx: *mut vgpu_ctx) -> i32;
+    pub fn vgpu_ctx_memory_stats(ctx: *mut vgpu_ctx, out: *mut u64, reset: i32) -> i32;
     pub fn vgpu_ctx_set_kernel_timing(ctx: *mut vgpu_ctx, on: i32) -> i32;
     pub fn vgpu_ctx_kernel_stats(ctx: *mut vgpu_ctx, names: *mut *const c_char, launches: *mut u32, ms: *mut f32, bytes: *mut f64, cap: u32) -> u32;
     pub fn vgpu_set_challenger(ctx: *mut vgpu_ctx, round_constants: *const u32, mds_16x16_or_null: *const u32) -> i32;

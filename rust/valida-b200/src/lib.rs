@@ -169,6 +169,26 @@ impl Context {
     pub fn launch_count(&self) -> u64 {
         unsafe { sys::vgpu_ctx_launch_count(self.raw) }
     }
+
+    /// Device memory of this context in bytes; `reset` restarts both peaks from the current live bytes.
+    pub fn memory_stats(&mut self, reset: bool) -> Result<MemoryStats> {
+        let mut out = [0u64; 4];
+        self.check(unsafe { sys::vgpu_ctx_memory_stats(self.raw, out.as_mut_ptr(), reset as i32) })?;
+        Ok(MemoryStats { live: out[0], peak: out[1], cached: out[2], symm_peak: out[3] })
+    }
+}
+
+/// What [`Context::memory_stats`] returns.
+#[derive(Clone, Copy, Debug, PartialEq, Eq)]
+pub struct MemoryStats {
+    /// Buffers in use.
+    pub live: u64,
+    /// Peak of `live` since the context was created or the last reset.
+    pub peak: u64,
+    /// Freed buffers kept for reuse by later calls (emptied by `vgpu_ctx_release_cached`).
+    pub cached: u64,
+    /// Peak live bytes of the symmetric heap of a split proof (0 without one).
+    pub symm_peak: u64,
 }
 
 impl Drop for Context {

@@ -44,6 +44,7 @@ def _load():
         "vgpu_ctx_synchronize": (C.c_int32, [vp]),
         "vgpu_ctx_launch_count": (u64, [vp]),
         "vgpu_ctx_release_cached": (C.c_int32, [vp]),
+        "vgpu_ctx_memory_stats": (C.c_int32, [vp, C.POINTER(u64), C.c_int32]),
         "vgpu_ctx_set_kernel_timing": (C.c_int32, [vp, C.c_int32]),
         "vgpu_ctx_kernel_stats": (C.c_uint32, [vp, C.POINTER(C.c_char_p), u32p, C.POINTER(C.c_float), C.POINTER(C.c_double), C.c_uint32]),
         "vgpu_host_register": (C.c_int32, [vp, vp, u64]),
@@ -147,6 +148,14 @@ class Context:
     def release_cached(self):
         """Free the device buffers kept for reuse by later calls (e.g. after a proof that filled most of the GPU)."""
         self.check(lib().vgpu_ctx_release_cached(self._h))
+
+    def memory_stats(self, reset=False):
+        """Device memory of this context in bytes: {"live", "peak" (of live, since creation or the last reset), "cached" (freed
+        buffers kept for reuse; release_cached() empties it), "symm_peak" (symmetric heap of a split proof)}.  reset=True restarts
+        both peaks from the current live bytes."""
+        out = (C.c_uint64 * 4)()
+        self.check(lib().vgpu_ctx_memory_stats(self._h, out, 1 if reset else 0))
+        return dict(zip(("live", "peak", "cached", "symm_peak"), (int(v) for v in out)))
 
     @property
     def launch_count(self):

@@ -176,11 +176,16 @@ int32_t vgpu_ctx_release_cached(vgpu_ctx* ctx) {
     ctx->free_bufs.clear(); ctx->cached_bytes = 0;
     return 0;
 }
+int32_t vgpu_ctx_memory_stats(vgpu_ctx* ctx, uint64_t out[4], int32_t reset) {
+    out[0] = ctx->live_bytes; out[1] = ctx->peak_bytes; out[2] = ctx->cached_bytes; out[3] = ctx->symm_peak_bytes;
+    if (reset) { ctx->peak_bytes = ctx->live_bytes; ctx->symm_peak_bytes = ctx->symm_live_bytes; }
+    return 0;
+}
 
 int32_t vgpu_ctx_set_kernel_timing(vgpu_ctx* ctx, int32_t on) { ctx->ktiming = on != 0; return 0; }
 static const char* KCLASS_NAMES[KC_COUNT] = {"ntt_pass_kernel", "leaf_hash_kernel", "compress_layer_kernel", "fri_leaf_hash_kernel", "transpose (rm<->cm)",
                                              "perm trace kernels", "quotient_kernel", "inverse denominators", "bary_kernel", "reduced_opening_kernel", "fri_fold_kernel", "peer-store exchange", "all-gathers + barriers (incl. waiting for the slowest rank)", "other",
-                                             "check_kernel"};
+                                             "check_kernel", "query_path_kernel"};
 uint32_t vgpu_ctx_kernel_stats(vgpu_ctx* ctx, const char** names, uint32_t* launches, float* ms, double* bytes, uint32_t cap) {
     cudaStreamSynchronize(ctx->stream);
     uint32_t n[KC_COUNT] = {0}; float t[KC_COUNT] = {0}; double b[KC_COUNT] = {0};

@@ -26,7 +26,7 @@ __device__ __forceinline__ uint32_t vg_pow_lookup(const uint32_t* lo, const uint
 }
 
 // kernel classes for the optional per-launch CUDA-event timing (bench.py's roofline line)
-enum KClass { KC_NTT = 0, KC_LEAF_HASH, KC_COMPRESS, KC_FRI_LEAF, KC_TRANSPOSE, KC_PERM, KC_QUOTIENT, KC_INVDEN, KC_BARY, KC_REDUCED_OPENING, KC_FRI_FOLD, KC_EXCHANGE, KC_COLLECTIVE, KC_OTHER, KC_CHECK, KC_COUNT };
+enum KClass { KC_NTT = 0, KC_LEAF_HASH, KC_COMPRESS, KC_FRI_LEAF, KC_TRANSPOSE, KC_PERM, KC_QUOTIENT, KC_INVDEN, KC_BARY, KC_REDUCED_OPENING, KC_FRI_FOLD, KC_EXCHANGE, KC_COLLECTIVE, KC_OTHER, KC_CHECK, KC_TREE_PATH, KC_COUNT };
 struct KTimer { cudaEvent_t a, b; int cls; double bytes; };
 
 struct vgpu_ctx {

@@ -85,10 +85,12 @@ struct OpenScratch {
     uint32_t* d_sums = nullptr;
     RowVec current;
     std::vector<FriLayer> layers;
+    uint32_t* paths = nullptr;                  // the rebuilt lower levels of the query paths (vg_tree_paths)
     explicit OpenScratch(vgpu_ctx* c) : ctx(c) {}
     void drop_invden() { for (auto& kv : invden) vg_free(ctx, kv.second); invden.clear(); vg_free(ctx, d_sums); d_sums = nullptr; }
     ~OpenScratch() {
         drop_invden();
+        vg_free(ctx, paths);
         for (auto& r : ro) vg_free(ctx, r.d);
         vg_free(ctx, current.d);
         for (auto& L : layers) { vg_free(ctx, L.values.d); vg_tree_free(ctx, &L.tree); }
@@ -234,19 +236,44 @@ int32_t open_multi_batches(vgpu_ctx* ctx, const std::vector<OpenRound>& rounds, 
     for (auto& L : S.layers) per_query += 5 + 8 * (L.tree.layer_ptr.size() - 1);
     for (const OpenRound& rd : rounds) { for (auto* m : rd.pd->ldes) per_query += m->w; per_query += 8 * (size_t)log2u(rd.pd->max_height); }
     const long nq = (long)indices.size();
+    // the path levels below the kept tree layers: every tree's, of every query, rebuilt in one launch (merkle.h) — by the rank that
+    // reports the leaf, as for the stored levels; tree t of query qi writes slot qi * trees + t
+    std::vector<VgPathTree> trees;
+    for (const FriLayer& L : S.layers) trees.push_back({&L.tree, nullptr, L.values.d - L.values.begin, L.values.count});
+    for (const OpenRound& rd : rounds) trees.push_back({&rd.pd->tree, rd.pd, nullptr, 0});
+    auto leaf_of = [&](size_t t, uint64_t index) -> uint64_t {     // the leaf of tree t a query index opens
+        if (t < S.layers.size()) return index >> (t + 1);
+        return index >> (log_max - log2u(rounds[t - S.layers.size()].pd->max_height));
+    };
+    std::vector<VgPathReq> reqs;
+    for (long qi = 0; qi < nq; qi++)
+        for (size_t t = 0; t < trees.size(); t++) {
+            const uint64_t leaf = leaf_of(t, indices[qi]);
+            if (trees[t].tree->rebuilt() && trees[t].tree->reports(ctx, 0, leaf)) reqs.push_back({(uint32_t)t, (uint32_t)(qi * trees.size() + t), leaf});
+        }
+    VG_TRY(vg_tree_paths(ctx, trees, reqs, (size_t)nq * trees.size(), &S.paths));
+    const uint32_t* paths = S.paths;
     std::vector<const uint32_t*> ptrs(per_query * (size_t)nq);
 #pragma omp parallel for schedule(static) num_threads(8)
     for (long qi = 0; qi < nq; qi++) {
         const uint64_t index = indices[qi];
         const uint32_t** o = ptrs.data() + per_query * (size_t)qi;
         auto push_digest = [&](const uint32_t* d) { for (int k = 0; k < 8; k++) *o++ = d ? d + k : nullptr; };
+        auto push_path = [&](size_t t) {     // the sibling digests of tree t's path, leaf level first
+            const VgTree& tr = *trees[t].tree;
+            const uint64_t leaf = leaf_of(t, index);
+            const uint32_t* rebuilt = tr.reports(ctx, 0, leaf) ? paths + ((size_t)qi * trees.size() + t) * VG_TREE_DROP * 8 : nullptr;
+            for (size_t lvl = 0; lvl < tr.depth(); lvl++)
+                push_digest(lvl < tr.rebuilt() ? (rebuilt ? rebuilt + lvl * 8 : nullptr) : tr.node(ctx, lvl, (leaf >> lvl) ^ 1));
+        };
         for (size_t i = 0; i < S.layers.size(); i++) {
             const FriLayer& L = S.layers[i];
-            uint64_t index_i = index >> i, sib = index_i ^ 1, pair = index_i >> 1;
+            uint64_t sib = (index >> i) ^ 1;
             for (int l = 0; l < 5; l++) *o++ = L.values.at(ctx, l, sib);
-            for (size_t lvl = 0; lvl + 1 < L.tree.layer_ptr.size(); lvl++) push_digest(L.tree.node(ctx, lvl, (pair >> lvl) ^ 1));
+            push_path(i);
         }
-        for (const OpenRound& rd : rounds) {
+        for (size_t r = 0; r < rounds.size(); r++) {
+            const OpenRound& rd = rounds[r];
             int lg = log2u(rd.pd->max_height);
             uint64_t bidx = index >> (log_max - lg);
             for (auto* m : rd.pd->ldes) {
@@ -254,7 +281,7 @@ int32_t open_multi_batches(vgpu_ctx* ctx, const std::vector<OpenRound>& rounds, 
                 const bool mine = m->dist == VG_ROWS ? (row >= m->row0 && row < m->row0 + m->h) : (ctx->comm_rank == 0 || !vg_sharded(ctx));
                 for (uint64_t c = 0; c < m->w; c++) *o++ = mine ? m->d + c * m->col_stride + (row - m->row0) : nullptr;
             }
-            for (int lvl = 0; lvl < lg; lvl++) push_digest(rd.pd->tree.node(ctx, lvl, (bidx >> lvl) ^ 1));
+            push_path(S.layers.size() + r);
         }
     }
     std::vector<uint32_t> words;

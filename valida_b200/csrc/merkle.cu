@@ -9,12 +9,15 @@
 //    "inject shorter matrices" rule: node = compress(compress(l, r), hash(rows at that height)).
 //  * short layers (<= 2^15 nodes): tree_tail_kernel reduces a sub-tree per CTA in shared memory, a thread per node while a level is
 //    wide, a warp per node (the Keccak state spread over 25 lanes) on the last levels, where only the dependent chain is left.
-// Digests are stored canonical, 8 words (32 B) per node, all layers kept for the opening phase.  Split proof (merkle.h): a rank
+//  * query_path_kernel: a query's path below the kept layers (merkle.h), rebuilt from the leaves by one CTA per path.
+// Digests are stored canonical, 8 words (32 B) per node.  Every layer is computed, but only layers VG_TREE_DROP and up are kept for
+// the opening phase; the lower ones live in a transient block freed when the build returns.  Split proof (merkle.h): a rank
 // computes and keeps its run of every layer — the sub-tree over its rows — and only the layer of comm_size sub-roots is all-gathered.
 #include "ctx.h"
 #include "keccak.cuh"
 #include "merkle.h"
 #include <algorithm>
+#include <cstring>
 #include <numeric>
 
 namespace {
@@ -280,6 +283,73 @@ __global__ void __launch_bounds__(128) fri_leaf_hash_kernel(const uint32_t* __re
     o[1] = make_uint4(wrap_mod_p(d[4]), wrap_mod_p(d[5]), wrap_mod_p(d[6]), wrap_mod_p(d[7]));
 }
 
+// One tree whose lower paths query_path_kernel rebuilds (merkle.h, VgPathTree).  Input tree: cols[col_at[j] .. col_at[j + 1]) are
+// the columns (virtual row bases, as in hash_rows) of the rows hashed at level j — the leaves at j = 0, the rows injected above.
+struct PathTree {
+    const uint32_t* const* cols;        // null for a FRI tree
+    const uint32_t* fri_v;              // FRI tree: the layer's values, limb stride fri_cs
+    uint64_t fri_cs;
+    uint32_t col_at[VG_TREE_DROP + 1];
+    uint32_t levels;                    // rebuilt levels s: the sub-tree has 2^s leaves
+};
+constexpr int PATH_THREADS = 1 << VG_TREE_DROP;    // a thread per leaf of the largest sub-tree
+
+// A CTA per request: recomputes the 2^s-leaf sub-tree holding the leaf, level by level in shared memory, with the build's sponge
+// and compression, and writes the sibling of the leaf's path at every level below s.
+__global__ void __launch_bounds__(PATH_THREADS) query_path_kernel(const PathTree* __restrict__ trees, const VgPathReq* __restrict__ reqs, uint32_t* __restrict__ out) {
+    __shared__ uint4 buf[2][2 * PATH_THREADS];      // one level's digests (two uint4 each); levels alternate between the halves
+    const VgPathReq q = reqs[blockIdx.x];
+    const PathTree& T = trees[q.tree];
+    const uint32_t s = T.levels, t = threadIdx.x;
+    const uint64_t base = q.leaf >> s << s;         // first leaf of the sub-tree
+    const uint32_t* const* cols = T.cols;
+    if (t < (1u << s)) {
+        uint32_t d[8];
+        if (cols) {
+            const uint64_t r = base + t;
+            keccak256_words(T.col_at[1], [&](uint32_t i) { return bb::from_monty(__ldg(cols[i] + r)); }, d);
+        } else {   // fri_leaf_hash_kernel's leaf: the pair (v[2i], v[2i+1]) flattened to 10 words
+            const uint64_t i = base + t;
+            uint32_t w[10];
+#pragma unroll
+            for (int l = 0; l < 5; l++) {
+                const uint2 v = __ldg(reinterpret_cast<const uint2*>(T.fri_v + (uint64_t)l * T.fri_cs + 2 * i));
+                w[l] = bb::from_monty(v.x); w[5 + l] = bb::from_monty(v.y);
+            }
+            keccak256_words<true>(10, [&](uint32_t k) { return w[k]; }, d);
+        }
+        buf[0][2 * t] = make_uint4(wrap_mod_p(d[0]), wrap_mod_p(d[1]), wrap_mod_p(d[2]), wrap_mod_p(d[3]));
+        buf[0][2 * t + 1] = make_uint4(wrap_mod_p(d[4]), wrap_mod_p(d[5]), wrap_mod_p(d[6]), wrap_mod_p(d[7]));
+    }
+    __syncthreads();
+    uint32_t cur = 0;
+    for (uint32_t j = 0; j < s; j++) {
+        const uint32_t sib = (uint32_t)(((q.leaf >> j) ^ 1) - (base >> j));
+        if (t < 2) reinterpret_cast<uint4*>(out + ((uint64_t)q.slot * VG_TREE_DROP + j) * 8)[t] = buf[cur][2 * sib + t];
+        if (j + 1 == s) break;
+        if (t < (1u << (s - j - 1))) {       // node t of level j + 1
+            const uint4 a = buf[cur][4 * t], b = buf[cur][4 * t + 1], c = buf[cur][4 * t + 2], e = buf[cur][4 * t + 3];
+            uint32_t l[8] = {a.x, a.y, a.z, a.w, b.x, b.y, b.z, b.w}, r[8] = {c.x, c.y, c.z, c.w, e.x, e.y, e.z, e.w}, o[8];
+            compress_pair(l, r, o);
+            const uint32_t c0 = cols ? T.col_at[j + 1] : 0, nw = cols ? T.col_at[j + 2] - c0 : 0;
+            if (nw) {   // node = compress(compress(l, r), hash(rows of the matrices of this level's height))
+                const uint64_t row = (base >> (j + 1)) + t;
+                uint32_t h[8], o2[8];
+                keccak256_words(nw, [&](uint32_t i) { return bb::from_monty(__ldg(cols[c0 + i] + row)); }, h);
+#pragma unroll
+                for (int k = 0; k < 8; k++) h[k] = wrap_mod_p(h[k]);
+                compress_pair(o, h, o2);
+#pragma unroll
+                for (int k = 0; k < 8; k++) o[k] = o2[k];
+            }
+            buf[cur ^ 1][2 * t] = make_uint4(o[0], o[1], o[2], o[3]);
+            buf[cur ^ 1][2 * t + 1] = make_uint4(o[4], o[5], o[6], o[7]);
+        }
+        __syncthreads();
+        cur ^= 1;
+    }
+}
+
 }  // namespace
 
 // ---- host side: layer plan, launches --------------------------------------------------------------------------
@@ -299,13 +369,28 @@ static std::vector<LayerPlan> plan_tree(const vgpu_ctx* ctx, uint64_t leaves, bo
     }
     return plan;
 }
-static int32_t alloc_tree(vgpu_ctx* ctx, const std::vector<LayerPlan>& plan, VgTree* t) {
-    uint64_t total = 0;
-    for (auto& p : plan) total += p.scount;
-    VG_TRY(vg_alloc(ctx, (void**)&t->digests, total * 32));
+// The layers below VG_TREE_DROP (all but the root of a shorter tree) of a tree being built: a transient block, handed back to the
+// context's cache when the build returns (the kernels writing and reading it are already enqueued on the context's stream), and
+// the tree's pointers into it cleared.
+struct LowerLayers {
+    vgpu_ctx* ctx; VgTree* t; uint32_t* d = nullptr; size_t n = 0;
+    ~LowerLayers() { vg_free(ctx, d); for (size_t i = 0; i < n; i++) t->layer_ptr[i] = nullptr; }
+};
+static int32_t alloc_tree(vgpu_ctx* ctx, const std::vector<LayerPlan>& plan, VgTree* t, LowerLayers* low) {
+    const size_t keep = std::min(plan.size() - 1, VG_TREE_DROP);     // first kept layer
+    uint64_t kept = 0, dropped = 0;
+    for (size_t i = 0; i < plan.size(); i++) (i < keep ? dropped : kept) += plan[i].scount;
+    VG_TRY(vg_alloc(ctx, (void**)&t->digests, kept * 32));
+    if (dropped) VG_TRY(vg_alloc(ctx, (void**)&low->d, dropped * 32));
     t->layer_ptr.clear(); t->layer_len.clear(); t->layer_begin.clear(); t->layer_count.clear();
-    uint32_t* at = t->digests;
-    for (auto& p : plan) { t->layer_ptr.push_back(at); t->layer_len.push_back(p.len); t->layer_begin.push_back(p.sbegin); t->layer_count.push_back(p.scount); at += p.scount * 8; }
+    uint32_t* at[2] = {low->d, t->digests};
+    for (size_t i = 0; i < plan.size(); i++) {
+        const LayerPlan& p = plan[i];
+        uint32_t*& a = at[i >= keep];
+        t->layer_ptr.push_back(a); t->layer_len.push_back(p.len); t->layer_begin.push_back(p.sbegin); t->layer_count.push_back(p.scount);
+        a += p.scount * 8;
+    }
+    low->n = keep;
     return 0;
 }
 void vg_tree_free(vgpu_ctx* ctx, VgTree* t) { vg_free(ctx, t->digests); t->digests = nullptr; }
@@ -410,7 +495,8 @@ static int32_t build_upper_layers(vgpu_ctx* ctx, const std::vector<LayerPlan>& p
 // Single-matrix tree over ext5 pairs (p3-fri commit phase).
 int32_t vg_fri_layer_commit(vgpu_ctx* ctx, const uint32_t* v, uint64_t cs, uint64_t npairs, bool v_is_shard, VgTree* tree, uint32_t root_out[8]) {
     const std::vector<LayerPlan> plan = plan_tree(ctx, npairs, v_is_shard);
-    VG_TRY(alloc_tree(ctx, plan, tree));
+    LowerLayers low{ctx, tree};
+    VG_TRY(alloc_tree(ctx, plan, tree, &low));
     const LayerPlan& l0 = plan[0];
     {
         // v holds the pairs of this rank's run when it is a shard (the run IS the computed run), all pairs otherwise
@@ -437,7 +523,8 @@ int32_t vg_merkle_build(vgpu_ctx* ctx, vgpu_prover_data* pd, const std::vector<u
     if (max_h & (max_h - 1)) VG_FAIL(ctx, "commit: heights must be powers of two");
     pd->max_height = max_h;
     const std::vector<LayerPlan> plan = plan_tree(ctx, max_h, vg_split_rows(ctx, max_h));
-    VG_TRY(alloc_tree(ctx, plan, &pd->tree));
+    LowerLayers low{ctx, &pd->tree};
+    VG_TRY(alloc_tree(ctx, plan, &pd->tree, &low));
     size_t pos = 0;
     std::vector<size_t> idx;
     std::vector<const vgpu_dmat*> group;
@@ -472,5 +559,59 @@ int32_t vg_merkle_build(vgpu_ctx* ctx, vgpu_prover_data* pd, const std::vector<u
     if (pos != n) VG_FAIL(ctx, "commit: a matrix height does not match any tree layer");
     VG_CUDA(ctx, cudaMemcpyAsync(pd->root, pd->tree.layer_ptr.back(), 32, cudaMemcpyDeviceToHost, ctx->stream));
     VG_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
+    return 0;
+}
+
+// The lower levels of the requested paths (merkle.h): one upload of the tree table, the column pointers and the requests, one launch.
+int32_t vg_tree_paths(vgpu_ctx* ctx, const std::vector<VgPathTree>& trees, const std::vector<VgPathReq>& reqs, size_t slots, uint32_t** out) {
+    VG_TRY(vg_alloc(ctx, (void**)out, slots * VG_TREE_DROP * 32));
+    if (reqs.empty()) return 0;
+    std::vector<PathTree> pt(trees.size());
+    std::vector<const uint32_t*> cols;
+    std::vector<size_t> col_first(trees.size());  // input tree: its first entry of the column table
+    std::vector<double> bytes(trees.size());      // per request: the sub-tree's rows read, and the sibling digests written
+    for (size_t k = 0; k < trees.size(); k++) {
+        const VgPathTree& src = trees[k];
+        PathTree& p = pt[k];
+        p.levels = (uint32_t)src.tree->rebuilt();
+        bytes[k] = 32.0 * p.levels;
+        if (!src.pd) {
+            p.fri_v = src.fri_v; p.fri_cs = src.fri_cs;
+            bytes[k] += 40.0 * (1u << p.levels);
+            continue;
+        }
+        // the columns of level j in the build's order: the matrices of height max_h >> j, in the caller's order
+        col_first[k] = cols.size();
+        for (uint32_t j = 0; j < p.levels; j++) {
+            p.col_at[j] = (uint32_t)(cols.size() - col_first[k]);
+            for (const vgpu_dmat* m : src.pd->ldes) {
+                if (m->gh != src.pd->max_height >> j) continue;
+                for (uint64_t c = 0; c < m->w; c++) cols.push_back(m->d + c * m->col_stride - m->row0);
+                bytes[k] += 4.0 * m->w * (double)(1u << (p.levels - j));
+            }
+        }
+        p.col_at[p.levels] = (uint32_t)(cols.size() - col_first[k]);
+    }
+    // one device block: [trees][requests][column table]
+    const size_t tree_b = pt.size() * sizeof(PathTree), req_b = reqs.size() * sizeof(VgPathReq), col_b = cols.size() * sizeof(void*);
+    uint8_t* blk = nullptr;
+    VG_TRY(vg_alloc(ctx, (void**)&blk, tree_b + req_b + col_b));
+    const uint32_t* const* dcols = reinterpret_cast<const uint32_t* const*>(blk + tree_b + req_b);
+    for (size_t k = 0; k < pt.size(); k++)
+        if (trees[k].pd) pt[k].cols = dcols + col_first[k];
+    std::vector<uint8_t> host(tree_b + req_b + col_b);
+    std::memcpy(host.data(), pt.data(), tree_b);
+    std::memcpy(host.data() + tree_b, reqs.data(), req_b);
+    std::memcpy(host.data() + tree_b + req_b, cols.data(), col_b);
+    // cudaMemcpyAsync from pageable memory stages synchronously: `host` may go once the call returns
+    VG_CUDA(ctx, cudaMemcpyAsync(blk, host.data(), host.size(), cudaMemcpyHostToDevice, ctx->stream));
+    double total = 0;
+    for (const VgPathReq& r : reqs) total += bytes[r.tree];
+    {
+        KScope ks(ctx, KC_TREE_PATH, total);
+        query_path_kernel<<<(unsigned)reqs.size(), PATH_THREADS, 0, ctx->stream>>>(reinterpret_cast<const PathTree*>(blk), reinterpret_cast<const VgPathReq*>(blk + tree_b), *out);
+    }
+    vg_free(ctx, blk);
+    VG_LAUNCH_CHECK(ctx);
     return 0;
 }

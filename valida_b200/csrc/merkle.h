@@ -3,20 +3,36 @@
 // Split proof: a layer of more than comm_size nodes is cut into comm_size contiguous runs and a rank computes and KEEPS
 // only its run (its sub-tree); the layer of exactly comm_size nodes — the sub-roots — is all-gathered (comm_size x 32 bytes,
 // the only collective of a tree) and the layers above it are computed by every rank.
+// A tree keeps only its layers VG_TREE_DROP and up (only the root for a tree of depth VG_TREE_DROP or less): a query's path below
+// them is rebuilt from the leaves by vg_tree_paths.  The lower layers are the bulk of a tree (2^-VG_TREE_DROP of it is kept), and
+// a proof reads 40 paths from them.
 #pragma once
 #include "ctx.h"
+#include <algorithm>
 #include <functional>
 
+// 8: the kept layers are 1/256 of a tree, and a rebuilt path recomputes a 256-leaf sub-tree, one CTA of 256 threads with a thread per
+// leaf.  It must not exceed 11: a split tree's run has at least 2048 leaves per rank (a FRI layer of 4096 values per rank, in pairs),
+// so every dropped node lies inside one rank's run, and the sub-root layer that is all-gathered is never dropped.
+constexpr size_t VG_TREE_DROP = 8;
+
 struct VgTree {
-    uint32_t* digests = nullptr;           // the stored parts of all layers, leaf layer first
-    std::vector<uint32_t*> layer_ptr;      // layer_ptr[i] -> node layer_begin[i] of layer i
+    uint32_t* digests = nullptr;           // the stored parts of the kept layers
+    std::vector<uint32_t*> layer_ptr;      // layer_ptr[i] -> node layer_begin[i] of layer i; null for a dropped layer
     std::vector<uint64_t> layer_len;       // nodes of the whole layer
-    std::vector<uint64_t> layer_begin, layer_count;   // the run of nodes stored on this rank
-    // address of node `j` of layer `lvl` if THIS rank is the one that reports it in a query answer (the owner of a split
-    // layer's run; rank 0 for the layers every rank holds), else null
+    std::vector<uint64_t> layer_begin, layer_count;   // the run of nodes computed on this rank (and stored, if the layer is kept)
+    size_t depth() const { return layer_len.size() - 1; }
+    // the levels of an authentication path that are not stored: vg_tree_paths rebuilds them
+    size_t rebuilt() const { return std::min(depth(), VG_TREE_DROP); }
+    // whether THIS rank is the one that reports node `j` of layer `lvl` in a query answer (the owner of a split layer's run;
+    // rank 0 for the layers every rank holds)
+    bool reports(const vgpu_ctx* ctx, size_t lvl, uint64_t j) const {
+        if (layer_count[lvl] == layer_len[lvl]) return ctx->comm_rank == 0 || !vg_sharded(ctx);
+        return j >= layer_begin[lvl] && j < layer_begin[lvl] + layer_count[lvl];
+    }
+    // address of node `j` of a kept layer `lvl` if this rank reports it, else null
     const uint32_t* node(const vgpu_ctx* ctx, size_t lvl, uint64_t j) const {
-        if (layer_count[lvl] == layer_len[lvl]) return ctx->comm_rank == 0 || !vg_sharded(ctx) ? layer_ptr[lvl] + j * 8 : nullptr;
-        return j >= layer_begin[lvl] && j < layer_begin[lvl] + layer_count[lvl] ? layer_ptr[lvl] + (j - layer_begin[lvl]) * 8 : nullptr;
+        return reports(ctx, lvl, j) ? layer_ptr[lvl] + (j - layer_begin[lvl]) * 8 : nullptr;
     }
 };
 
@@ -38,3 +54,12 @@ int32_t vg_merkle_build(vgpu_ctx* ctx, vgpu_prover_data* pd, const std::vector<u
 // once the context's stream has been synchronised (the caller needs it for the transcript anyway).
 int32_t vg_fri_layer_commit(vgpu_ctx* ctx, const uint32_t* v, uint64_t cs, uint64_t npairs, bool v_is_shard, VgTree* tree, uint32_t root_out[8]);
 void vg_tree_free(vgpu_ctx* ctx, VgTree* t);
+
+// The leaves of a tree whose lower paths vg_tree_paths rebuilds: the rows of pd->ldes (an input tree, pd->tree), or the ext5
+// pairs of a FRI layer's values (fri_v: limb-major, limb stride fri_cs, addressed by the layer's global element index).
+struct VgPathTree { const VgTree* tree; const vgpu_prover_data* pd; const uint32_t* fri_v; uint64_t fri_cs; };
+struct VgPathReq { uint32_t tree, slot; uint64_t leaf; };
+// Enqueues ONE launch that writes, for every request, the sibling digests of levels 0 .. rebuilt() - 1 of leaf `leaf`'s path to
+// out[(slot * VG_TREE_DROP + lvl) * 8 ..]; out holds `slots` * VG_TREE_DROP digests (the caller frees it with vg_free).  Every
+// requested leaf must be one this rank reports (VgTree::reports at layer 0).
+int32_t vg_tree_paths(vgpu_ctx* ctx, const std::vector<VgPathTree>& trees, const std::vector<VgPathReq>& reqs, size_t slots, uint32_t** out);
