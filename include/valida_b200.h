@@ -62,6 +62,17 @@ uint32_t vgpu_ctx_kernel_stats(vgpu_ctx* ctx, const char** names, uint32_t* laun
  * (basic/src/bin/valida.rs:360-365,382,397): 480 round constants (canonical), 16x16 MDS matrix
  * row-major or NULL for CosetMds<_,16>::default(). */
 int32_t vgpu_set_challenger(vgpu_ctx* ctx, const uint32_t round_constants[480], const uint32_t* mds_16x16_or_null);
+/* The hash of the Merkle trees (the MMCS of StarkConfig::Pcs) used by the calls that follow: vgpu_commit_batches[_host], vgpu_open
+ * (its FRI layer trees and query paths), vgpu_prove, vgpu_prove_device and vgpu_verify (the re-commit of the preprocessed traces and
+ * every Merkle check).
+ *   VGPU_MERKLE_KECCAK256 (default): FieldMerkleTreeMmcs<_, SerializingHasher32<Keccak256Hash>, CompressionFunctionFromHasher<_, _, 2, 8>, 8>.
+ *   VGPU_MERKLE_POSEIDON16: FieldMerkleTreeMmcs<_, PaddingFreeSponge<Perm16, 16, 8, 8>, TruncatedPermutation<Perm16, 2, 8, 16>, 8> over
+ *     the challenger's Poseidon-16 instance (vgpu_set_challenger must come first: a commit before it is an error).
+ * A prover data handle keeps the hash it was built with; vgpu_open refuses a round built under another.  Digests are 8 canonical
+ * words either way, so the proof format does not change.  Unknown values are an error.  Every rank of a split proof makes the call. */
+#define VGPU_MERKLE_KECCAK256 0
+#define VGPU_MERKLE_POSEIDON16 1
+int32_t vgpu_ctx_set_merkle_hash(vgpu_ctx* ctx, int32_t hash);
 
 /* ---- caller memory: page-lock the buffers that vgpu_prove / vgpu_commit_batches_host read (RowMajorMatrix<Val>.values of the traces), so
  * that their host-to-device copies run asynchronously and overlap the commits; without it the CUDA runtime stages each copy and the call

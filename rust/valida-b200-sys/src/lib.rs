@@ -18,6 +18,9 @@ pub const VGPU_MAX_TERMS: usize = 4;
 pub const VGPU_MAX_FIELDS: usize = 14;
 pub const VGPU_MAX_INTERACTIONS: usize = 5;
 pub const VGPU_COMM_ID_BYTES: usize = 128;
+/// Merkle tree hash of [`vgpu_ctx_set_merkle_hash`]: Keccak-256 (the default) or the challenger's Poseidon-16.
+pub const VGPU_MERKLE_KECCAK256: i32 = 0;
+pub const VGPU_MERKLE_POSEIDON16: i32 = 1;
 
 pub const VGPU_ACCEPT: i32 = 0;
 pub const VGPU_REJECT_MALFORMED: i32 = -1;
@@ -94,6 +97,7 @@ extern "C" {
     pub fn vgpu_ctx_set_kernel_timing(ctx: *mut vgpu_ctx, on: i32) -> i32;
     pub fn vgpu_ctx_kernel_stats(ctx: *mut vgpu_ctx, names: *mut *const c_char, launches: *mut u32, ms: *mut f32, bytes: *mut f64, cap: u32) -> u32;
     pub fn vgpu_set_challenger(ctx: *mut vgpu_ctx, round_constants: *const u32, mds_16x16_or_null: *const u32) -> i32;
+    pub fn vgpu_ctx_set_merkle_hash(ctx: *mut vgpu_ctx, hash: i32) -> i32;
 
     // ---- caller memory ----
     pub fn vgpu_host_register(ctx: *mut vgpu_ctx, p: *const c_void, bytes: u64) -> i32;

@@ -54,6 +54,25 @@ impl Repr {
     }
 }
 
+/// The hash of the Merkle trees (the `ValMmcs` of the `StarkConfig`), chosen with [`Context::set_merkle_hash`].
+#[derive(Clone, Copy, Debug, PartialEq, Eq)]
+pub enum MerkleHash {
+    /// `FieldMerkleTreeMmcs<Val, SerializingHasher32<Keccak256Hash>, CompressionFunctionFromHasher<_, _, 2, 8>, 8>` (the default).
+    Keccak256,
+    /// `FieldMerkleTreeMmcs<Val, PaddingFreeSponge<Perm16, 16, 8, 8>, TruncatedPermutation<Perm16, 2, 8, 16>, 8>` over the
+    /// challenger's Poseidon-16 instance.
+    Poseidon16,
+}
+
+impl MerkleHash {
+    fn raw(self) -> i32 {
+        match self {
+            MerkleHash::Keccak256 => sys::VGPU_MERKLE_KECCAK256,
+            MerkleHash::Poseidon16 => sys::VGPU_MERKLE_POSEIDON16,
+        }
+    }
+}
+
 /// A borrowed row-major matrix of field words (`RowMajorMatrix<Val>`).
 #[derive(Clone, Copy)]
 pub struct MatrixView<'a> {
@@ -126,6 +145,13 @@ impl Context {
     pub fn set_challenger(&mut self, round_constants: &[u32; 480], mds: Option<&[u32; 256]>) -> Result<()> {
         let mds_ptr = mds.map_or(ptr::null(), |m| m.as_ptr());
         self.check(unsafe { sys::vgpu_set_challenger(self.raw, round_constants.as_ptr(), mds_ptr) })
+    }
+
+    /// The Merkle tree hash of the commits, openings, proofs and verifications that follow.  `Poseidon16` uses the instance of
+    /// [`Context::set_challenger`], which must come first.  Proof bytes keep their format; a proof verifies only under the hash
+    /// it was made with.
+    pub fn set_merkle_hash(&mut self, hash: MerkleHash) -> Result<()> {
+        self.check(unsafe { sys::vgpu_ctx_set_merkle_hash(self.raw, hash.raw()) })
     }
 
     /// Debug mode of [`Context::prove_bytes`] (off by default): every chip's constraints on every trace row and the cumulative sums

@@ -6,6 +6,8 @@ Context without a CUDA device raises.
 """
 from .api import (  # noqa: F401
     BABYBEAR_P,
+    MERKLE_KECCAK256,
+    MERKLE_POSEIDON16,
     Context,
     DeviceMatrix,
     ProverData,

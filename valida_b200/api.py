@@ -17,6 +17,7 @@ import numpy as np
 BABYBEAR_P = 2013265921
 REPR_CANONICAL, REPR_MONTY_R32 = 0, 1
 NUM_CHIPS = 14
+MERKLE_KECCAK256, MERKLE_POSEIDON16 = 0, 1     # vgpu_ctx_set_merkle_hash
 
 _HERE = os.path.dirname(os.path.abspath(__file__))
 lib_path = os.path.join(_HERE, "libvalida_b200.so")
@@ -68,6 +69,7 @@ def _load():
         "vgpu_check_constraints": (C.c_int32, [vp, vp, vp, vp, vp, u32p, C.POINTER(C.c_int64), u32p, C.POINTER(u64)]),
         "vgpu_ctx_set_debug_checks": (C.c_int32, [vp, C.c_int32]),
         "vgpu_set_challenger": (C.c_int32, [vp, u32p, u32p]),
+        "vgpu_ctx_set_merkle_hash": (C.c_int32, [vp, C.c_int32]),
         "vgpu_challenger_reset": (C.c_int32, [vp]),
         "vgpu_challenger_observe": (C.c_int32, [vp, u32p, C.c_uint32]),
         "vgpu_challenger_sample_ext": (C.c_int32, [vp, u32p]),
@@ -169,10 +171,17 @@ class Context:
         before committing to a proof; a bad witness raises VgpuError naming each failing chip, row and constraint."""
         self.check(lib().vgpu_ctx_set_debug_checks(self._h, 1 if on else 0))
 
+    def set_merkle_hash(self, hash):
+        """The Merkle tree hash of the commits, openings, proofs and verifications that follow on this context:
+        MERKLE_KECCAK256 (the default) or MERKLE_POSEIDON16 (PaddingFreeSponge / TruncatedPermutation over the challenger's
+        Poseidon-16, which StarkConfig must have set first).  Proof bytes keep their format; a proof verifies only under the
+        hash it was made with.  Every rank of a split proof makes the same call."""
+        self.check(lib().vgpu_ctx_set_merkle_hash(self._h, int(hash)))
+
     def kernel_stats(self):
         """[(kernel class, launches, total ms, algorithmic bytes)] since the last call (synchronises)."""
-        names = (C.c_char_p * 16)(); ln = (C.c_uint32 * 16)(); ms = (C.c_float * 16)(); by = (C.c_double * 16)()
-        n = lib().vgpu_ctx_kernel_stats(self._h, names, ln, ms, by, 16)
+        names = (C.c_char_p * 32)(); ln = (C.c_uint32 * 32)(); ms = (C.c_float * 32)(); by = (C.c_double * 32)()
+        n = lib().vgpu_ctx_kernel_stats(self._h, names, ln, ms, by, 32)
         return [(names[i].decode(), int(ln[i]), float(ms[i]), float(by[i])) for i in range(n)]
 
     # ---- multi-GPU: one rank per GPU (include/valida_b200.h, "multi-GPU") ----

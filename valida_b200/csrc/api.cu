@@ -183,9 +183,16 @@ int32_t vgpu_ctx_memory_stats(vgpu_ctx* ctx, uint64_t out[4], int32_t reset) {
 }
 
 int32_t vgpu_ctx_set_kernel_timing(vgpu_ctx* ctx, int32_t on) { ctx->ktiming = on != 0; return 0; }
+int32_t vgpu_ctx_set_merkle_hash(vgpu_ctx* ctx, int32_t hash) {
+    if (!ctx) return -1;
+    if (hash != VGPU_MERKLE_KECCAK256 && hash != VGPU_MERKLE_POSEIDON16) VG_FAIL(ctx, "set_merkle_hash: unknown hash %d", hash);
+    ctx->merkle_hash = hash;
+    return 0;
+}
 static const char* KCLASS_NAMES[KC_COUNT] = {"ntt_pass_kernel", "leaf_hash_kernel", "compress_layer_kernel", "fri_leaf_hash_kernel", "transpose (rm<->cm)",
                                              "perm trace kernels", "quotient_kernel", "inverse denominators", "bary_kernel", "reduced_opening_kernel", "fri_fold_kernel", "peer-store exchange", "all-gathers + barriers (incl. waiting for the slowest rank)", "other",
-                                             "check_kernel", "query_path_kernel"};
+                                             "check_kernel", "query_path_kernel", "p16_leaf_kernel", "p16_layer_kernel + p16_tail_kernel", "p16_fri_leaf_kernel",
+                                             "p16_path_kernel"};
 uint32_t vgpu_ctx_kernel_stats(vgpu_ctx* ctx, const char** names, uint32_t* launches, float* ms, double* bytes, uint32_t cap) {
     cudaStreamSynchronize(ctx->stream);
     uint32_t n[KC_COUNT] = {0}; float t[KC_COUNT] = {0}; double b[KC_COUNT] = {0};
@@ -446,6 +453,7 @@ static int32_t extend_split(vgpu_ctx* ctx, vgpu_prover_data* pd, const vgpu_dmat
 int32_t vgpu_commit_batches(vgpu_ctx* ctx, const vgpu_dmat* const* mats, uint32_t n, const uint32_t* coset_shifts_or_null,
                             uint32_t digest_out[8], vgpu_prover_data** out) {
     VG_TRY(vg_enter(ctx));
+    if (ctx->merkle_hash == VGPU_MERKLE_POSEIDON16 && !ctx->challenger_set) VG_FAIL(ctx, "commit: the Poseidon-16 Merkle hash needs vgpu_set_challenger first");
     vgpu_prover_data* pd = new (std::nothrow) vgpu_prover_data();
     if (!pd) VG_FAIL(ctx, "out of host memory");
     pd->ctx = ctx;

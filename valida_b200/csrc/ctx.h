@@ -26,7 +26,8 @@ __device__ __forceinline__ uint32_t vg_pow_lookup(const uint32_t* lo, const uint
 }
 
 // kernel classes for the optional per-launch CUDA-event timing (bench.py's roofline line)
-enum KClass { KC_NTT = 0, KC_LEAF_HASH, KC_COMPRESS, KC_FRI_LEAF, KC_TRANSPOSE, KC_PERM, KC_QUOTIENT, KC_INVDEN, KC_BARY, KC_REDUCED_OPENING, KC_FRI_FOLD, KC_EXCHANGE, KC_COLLECTIVE, KC_OTHER, KC_CHECK, KC_TREE_PATH, KC_COUNT };
+enum KClass { KC_NTT = 0, KC_LEAF_HASH, KC_COMPRESS, KC_FRI_LEAF, KC_TRANSPOSE, KC_PERM, KC_QUOTIENT, KC_INVDEN, KC_BARY, KC_REDUCED_OPENING, KC_FRI_FOLD, KC_EXCHANGE, KC_COLLECTIVE, KC_OTHER, KC_CHECK, KC_TREE_PATH,
+             KC_P16_LEAF, KC_P16_COMPRESS, KC_P16_FRI_LEAF, KC_P16_PATH, KC_COUNT };   // KC_P16_*: the Poseidon-16 Merkle kernels (merkle.cu)
 struct KTimer { cudaEvent_t a, b; int cls; double bytes; };
 
 struct vgpu_ctx {
@@ -47,6 +48,7 @@ struct vgpu_ctx {
     void* challenger = nullptr;                                  // vgh::Challenger* (host/challenger.h)
     void* poseidon = nullptr;                                    // vgh::Poseidon16*
     uint32_t* d_poseidon = nullptr;                              // device copy of the round constants + MDS (pow.cu), dropped when they change
+    int32_t merkle_hash = VGPU_MERKLE_KECCAK256;                 // the MMCS hash of the commits and Merkle checks that follow (vgpu_ctx_set_merkle_hash)
     std::vector<std::pair<const char*, float>> phases;          // last prove: per-phase milliseconds
     struct PhaseMark { const char* name; cudaEvent_t a, b; };
     std::vector<PhaseMark> phase_marks;                         // event pairs of the last prove (read by vgpu_last_prove_phases)
@@ -138,6 +140,8 @@ int32_t vg_enter(vgpu_ctx* ctx);                          // make ctx->device cu
 int32_t vg_alloc(vgpu_ctx* ctx, void** p, size_t bytes);
 void vg_free(vgpu_ctx* ctx, void* p);
 int32_t vg_dmat_alloc(vgpu_ctx* ctx, uint64_t h, uint64_t w, vgpu_dmat** out);
+// pow.cu: the context's Poseidon-16 constants on the device (poseidon.cuh layout), uploaded on first use; an error before vgpu_set_challenger
+int32_t vg_poseidon_consts(vgpu_ctx* ctx, uint32_t** out);
 int32_t vg_get_shift_table(vgpu_ctx* ctx, uint32_t shift_canonical, uint32_t scale_canonical, uint64_t max_exp, const PowTable** out);
 
 // host/comm.cc — every rank calls these in the same order with the same sizes

@@ -411,6 +411,7 @@ int32_t vgpu_open(vgpu_ctx* ctx, const vgpu_prover_data* const* rounds, uint32_t
     size_t mi = 0, pi = 0;
     for (uint32_t r = 0; r < n_rounds; r++) {
         if (!rounds[r]) VG_FAIL(ctx, "open: round %u has no prover data", r);
+        if (rounds[r]->tree.hash != ctx->merkle_hash) VG_FAIL(ctx, "open: round %u was committed with another Merkle hash than the context's", r);
         rds[r].pd = rounds[r];
         for (size_t m = 0; m < rounds[r]->ldes.size(); m++, mi++) {
             std::vector<E5> pts;

@@ -73,12 +73,41 @@ Digest compress2(const Digest& l, const Digest& r) {
     return hash_canonical_words(w);
 }
 
+// The Poseidon-16 MMCS (VGPU_MERKLE_POSEIDON16) on the challenger's permutation.  PaddingFreeSponge<Perm16, 16, 8, 8>: state zero,
+// each chunk of 8 words overwrites state[0 .. len) and is followed by a permutation, digest = state[0 .. 8).
+Digest p16_hash(const vgh::Poseidon16& perm, const std::vector<uint32_t>& w) {
+    uint32_t s[16] = {0};
+    for (size_t i = 0; i < w.size(); i += 8) {
+        for (size_t k = 0; k < 8 && i + k < w.size(); k++) s[k] = bb::to_monty(w[i + k]);
+        perm.permute(s);
+    }
+    Digest d;
+    for (int k = 0; k < 8; k++) d[k] = bb::from_monty(s[k]);
+    return d;
+}
+// TruncatedPermutation<Perm16, 2, 8, 16>: permute(l || r)[0 .. 8)
+Digest p16_compress(const vgh::Poseidon16& perm, const Digest& l, const Digest& r) {
+    uint32_t s[16];
+    for (int k = 0; k < 8; k++) { s[k] = bb::to_monty(l[k]); s[8 + k] = bb::to_monty(r[k]); }
+    perm.permute(s);
+    Digest d;
+    for (int k = 0; k < 8; k++) d[k] = bb::from_monty(s[k]);
+    return d;
+}
+
+// The context's MMCS: Keccak-256 when p16 is null, else Poseidon-16 over *p16.  Digests and words are canonical.
+struct Mmcs {
+    const vgh::Poseidon16* p16 = nullptr;
+    Digest hash(const std::vector<uint32_t>& w) const { return p16 ? p16_hash(*p16, w) : hash_canonical_words(w); }
+    Digest compress(const Digest& l, const Digest& r) const { return p16 ? p16_compress(*p16, l, r) : compress2(l, r); }
+};
+
 int log2_ceil(uint64_t n) { int l = 0; while ((1ull << l) < n) l++; return l; }
 
 // FieldMerkleTreeMmcs::verify_batch [P3-UNVERIFIED; SURVEY App. A item 8]: matrices sorted by height (stable, tallest
 // first); rows of equal padded height are hashed together; a shorter group is injected when the running height reaches it.
 struct Dim { uint64_t w, h; };
-bool merkle_verify_batch(const Digest& commit, const std::vector<Dim>& dims, uint64_t index,
+bool merkle_verify_batch(const Mmcs& mmcs, const Digest& commit, const std::vector<Dim>& dims, uint64_t index,
                          const std::vector<std::vector<uint32_t>>& opened_canonical, const std::vector<Digest>& path) {
     if (dims.empty() || dims.size() != opened_canonical.size()) return false;
     std::vector<size_t> order;
@@ -91,13 +120,13 @@ bool merkle_verify_batch(const Digest& commit, const std::vector<Dim>& dims, uin
     auto group = [&](int lvl) {
         std::vector<uint32_t> cat;
         while (pos < order.size() && log2_ceil(dims[order[pos]].h) == lvl) { auto& r = opened_canonical[order[pos]]; cat.insert(cat.end(), r.begin(), r.end()); pos++; }
-        return hash_canonical_words(cat);
+        return mmcs.hash(cat);
     };
     Digest node = group(level);
     for (const Digest& sib : path) {
-        node = (index & 1) ? compress2(sib, node) : compress2(node, sib);
+        node = (index & 1) ? mmcs.compress(sib, node) : mmcs.compress(node, sib);
         index >>= 1; level--;
-        if (pos < order.size() && log2_ceil(dims[order[pos]].h) == level) node = compress2(node, group(level));
+        if (pos < order.size() && log2_ceil(dims[order[pos]].h) == level) node = mmcs.compress(node, group(level));
     }
     return pos == order.size() && node == commit;
 }
@@ -105,7 +134,7 @@ bool merkle_verify_batch(const Digest& commit, const std::vector<Dim>& dims, uin
 struct RoundV { Digest commit; std::vector<Dim> dims; std::vector<std::vector<E5>> points; std::vector<std::vector<const std::vector<E5>*>> values; };
 
 // TwoAdicFriPcs::verify_multi_batches + p3-fri verifier; 0 = accept, otherwise the verdict code of include/valida_b200.h
-int32_t verify_openings(const std::vector<RoundV>& rounds, const vgh::PcsProof& pf, vgh::Challenger& ch) {
+int32_t verify_openings(const Mmcs& mmcs, const std::vector<RoundV>& rounds, const vgh::PcsProof& pf, vgh::Challenger& ch) {
     const E5 alpha = ch.sample_ext();
     std::vector<E5> betas;
     for (const Digest& c : pf.commit_phase_commits) { ch.observe_digest_canonical(c.data()); betas.push_back(ch.sample_ext()); }
@@ -133,7 +162,7 @@ int32_t verify_openings(const std::vector<RoundV>& rounds, const vgh::PcsProof& 
             std::vector<std::vector<uint32_t>> canon_rows;
             for (auto& row : bo.opened_values) { std::vector<uint32_t> c; for (uint32_t x : row) c.push_back(bb::from_monty(x)); canon_rows.push_back(std::move(c)); }
             const uint64_t batch_index = index >> (log_max_height - log2_ceil(max_h));
-            if (!merkle_verify_batch(rd.commit, lde_dims, batch_index, canon_rows, bo.opening_proof)) return VGPU_REJECT_INPUT_MERKLE;
+            if (!merkle_verify_batch(mmcs, rd.commit, lde_dims, batch_index, canon_rows, bo.opening_proof)) return VGPU_REJECT_INPUT_MERKLE;
             for (size_t mi = 0; mi < rd.dims.size(); mi++) {
                 const int lh = log2_ceil(rd.dims[mi].h) + LOG_BLOWUP;
                 const uint32_t rev = bb::reverse_bits((uint32_t)(index >> (log_max_height - lh)), lh);
@@ -166,7 +195,7 @@ int32_t verify_openings(const std::vector<RoundV>& rounds, const vgh::PcsProof& 
             evals[sib] = steps[si].sibling_value;
             std::vector<uint32_t> row(10);
             for (int e = 0; e < 2; e++) for (int l = 0; l < 5; l++) row[5 * e + l] = bb::from_monty(evals[e].c[l]);
-            if (!merkle_verify_batch(pf.commit_phase_commits[si], {{10, 1ull << lfh}}, pair, {row}, steps[si].opening_proof)) return VGPU_REJECT_FRI_MERKLE;
+            if (!merkle_verify_batch(mmcs, pf.commit_phase_commits[si], {{10, 1ull << lfh}}, pair, {row}, steps[si].opening_proof)) return VGPU_REJECT_FRI_MERKLE;
             uint32_t xs[2] = {x, x};
             xs[sib] = bb::mul(xs[sib], minus_one);
             // line through (xs[0], evals[0]), (xs[1], evals[1]) evaluated at beta; xs[1] - xs[0] = -2 xs[0]
@@ -240,7 +269,9 @@ extern "C" int32_t vgpu_verify(vgpu_ctx* ctx, const uint8_t* proof, uint64_t pro
         rounds[1].points.push_back({zeta, zg}); rounds[1].values.push_back({&c.permutation_local, &c.permutation_next});
         rounds[2].points.push_back({bb::e5_sqr(zeta)}); rounds[2].values.push_back({&c.quotient_chunks});
     }
-    int32_t v = verify_openings(rounds, pf.opening_proof, ch);
+    Mmcs mmcs;
+    if (ctx->merkle_hash == VGPU_MERKLE_POSEIDON16) mmcs.p16 = &perm;
+    int32_t v = verify_openings(mmcs, rounds, pf.opening_proof, ch);
     if (v != VGPU_ACCEPT) { *verdict = v; return 0; }
     for (int i = 0; i < VGPU_NUM_CHIPS; i++) {
         bool ok = false;

@@ -10,12 +10,14 @@
 //  * short layers (<= 2^15 nodes): tree_tail_kernel reduces a sub-tree per CTA in shared memory, a thread per node while a level is
 //    wide, a warp per node (the Keccak state spread over 25 lanes) on the last levels, where only the dependent chain is left.
 //  * query_path_kernel: a query's path below the kept layers (merkle.h), rebuilt from the leaves by one CTA per path.
+// With VGPU_MERKLE_POSEIDON16 the p16_* kernels take the place of each of these, with the same plan, layout and launches.
 // Digests are stored canonical, 8 words (32 B) per node.  Every layer is computed, but only layers VG_TREE_DROP and up are kept for
 // the opening phase; the lower ones live in a transient block freed when the build returns.  Split proof (merkle.h): a rank
 // computes and keeps its run of every layer — the sub-tree over its rows — and only the layer of comm_size sub-roots is all-gathered.
 #include "ctx.h"
 #include "keccak.cuh"
 #include "merkle.h"
+#include "poseidon.cuh"
 #include <algorithm>
 #include <cstring>
 #include <numeric>
@@ -350,6 +352,207 @@ __global__ void __launch_bounds__(PATH_THREADS) query_path_kernel(const PathTree
     }
 }
 
+// ---- Poseidon-16 MMCS (VGPU_MERKLE_POSEIDON16) --------------------------------------------------------------------------------
+// The same trees with FieldMerkleTreeMmcs<_, PaddingFreeSponge<Perm16, 16, 8, 8>, TruncatedPermutation<Perm16, 2, 8, 16>, 8> over
+// the challenger's permutation (poseidon.cuh).  Each kernel below mirrors the Keccak kernel above it in indexing, virtual bases,
+// shard runs and injection; the permutation runs on Montgomery words, so the leaves absorb the LDE words as stored and only the
+// eight digest words are converted to canonical.  Every CTA first copies the 736 constants to shared memory.
+
+// PaddingFreeSponge: state zero; each chunk of 8 words overwrites state[0 .. len) and is followed by one permutation (ceil(n / 8)
+// in all, none extra when 8 divides n); the digest is state[0 .. 8)
+template <class Fetch>
+__device__ __forceinline__ void p16_sponge(const uint32_t nwords, Fetch fetch, const uint32_t* sc, uint32_t out[8]) {
+    uint32_t s[16];
+#pragma unroll
+    for (int i = 0; i < 16; i++) s[i] = 0;
+    for (uint32_t b = 0; b < nwords; b += 8) {
+#pragma unroll
+        for (int i = 0; i < 8; i++) if (b + i < nwords) s[i] = fetch(b + i);
+        p16::permute(s, sc, sc + p16::RC_WORDS);
+    }
+#pragma unroll
+    for (int i = 0; i < 8; i++) out[i] = bb::from_monty(s[i]);
+}
+// TruncatedPermutation: permute(l || r)[0 .. 8); digests are canonical in and out
+__device__ __forceinline__ void p16_compress(const uint32_t l[8], const uint32_t r[8], const uint32_t* sc, uint32_t out[8]) {
+    uint32_t s[16];
+#pragma unroll
+    for (int i = 0; i < 8; i++) { s[i] = bb::to_monty(l[i]); s[8 + i] = bb::to_monty(r[i]); }
+    p16::permute(s, sc, sc + p16::RC_WORDS);
+#pragma unroll
+    for (int i = 0; i < 8; i++) out[i] = bb::from_monty(s[i]);
+}
+__device__ __forceinline__ void store_digest(uint32_t* at, const uint32_t d[8]) {
+    uint4* o = reinterpret_cast<uint4*>(at);
+    o[0] = make_uint4(d[0], d[1], d[2], d[3]);
+    o[1] = make_uint4(d[4], d[5], d[6], d[7]);
+}
+__device__ __forceinline__ void load_digest(const uint32_t* at, uint32_t d[8]) {
+    const uint4* q = reinterpret_cast<const uint4*>(at);
+    const uint4 e = __ldg(q), f = __ldg(q + 1);
+    d[0] = e.x; d[1] = e.y; d[2] = e.z; d[3] = e.w; d[4] = f.x; d[5] = f.y; d[6] = f.z; d[7] = f.w;
+}
+
+// word k of FRI leaf i: limb k % 5 of element 2i + k / 5 (v limb-major, limb stride cs)
+__device__ __forceinline__ uint32_t fri_word(const uint32_t* __restrict__ v, uint64_t cs, uint64_t i, uint32_t k) {
+    return __ldg(v + (uint64_t)(k % 5) * cs + 2 * i + k / 5);
+}
+
+// leaf_hash_kernel: a thread per row of [row0, row0 + nrows), the concatenated row read through the column table
+__global__ void __launch_bounds__(128) p16_leaf_kernel(const uint32_t* const* __restrict__ colptr, uint32_t nwords, uint64_t row0, uint64_t nrows,
+                                                      uint32_t* __restrict__ digests, const uint32_t* __restrict__ consts) {
+    __shared__ uint32_t sc[p16::CONST_WORDS];
+    p16::load_consts(sc, consts);
+    __syncthreads();
+    uint64_t r = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
+    if (r >= nrows) return;
+    r += row0;
+    uint32_t d[8];
+    p16_sponge(nwords, [&](uint32_t i) { return __ldg(colptr[i] + r); }, sc, d);
+    store_digest(digests + r * 8, d);
+}
+
+// compress_layer_kernel: next[i] = compress(prev[2i], prev[2i+1]), then compress(next[i], inject[i]) when a shorter group joins
+__global__ void __launch_bounds__(128) p16_layer_kernel(const uint32_t* __restrict__ prev, const uint32_t* __restrict__ inject, uint64_t i0, uint64_t n_next,
+                                                       uint32_t* __restrict__ next, const uint32_t* __restrict__ consts) {
+    __shared__ uint32_t sc[p16::CONST_WORDS];
+    p16::load_consts(sc, consts);
+    __syncthreads();
+    uint64_t i = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= n_next) return;
+    i += i0;
+    uint32_t l[8], r[8], o[8];
+    load_digest(prev + i * 16, l);
+    load_digest(prev + i * 16 + 8, r);
+    p16_compress(l, r, sc, o);
+    if (inject) {
+        load_digest(inject + i * 8, r);
+        p16_compress(o, r, sc, l);
+#pragma unroll
+        for (int k = 0; k < 8; k++) o[k] = l[k];
+    }
+    store_digest(next + i * 8, o);
+}
+
+// tree_tail_kernel's fused short layers (same TailParams, same launch shape), a thread per node on every level
+__global__ void __launch_bounds__(TAIL_THREADS) p16_tail_kernel(const __grid_constant__ TailParams p, const uint32_t* __restrict__ consts) {
+    __shared__ uint4 buf_a[2 * TAIL_SUB * 2];
+    __shared__ uint4 buf_b[TAIL_SUB * 2];
+    __shared__ uint32_t sc[p16::CONST_WORDS];
+    p16::load_consts(sc, consts);
+    const uint64_t node0 = p.first_begin + (uint64_t)blockIdx.x * p.sub;
+    {
+        const uint4* src = reinterpret_cast<const uint4*>(p.prev_v + 2 * node0 * 8);
+        for (uint32_t i = threadIdx.x; i < 4 * p.sub; i += TAIL_THREADS) buf_a[i] = __ldg(src + i);
+    }
+    __syncthreads();
+    uint4* cur = buf_a; uint4* nxt = buf_b;
+    for (uint32_t k = 0; k < p.levels; k++) {
+        const uint32_t n = p.sub >> k;
+        const uint64_t base = node0 >> k;
+        for (uint32_t t = threadIdx.x; t < n; t += TAIL_THREADS) {
+            const uint4 a = cur[4 * t], b = cur[4 * t + 1], c = cur[4 * t + 2], d = cur[4 * t + 3];
+            uint32_t l[8] = {a.x, a.y, a.z, a.w, b.x, b.y, b.z, b.w}, r[8] = {c.x, c.y, c.z, c.w, d.x, d.y, d.z, d.w}, o[8];
+            p16_compress(l, r, sc, o);
+            if (p.inj_v[k]) {
+                load_digest(p.inj_v[k] + (base + t) * 8, r);
+                p16_compress(o, r, sc, l);
+#pragma unroll
+                for (int i = 0; i < 8; i++) o[i] = l[i];
+            }
+            const uint4 w0 = make_uint4(o[0], o[1], o[2], o[3]), w1 = make_uint4(o[4], o[5], o[6], o[7]);
+            nxt[2 * t] = w0; nxt[2 * t + 1] = w1;
+            uint4* g = reinterpret_cast<uint4*>(p.next_v[k] + (base + t) * 8);
+            g[0] = w0; g[1] = w1;
+        }
+        __syncthreads();
+        uint4* tmp = cur; cur = nxt; nxt = tmp;
+    }
+}
+
+// fri_leaf_hash_kernel: the pair (v[2i], v[2i+1]) of ext5 values flattened to 10 base words, two permutations
+__global__ void __launch_bounds__(128) p16_fri_leaf_kernel(const uint32_t* __restrict__ v, uint64_t cs, uint64_t i0, uint64_t npairs, uint32_t* __restrict__ digests,
+                                                          const uint32_t* __restrict__ consts) {
+    __shared__ uint32_t sc[p16::CONST_WORDS];
+    p16::load_consts(sc, consts);
+    __syncthreads();
+    uint64_t i = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= npairs) return;
+    i += i0;
+    uint32_t d[8];
+    p16_sponge(10, [&](uint32_t k) { return fri_word(v, cs, i, k); }, sc, d);
+    store_digest(digests + i * 8, d);
+}
+
+// query_path_kernel with the Poseidon-16 sponge and compression: a CTA per request rebuilds the 2^s-leaf sub-tree holding the leaf.
+// A node of a level is one to ceil(nw / 8) + 2 permutations (compression; the sponge of the injected row and the second compression)
+// run by ONE loop around ONE inlined permutation: each inlined copy costs ~2k instructions of registers and code.
+__global__ void __launch_bounds__(PATH_THREADS) p16_path_kernel(const PathTree* __restrict__ trees, const VgPathReq* __restrict__ reqs, uint32_t* __restrict__ out,
+                                                               const uint32_t* __restrict__ consts) {
+    __shared__ uint4 buf[2][2 * PATH_THREADS];
+    __shared__ uint32_t sc[p16::CONST_WORDS];
+    p16::load_consts(sc, consts);
+    const VgPathReq q = reqs[blockIdx.x];
+    const PathTree& T = trees[q.tree];
+    const uint32_t s = T.levels, t = threadIdx.x;
+    const uint64_t base = q.leaf >> s << s;
+    const uint32_t* const* cols = T.cols;
+    __syncthreads();
+    if (t < (1u << s)) {
+        uint32_t d[8];
+        if (cols) {
+            const uint64_t r = base + t;
+            p16_sponge(T.col_at[1], [&](uint32_t i) { return __ldg(cols[i] + r); }, sc, d);
+        } else {   // p16_fri_leaf_kernel's leaf
+            p16_sponge(10, [&](uint32_t k) { return fri_word(T.fri_v, T.fri_cs, base + t, k); }, sc, d);
+        }
+        buf[0][2 * t] = make_uint4(d[0], d[1], d[2], d[3]);
+        buf[0][2 * t + 1] = make_uint4(d[4], d[5], d[6], d[7]);
+    }
+    __syncthreads();
+    uint32_t cur = 0;
+    for (uint32_t j = 0; j < s; j++) {
+        const uint32_t sib = (uint32_t)(((q.leaf >> j) ^ 1) - (base >> j));
+        if (t < 2) reinterpret_cast<uint4*>(out + ((uint64_t)q.slot * VG_TREE_DROP + j) * 8)[t] = buf[cur][2 * sib + t];
+        if (j + 1 == s) break;
+        if (t < (1u << (s - j - 1))) {       // node t of level j + 1
+            const uint32_t c0 = cols ? T.col_at[j + 1] : 0, nw = cols ? T.col_at[j + 2] - c0 : 0;
+            const uint64_t row = (base >> (j + 1)) + t;
+            const uint32_t chunks = (nw + 7) / 8, steps = nw ? chunks + 2 : 1;
+            const uint32_t* kids = reinterpret_cast<const uint32_t*>(&buf[cur][4 * t]);
+            uint32_t st[16], o[8];       // o: the first compression's output (Montgomery)
+            for (uint32_t k = 0; k < steps; k++) {
+                if (k == 0) {                        // compress(left, right)
+#pragma unroll
+                    for (int i = 0; i < 16; i++) st[i] = bb::to_monty(kids[i]);
+                } else if (k <= chunks) {            // sponge of the rows injected at this level
+                    if (k == 1) {
+#pragma unroll
+                        for (int i = 0; i < 16; i++) st[i] = 0;
+                    }
+                    const uint32_t w0 = (k - 1) * 8;
+#pragma unroll
+                    for (int i = 0; i < 8; i++) if (w0 + i < nw) st[i] = __ldg(cols[c0 + w0 + i] + row);
+                } else {                             // compress(node, row digest)
+#pragma unroll
+                    for (int i = 0; i < 8; i++) { st[8 + i] = st[i]; st[i] = o[i]; }
+                }
+                p16::permute(st, sc, sc + p16::RC_WORDS);
+                if (k == 0) {
+#pragma unroll
+                    for (int i = 0; i < 8; i++) o[i] = st[i];
+                }
+            }
+#pragma unroll
+            for (int i = 0; i < 8; i++) o[i] = bb::from_monty(st[i]);
+            buf[cur ^ 1][2 * t] = make_uint4(o[0], o[1], o[2], o[3]);
+            buf[cur ^ 1][2 * t + 1] = make_uint4(o[4], o[5], o[6], o[7]);
+        }
+        __syncthreads();
+        cur ^= 1;
+    }
+}
+
 }  // namespace
 
 // ---- host side: layer plan, launches --------------------------------------------------------------------------
@@ -397,14 +600,17 @@ void vg_tree_free(vgpu_ctx* ctx, VgTree* t) { vg_free(ctx, t->digests); t->diges
 
 // digest of rows [row0, row0 + nrows) of the concatenated matrices, written to digests_v[row * 8] (digests_v is a VIRTUAL
 // base: the stored run starts at its first row).  A row shard contributes its local rows through a base shifted likewise.
-static int32_t hash_rows(vgpu_ctx* ctx, const std::vector<const vgpu_dmat*>& mats, uint64_t row0, uint64_t nrows, uint32_t* digests_v) {
+// p16: Poseidon-16 sponge (always through a column table in global memory), else Keccak-256.
+static int32_t hash_rows(vgpu_ctx* ctx, bool p16, const std::vector<const vgpu_dmat*>& mats, uint64_t row0, uint64_t nrows, uint32_t* digests_v) {
     std::vector<const uint32_t*> cols;
     for (auto* m : mats) {
         if (m->dist == VG_ROWS && (row0 < m->row0 || row0 + nrows > m->row0 + m->h)) VG_FAIL(ctx, "commit: rows [%llu, +%llu) are not in this rank's shard", (unsigned long long)row0, (unsigned long long)nrows);
         for (uint64_t c = 0; c < m->w; c++) cols.push_back(m->d + c * m->col_stride - m->row0);
     }
     const uint32_t nwords = (uint32_t)cols.size(), nblocks = nwords / RATE_WORDS + 1, grid = (uint32_t)((nrows + 127) / 128);
-    if (nblocks <= LEAF_NB_MAX) {
+    uint32_t* consts = nullptr;
+    if (p16) VG_TRY(vg_poseidon_consts(ctx, &consts));
+    if (!p16 && nblocks <= LEAF_NB_MAX) {
         LeafCols lc{};
         std::copy(cols.begin(), cols.end(), lc.col);
         {
@@ -420,8 +626,9 @@ static int32_t hash_rows(vgpu_ctx* ctx, const std::vector<const vgpu_dmat*>& mat
     // cudaMemcpyAsync from pageable memory stages synchronously: `cols` may go once the call returns
     VG_CUDA(ctx, cudaMemcpyAsync(dcols, cols.data(), cols.size() * sizeof(void*), cudaMemcpyHostToDevice, ctx->stream));
     {
-        KScope ks(ctx, KC_LEAF_HASH, (double)nrows * (4.0 * nwords + 32.0));
-        leaf_hash_kernel<<<grid, 128, 0, ctx->stream>>>(dcols, nwords, row0, nrows, digests_v);
+        KScope ks(ctx, p16 ? KC_P16_LEAF : KC_LEAF_HASH, (double)nrows * (4.0 * nwords + 32.0));
+        if (p16) p16_leaf_kernel<<<grid, 128, 0, ctx->stream>>>(dcols, nwords, row0, nrows, digests_v, consts);
+        else leaf_hash_kernel<<<grid, 128, 0, ctx->stream>>>(dcols, nwords, row0, nrows, digests_v);
     }
     VG_LAUNCH_CHECK(ctx);
     vg_free(ctx, dcols);
@@ -435,6 +642,9 @@ static int32_t hash_rows(vgpu_ctx* ctx, const std::vector<const vgpu_dmat*>& mat
 constexpr uint64_t TAIL_FUSE = 1u << 15;
 template <class Inject>
 static int32_t build_upper_layers(vgpu_ctx* ctx, const std::vector<LayerPlan>& plan, VgTree* t, uint32_t* inject_buf, Inject inject) {
+    const bool p16 = t->hash == VGPU_MERKLE_POSEIDON16;
+    uint32_t* consts = nullptr;
+    if (p16) VG_TRY(vg_poseidon_consts(ctx, &consts));
     if (plan[0].gather) VG_TRY(vg_comm_allgather_inplace(ctx, t->layer_ptr[0], 8));
     size_t lvl = 1;
     while (lvl < plan.size()) {
@@ -465,8 +675,9 @@ static int32_t build_upper_layers(vgpu_ctx* ctx, const std::vector<LayerPlan>& p
             }
             tp.levels = n;
             {
-                KScope ks(ctx, KC_COMPRESS, bytes);
-                tree_tail_kernel<<<(unsigned)(p.ccount / tp.sub), TAIL_THREADS, 0, ctx->stream>>>(tp);
+                KScope ks(ctx, p16 ? KC_P16_COMPRESS : KC_COMPRESS, bytes);
+                if (p16) p16_tail_kernel<<<(unsigned)(p.ccount / tp.sub), TAIL_THREADS, 0, ctx->stream>>>(tp, consts);
+                else tree_tail_kernel<<<(unsigned)(p.ccount / tp.sub), TAIL_THREADS, 0, ctx->stream>>>(tp);
             }
             VG_LAUNCH_CHECK(ctx);
             lvl += n;
@@ -482,8 +693,9 @@ static int32_t build_upper_layers(vgpu_ctx* ctx, const std::vector<LayerPlan>& p
             if (have) inj_v = buf_v;
         }
         {
-            KScope ks(ctx, KC_COMPRESS, (double)p.ccount * (inj_v ? 128.0 : 96.0));
-            compress_layer_kernel<<<(unsigned)((p.ccount + 127) / 128), 128, 0, ctx->stream>>>(prev_v, inj_v, p.cbegin, p.ccount, next_v);
+            KScope ks(ctx, p16 ? KC_P16_COMPRESS : KC_COMPRESS, (double)p.ccount * (inj_v ? 128.0 : 96.0));
+            if (p16) p16_layer_kernel<<<(unsigned)((p.ccount + 127) / 128), 128, 0, ctx->stream>>>(prev_v, inj_v, p.cbegin, p.ccount, next_v, consts);
+            else compress_layer_kernel<<<(unsigned)((p.ccount + 127) / 128), 128, 0, ctx->stream>>>(prev_v, inj_v, p.cbegin, p.ccount, next_v);
         }
         VG_LAUNCH_CHECK(ctx);
         if (p.gather) VG_TRY(vg_comm_allgather_inplace(ctx, t->layer_ptr[lvl], 8));
@@ -497,12 +709,18 @@ int32_t vg_fri_layer_commit(vgpu_ctx* ctx, const uint32_t* v, uint64_t cs, uint6
     const std::vector<LayerPlan> plan = plan_tree(ctx, npairs, v_is_shard);
     LowerLayers low{ctx, tree};
     VG_TRY(alloc_tree(ctx, plan, tree, &low));
+    tree->hash = ctx->merkle_hash;
+    const bool p16 = tree->hash == VGPU_MERKLE_POSEIDON16;
+    uint32_t* consts = nullptr;
+    if (p16) VG_TRY(vg_poseidon_consts(ctx, &consts));
     const LayerPlan& l0 = plan[0];
     {
         // v holds the pairs of this rank's run when it is a shard (the run IS the computed run), all pairs otherwise
         const uint32_t* v_v = v_is_shard ? v - 2 * l0.cbegin : v;
-        KScope ks(ctx, KC_FRI_LEAF, (double)l0.ccount * 72.0);
-        fri_leaf_hash_kernel<<<(unsigned)((l0.ccount + 127) / 128), 128, 0, ctx->stream>>>(v_v, cs, l0.cbegin, l0.ccount, tree->layer_ptr[0] - l0.sbegin * 8);
+        KScope ks(ctx, p16 ? KC_P16_FRI_LEAF : KC_FRI_LEAF, (double)l0.ccount * 72.0);
+        const unsigned grid = (unsigned)((l0.ccount + 127) / 128);
+        if (p16) p16_fri_leaf_kernel<<<grid, 128, 0, ctx->stream>>>(v_v, cs, l0.cbegin, l0.ccount, tree->layer_ptr[0] - l0.sbegin * 8, consts);
+        else fri_leaf_hash_kernel<<<grid, 128, 0, ctx->stream>>>(v_v, cs, l0.cbegin, l0.ccount, tree->layer_ptr[0] - l0.sbegin * 8);
     }
     VG_LAUNCH_CHECK(ctx);
     VG_TRY(build_upper_layers(ctx, plan, tree, nullptr, [](size_t, const LayerPlan&, uint32_t*, bool*) { return 0; }));
@@ -525,6 +743,8 @@ int32_t vg_merkle_build(vgpu_ctx* ctx, vgpu_prover_data* pd, const std::vector<u
     const std::vector<LayerPlan> plan = plan_tree(ctx, max_h, vg_split_rows(ctx, max_h));
     LowerLayers low{ctx, &pd->tree};
     VG_TRY(alloc_tree(ctx, plan, &pd->tree, &low));
+    pd->tree.hash = ctx->merkle_hash;
+    const bool p16 = pd->tree.hash == VGPU_MERKLE_POSEIDON16;
     size_t pos = 0;
     std::vector<size_t> idx;
     std::vector<const vgpu_dmat*> group;
@@ -540,7 +760,7 @@ int32_t vg_merkle_build(vgpu_ctx* ctx, vgpu_prover_data* pd, const std::vector<u
         return 0;
     };
     VG_TRY(take(max_h));
-    VG_TRY(hash_rows(ctx, group, plan[0].cbegin, plan[0].ccount, pd->tree.layer_ptr[0] - plan[0].sbegin * 8));
+    VG_TRY(hash_rows(ctx, p16, group, plan[0].cbegin, plan[0].ccount, pd->tree.layer_ptr[0] - plan[0].sbegin * 8));
     uint32_t* inject_buf = nullptr;
     if (pos < n) {
         // one layer's row digests at a time — except inside a fused run of short layers, where the digests of every injecting
@@ -551,7 +771,7 @@ int32_t vg_merkle_build(vgpu_ctx* ctx, vgpu_prover_data* pd, const std::vector<u
     int32_t rc = build_upper_layers(ctx, plan, &pd->tree, inject_buf, [&](size_t, const LayerPlan& p, uint32_t* buf_v, bool* have) -> int32_t {
         VG_TRY(take(p.len));
         *have = !group.empty();
-        if (*have) VG_TRY(hash_rows(ctx, group, p.cbegin, p.ccount, buf_v));
+        if (*have) VG_TRY(hash_rows(ctx, p16, group, p.cbegin, p.ccount, buf_v));
         return 0;
     });
     if (inject_buf) vg_free(ctx, inject_buf);
@@ -566,6 +786,11 @@ int32_t vg_merkle_build(vgpu_ctx* ctx, vgpu_prover_data* pd, const std::vector<u
 int32_t vg_tree_paths(vgpu_ctx* ctx, const std::vector<VgPathTree>& trees, const std::vector<VgPathReq>& reqs, size_t slots, uint32_t** out) {
     VG_TRY(vg_alloc(ctx, (void**)out, slots * VG_TREE_DROP * 32));
     if (reqs.empty()) return 0;
+    const bool p16 = trees[0].tree->hash == VGPU_MERKLE_POSEIDON16;
+    for (const VgPathTree& t : trees)
+        if (t.tree->hash != trees[0].tree->hash) VG_FAIL(ctx, "tree paths: the trees of one request were built with different hashes");
+    uint32_t* consts = nullptr;
+    if (p16) VG_TRY(vg_poseidon_consts(ctx, &consts));
     std::vector<PathTree> pt(trees.size());
     std::vector<const uint32_t*> cols;
     std::vector<size_t> col_first(trees.size());  // input tree: its first entry of the column table
@@ -608,8 +833,11 @@ int32_t vg_tree_paths(vgpu_ctx* ctx, const std::vector<VgPathTree>& trees, const
     double total = 0;
     for (const VgPathReq& r : reqs) total += bytes[r.tree];
     {
-        KScope ks(ctx, KC_TREE_PATH, total);
-        query_path_kernel<<<(unsigned)reqs.size(), PATH_THREADS, 0, ctx->stream>>>(reinterpret_cast<const PathTree*>(blk), reinterpret_cast<const VgPathReq*>(blk + tree_b), *out);
+        KScope ks(ctx, p16 ? KC_P16_PATH : KC_TREE_PATH, total);
+        const PathTree* dt = reinterpret_cast<const PathTree*>(blk);
+        const VgPathReq* dr = reinterpret_cast<const VgPathReq*>(blk + tree_b);
+        if (p16) p16_path_kernel<<<(unsigned)reqs.size(), PATH_THREADS, 0, ctx->stream>>>(dt, dr, *out, consts);
+        else query_path_kernel<<<(unsigned)reqs.size(), PATH_THREADS, 0, ctx->stream>>>(dt, dr, *out);
     }
     vg_free(ctx, blk);
     VG_LAUNCH_CHECK(ctx);

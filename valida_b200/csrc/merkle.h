@@ -17,6 +17,7 @@
 constexpr size_t VG_TREE_DROP = 8;
 
 struct VgTree {
+    int32_t hash = VGPU_MERKLE_KECCAK256;  // the hash it was built with (vgpu_ctx_set_merkle_hash)
     uint32_t* digests = nullptr;           // the stored parts of the kept layers
     std::vector<uint32_t*> layer_ptr;      // layer_ptr[i] -> node layer_begin[i] of layer i; null for a dropped layer
     std::vector<uint64_t> layer_len;       // nodes of the whole layer

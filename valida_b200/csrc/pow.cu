@@ -1,20 +1,19 @@
 // K11 — proof-of-work grinding on the device: DuplexChallenger::grind(bits) of p3-challenger as used by p3-fri's prover
 // (FriConfig{proof_of_work_bits: 8}, basic/src/bin/valida.rs:385-390) [P3-UNVERIFIED: the reference searches with rayon's
 // find_any and may return any witness; this search returns the SMALLEST one, which the verifier's check_witness accepts
-// like any other].  One thread per candidate: overlay the candidate on the sponge state, run Poseidon-16 (alpha = 5,
-// 4 + 22 + 4 rounds, dense 16 x 16 MDS taken from shared memory as broadcast reads), test the low bits of the last lane.
+// like any other].  One thread per candidate: overlay the candidate on the sponge state, run Poseidon-16 (poseidon.cuh,
+// constants from shared memory as broadcast reads), test the low bits of the last lane.
 // ~2000 candidates cost one launch (~50 us) where the host search took ~3 ms of otherwise idle GPU time per proof.
 #include "ctx.h"
+#include "poseidon.cuh"
 #include "host/challenger.h"
 
 namespace {
 
-__device__ __forceinline__ uint32_t sbox5(uint32_t x) { const uint32_t x2 = bb::sqr(x), x4 = bb::sqr(x2); return bb::mul(x4, x); }
-
 __global__ void __launch_bounds__(256) pow_grind_kernel(const uint32_t* __restrict__ consts /* 480 rc + 256 mds, Montgomery */, const uint32_t* __restrict__ base_state,
                                                        uint32_t slot, uint32_t w0, uint32_t count, uint32_t mask, uint32_t* __restrict__ result) {
-    __shared__ uint32_t sc[480 + 256];
-    for (uint32_t i = threadIdx.x; i < 480 + 256; i += blockDim.x) sc[i] = consts[i];
+    __shared__ uint32_t sc[p16::CONST_WORDS];
+    p16::load_consts(sc, consts);
     __syncthreads();
     const uint32_t gid = blockIdx.x * blockDim.x + threadIdx.x;
     if (gid >= count) return;
@@ -24,45 +23,36 @@ __global__ void __launch_bounds__(256) pow_grind_kernel(const uint32_t* __restri
     for (int i = 0; i < 16; i++) s[i] = base_state[i];
 #pragma unroll
     for (int i = 0; i < 16; i++) if ((uint32_t)i == slot) s[i] = bb::to_monty(w);
-    const uint32_t* rc = sc;
-    const uint32_t* mds = sc + 480;
-#pragma unroll 1
-    for (int round = 0; round < 30; round++) {
-#pragma unroll
-        for (int i = 0; i < 16; i++) s[i] = bb::add(s[i], rc[round * 16 + i]);
-        if (round >= 4 && round < 26) s[0] = sbox5(s[0]);
-        else {
-#pragma unroll
-            for (int i = 0; i < 16; i++) s[i] = sbox5(s[i]);
-        }
-        uint32_t o[16];
-#pragma unroll
-        for (int i = 0; i < 16; i++) {
-            uint64_t acc = 0;
-#pragma unroll
-            for (int j = 0; j < 16; j++) { acc = bb::madw(mds[i * 16 + j], s[j], acc); if ((j & 3) == 3) acc = bb::lazy_fold(acc); }
-            o[i] = bb::monty_reduce64(acc);
-        }
-#pragma unroll
-        for (int i = 0; i < 16; i++) s[i] = o[i];
-    }
+    p16::permute(s, sc, sc + p16::RC_WORDS);
     if ((bb::from_monty(s[15]) & mask) == 0) atomicMin(result, w);
 }
 
 }  // namespace
 
-// Smallest canonical witness w with check_witness(bits, w); the challenger is advanced exactly as grind() would.
-int32_t vg_pow_grind(vgpu_ctx* ctx, vgh::Challenger& ch, int bits, uint32_t* witness_monty) {
-    if (ch.input.size() >= 16) VG_FAIL(ctx, "grind: the sponge has a full input buffer");
+// The context's Poseidon-16 constants on the device (480 round constants + the MDS, Montgomery; then 17 words of grinding
+// scratch), uploaded on first use after vgpu_set_challenger.
+int32_t vg_poseidon_consts(vgpu_ctx* ctx, uint32_t** out) {
+    if (!ctx->challenger_set) VG_FAIL(ctx, "Poseidon-16: vgpu_set_challenger has not been called");
     if (!ctx->d_poseidon) {
-        std::vector<uint32_t> c(480 + 256);
-        for (int i = 0; i < 480; i++) c[i] = ch.perm->rc[i];
-        for (int i = 0; i < 16; i++) for (int j = 0; j < 16; j++) c[480 + i * 16 + j] = ch.perm->mds[i][j];
+        vgh::Poseidon16 perm;
+        perm.set(ctx->poseidon_rc, ctx->poseidon_has_mds ? ctx->poseidon_mds : nullptr);
+        std::vector<uint32_t> c(p16::CONST_WORDS);
+        for (int i = 0; i < 480; i++) c[i] = perm.rc[i];
+        for (int i = 0; i < 16; i++) for (int j = 0; j < 16; j++) c[480 + i * 16 + j] = perm.mds[i][j];
         VG_TRY(vg_alloc(ctx, (void**)&ctx->d_poseidon, (c.size() + 16 + 1) * 4));
         VG_CUDA(ctx, cudaMemcpyAsync(ctx->d_poseidon, c.data(), c.size() * 4, cudaMemcpyHostToDevice, ctx->stream));
         VG_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
     }
-    uint32_t* d_state = ctx->d_poseidon + 480 + 256;
+    *out = ctx->d_poseidon;
+    return 0;
+}
+
+// Smallest canonical witness w with check_witness(bits, w); the challenger is advanced exactly as grind() would.
+int32_t vg_pow_grind(vgpu_ctx* ctx, vgh::Challenger& ch, int bits, uint32_t* witness_monty) {
+    if (ch.input.size() >= 16) VG_FAIL(ctx, "grind: the sponge has a full input buffer");
+    uint32_t* consts = nullptr;
+    VG_TRY(vg_poseidon_consts(ctx, &consts));
+    uint32_t* d_state = consts + p16::CONST_WORDS;
     uint32_t* d_result = d_state + 16;
     uint32_t hs[17];
     for (int i = 0; i < 16; i++) hs[i] = i < (int)ch.input.size() ? ch.input[i] : ch.state[i];
@@ -72,7 +62,7 @@ int32_t vg_pow_grind(vgpu_ctx* ctx, vgh::Challenger& ch, int bits, uint32_t* wit
         hs[16] = 0xffffffffu;
         VG_CUDA(ctx, cudaMemcpyAsync(d_state, hs, 17 * 4, cudaMemcpyHostToDevice, ctx->stream));
         const uint32_t count = bb::P - w0 < batch ? bb::P - w0 : batch;
-        pow_grind_kernel<<<(count + 255) / 256, 256, 0, ctx->stream>>>(ctx->d_poseidon, d_state, slot, w0, count, mask, d_result);
+        pow_grind_kernel<<<(count + 255) / 256, 256, 0, ctx->stream>>>(consts, d_state, slot, w0, count, mask, d_result);
         VG_LAUNCH_CHECK(ctx);
         uint32_t found = 0;
         VG_CUDA(ctx, cudaMemcpyAsync(&found, d_result, 4, cudaMemcpyDeviceToHost, ctx->stream));
