@@ -44,6 +44,11 @@ int32_t vgpu_ctx_create(int32_t device, void* cuda_stream, vgpu_ctx** out);
 void vgpu_ctx_destroy(vgpu_ctx* ctx);
 const char* vgpu_last_error(const vgpu_ctx* ctx);
 int32_t vgpu_ctx_synchronize(vgpu_ctx* ctx);
+/* Stream order against the caller's own streams, with no host synchronisation (`cuda_event` is a cudaEvent_t of the context's
+ * device): wait_event makes the context's stream wait for an event the caller recorded on a producer stream (before an import or
+ * borrow of what that stream wrote); record_event records one on the context's stream for a consumer to wait for (after an export). */
+int32_t vgpu_ctx_wait_event(vgpu_ctx* ctx, void* cuda_event);
+int32_t vgpu_ctx_record_event(vgpu_ctx* ctx, void* cuda_event);
 /* Number of kernels this context has launched since creation (bench.py's gpu_launches). */
 uint64_t vgpu_ctx_launch_count(const vgpu_ctx* ctx);
 /* Frees the device buffers the context keeps for reuse by its next calls (otherwise held until vgpu_ctx_destroy): after a
@@ -87,6 +92,35 @@ int32_t vgpu_dmat_upload(vgpu_ctx* ctx, const vgpu_matrix* host, int32_t repr, v
 int32_t vgpu_dmat_upload_rows(vgpu_ctx* ctx, const vgpu_matrix* host, int32_t repr, vgpu_dmat** out);
 /* Writes the rows this rank holds at their place in the caller's height x width row-major buffer. */
 int32_t vgpu_dmat_download(vgpu_ctx* ctx, const vgpu_dmat* m, int32_t repr, uint32_t* host_row_major_out);
+/* View of caller DEVICE memory (a torch tensor, the output of the caller's own kernels), strides counted in words: row-major is
+ * (width, 1), column-major is (1, height), a sub-matrix of a larger buffer has larger strides.  Every call below refuses, before
+ * anything is enqueued, a view that is not device memory of the context's device (first and last word), a pointer that is not
+ * 4-byte aligned, and a view whose element indices or byte addresses overflow 64 bits.  4 bytes is all the kernels that read
+ * traces assume: the LDE's NTT passes, the LogUp sweeps, the check sweep and the import / export kernels load and store single
+ * 32-bit words at any column stride; the vector loads of the library (leaf hashing, openings, row-shard exchanges) read only
+ * buffers the library allocated itself.  Empty views (height or width 0) are handled as the uploads handle empty matrices. */
+typedef struct vgpu_dev_matrix {
+    const uint32_t* data;      /* device pointer on the context's device */
+    uint64_t height, width;
+    uint64_t row_stride;       /* elements between (r, c) and (r + 1, c) */
+    uint64_t col_stride;       /* elements between (r, c) and (r, c + 1) */
+} vgpu_dev_matrix;
+/* Device twin of vgpu_dmat_upload: a copy into a library-owned (column-major Montgomery) matrix on the context's stream, equal
+ * word for word to the upload of the same words.  Every word must be below p in either repr: otherwise the call fails naming the
+ * first offending (row, column) and creates no matrix.  Synchronises the context's stream once, to read that verdict; the caller's
+ * buffer may change once the call has returned. */
+int32_t vgpu_dmat_import(vgpu_ctx* ctx, const vgpu_dev_matrix* src, int32_t repr, vgpu_dmat** out);
+/* Device twin of vgpu_dmat_upload_rows: every rank passes a view of the whole matrix on its own device and only its run of rows is read. */
+int32_t vgpu_dmat_import_rows(vgpu_ctx* ctx, const vgpu_dev_matrix* src, int32_t repr, vgpu_dmat** out);
+/* Zero-copy: the caller's column-major Montgomery buffer (element (r, c) at data[c * col_stride + r], col_stride >= height) becomes
+ * a matrix that the library reads in place.  One read pass checks that every word is below p (synchronises once, copies nothing).
+ * The library never writes or frees the buffer (vgpu_ntt_batch refuses a borrowed matrix); the caller keeps it alive and unchanged
+ * until vgpu_dmat_free of the handle AND until every call that read it has returned.  Whole matrices only (not a rank's row shard). */
+int32_t vgpu_dmat_borrow(vgpu_ctx* ctx, uint32_t* data, uint64_t height, uint64_t width, uint64_t col_stride, vgpu_dmat** out);
+/* Device twin of vgpu_dmat_download: writes the rows this rank holds at their place in the caller's height x width view, in natural
+ * row order (a bit-reversed matrix, e.g. quotient chunks, is mapped by the kernel), on the context's stream with no host
+ * synchronisation (vgpu_ctx_record_event orders a consumer after it).  Refuses what the download refuses. */
+int32_t vgpu_dmat_export(vgpu_ctx* ctx, const vgpu_dmat* m, int32_t repr, const vgpu_dev_matrix* dst);
 /* Logical dimensions (of the whole matrix, also for a shard). */
 int32_t vgpu_dmat_dims(const vgpu_dmat* m, uint64_t* height, uint64_t* width);
 /* The rows held here; returns 0 = whole matrix, 1 = row shard, 2 = column share. */

@@ -48,6 +48,17 @@ pub struct vgpu_matrix {
     pub width: u64,
 }
 
+/// View of caller device memory on the context's device; strides in elements: row-major is `(width, 1)`, column-major `(1, height)`.
+#[repr(C)]
+#[derive(Clone, Copy)]
+pub struct vgpu_dev_matrix {
+    pub data: *const u32,
+    pub height: u64,
+    pub width: u64,
+    pub row_stride: u64,
+    pub col_stride: u64,
+}
+
 #[repr(C)]
 #[derive(Clone, Copy)]
 pub struct vgpu_pair_term {
@@ -91,6 +102,8 @@ extern "C" {
     pub fn vgpu_ctx_destroy(ctx: *mut vgpu_ctx);
     pub fn vgpu_last_error(ctx: *const vgpu_ctx) -> *const c_char;
     pub fn vgpu_ctx_synchronize(ctx: *mut vgpu_ctx) -> i32;
+    pub fn vgpu_ctx_wait_event(ctx: *mut vgpu_ctx, cuda_event: *mut c_void) -> i32;
+    pub fn vgpu_ctx_record_event(ctx: *mut vgpu_ctx, cuda_event: *mut c_void) -> i32;
     pub fn vgpu_ctx_launch_count(ctx: *const vgpu_ctx) -> u64;
     pub fn vgpu_ctx_release_cached(ctx: *mut vgpu_ctx) -> i32;
     pub fn vgpu_ctx_memory_stats(ctx: *mut vgpu_ctx, out: *mut u64, reset: i32) -> i32;
@@ -107,6 +120,10 @@ extern "C" {
     pub fn vgpu_dmat_upload(ctx: *mut vgpu_ctx, host: *const vgpu_matrix, repr: i32, out: *mut *mut vgpu_dmat) -> i32;
     pub fn vgpu_dmat_upload_rows(ctx: *mut vgpu_ctx, host: *const vgpu_matrix, repr: i32, out: *mut *mut vgpu_dmat) -> i32;
     pub fn vgpu_dmat_download(ctx: *mut vgpu_ctx, m: *const vgpu_dmat, repr: i32, host_row_major_out: *mut u32) -> i32;
+    pub fn vgpu_dmat_import(ctx: *mut vgpu_ctx, src: *const vgpu_dev_matrix, repr: i32, out: *mut *mut vgpu_dmat) -> i32;
+    pub fn vgpu_dmat_import_rows(ctx: *mut vgpu_ctx, src: *const vgpu_dev_matrix, repr: i32, out: *mut *mut vgpu_dmat) -> i32;
+    pub fn vgpu_dmat_borrow(ctx: *mut vgpu_ctx, data: *mut u32, height: u64, width: u64, col_stride: u64, out: *mut *mut vgpu_dmat) -> i32;
+    pub fn vgpu_dmat_export(ctx: *mut vgpu_ctx, m: *const vgpu_dmat, repr: i32, dst: *const vgpu_dev_matrix) -> i32;
     pub fn vgpu_dmat_dims(m: *const vgpu_dmat, height: *mut u64, width: *mut u64) -> i32;
     pub fn vgpu_dmat_local_rows(m: *const vgpu_dmat, row0: *mut u64, rows: *mut u64) -> i32;
     pub fn vgpu_dmat_free(m: *mut vgpu_dmat);

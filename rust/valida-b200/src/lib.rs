@@ -14,10 +14,11 @@
 
 use std::ffi::{c_void, CStr};
 use std::fmt;
+use std::marker::PhantomData;
 use std::ptr;
 
 pub use valida_b200_sys as sys;
-use sys::{vgpu_ctx, vgpu_matrix};
+use sys::{vgpu_ctx, vgpu_dev_matrix, vgpu_dmat, vgpu_matrix};
 
 /// An error reported by the library (status code + `vgpu_last_error` text).  The reference's prover panics on failure
 /// (`derive/src/lib.rs:319,364,396`); callers that want that behaviour `unwrap()`.
@@ -90,6 +91,65 @@ impl<'a> MatrixView<'a> {
     }
     fn raw(&self) -> vgpu_matrix {
         vgpu_matrix { data: self.values.as_ptr(), height: self.height() as u64, width: self.width as u64 }
+    }
+}
+
+/// A strided matrix of field words in device memory of the context's device (a buffer the caller's own kernels filled).  Strides
+/// count elements: element `(r, c)` is at `ptr[r * row_stride + c * col_stride]`.
+#[derive(Clone, Copy, Debug)]
+pub struct DeviceView {
+    pub ptr: *const u32,
+    pub height: u64,
+    pub width: u64,
+    pub row_stride: u64,
+    pub col_stride: u64,
+}
+
+impl DeviceView {
+    pub fn row_major(ptr: *const u32, height: u64, width: u64) -> Self {
+        Self { ptr, height, width, row_stride: width, col_stride: 1 }
+    }
+    pub fn col_major(ptr: *const u32, height: u64, width: u64) -> Self {
+        Self { ptr, height, width, row_stride: 1, col_stride: height }
+    }
+    fn raw(&self) -> vgpu_dev_matrix {
+        vgpu_dev_matrix { data: self.ptr, height: self.height, width: self.width, row_stride: self.row_stride, col_stride: self.col_stride }
+    }
+}
+
+/// A matrix on the device, in the library's layout: imported (a library-owned copy) or borrowed (the caller's buffer, read in
+/// place).  It cannot outlive the [`Context`] it was made on; dropping it releases the handle (never a borrowed buffer).
+pub struct DMat<'ctx> {
+    raw: *mut vgpu_dmat,
+    _ctx: PhantomData<&'ctx Context>,
+}
+
+impl DMat<'_> {
+    pub fn as_ptr(&self) -> *const vgpu_dmat {
+        self.raw
+    }
+
+    /// Logical (height, width).
+    pub fn dims(&self) -> (u64, u64) {
+        let (mut h, mut w) = (0u64, 0u64);
+        unsafe { sys::vgpu_dmat_dims(self.raw, &mut h, &mut w) };
+        (h, w)
+    }
+
+    /// Writes the rows held here into the caller's `height x width` view, in natural row order and `repr` words, on the context's
+    /// stream without a host synchronisation; order a consumer after it with [`Context::record_event`].
+    ///
+    /// # Safety
+    /// `dst` must describe writable device memory of `ctx`'s device that nothing else reads or writes until the export has run.
+    pub unsafe fn export_device(&self, ctx: &Context, repr: Repr, dst: &DeviceView) -> Result<()> {
+        let raw = dst.raw();
+        ctx.check(sys::vgpu_dmat_export(ctx.raw, self.raw, repr.raw(), &raw))
+    }
+}
+
+impl Drop for DMat<'_> {
+    fn drop(&mut self) {
+        unsafe { sys::vgpu_dmat_free(self.raw) }
     }
 }
 
@@ -189,6 +249,73 @@ impl Context {
         let code = unsafe { sys::vgpu_verify(self.raw, proof.as_ptr(), proof.len() as u64, prep_raw.as_ptr(), repr.raw(), &mut verdict) };
         self.check(code)?;
         Ok(if verdict == sys::VGPU_ACCEPT { Verdict::Accept } else { Verdict::Reject(verdict) })
+    }
+
+    /// Copies a device matrix the caller holds (any strides, `repr` words) into a library-owned one, on the context's stream.
+    /// Every word must be below p: otherwise the error names the first offending (row, column) and nothing is created.
+    /// Synchronises the context's stream once; the caller's buffer may change as soon as this returns.
+    ///
+    /// # Safety
+    /// `src` must describe readable device memory of this context's device, and whatever writes it must be ordered before the
+    /// context's stream (the same stream, or [`Context::wait_event`]).
+    pub unsafe fn import_device(&self, src: &DeviceView, repr: Repr) -> Result<DMat<'_>> {
+        let raw = src.raw();
+        let mut out: *mut vgpu_dmat = ptr::null_mut();
+        self.check(sys::vgpu_dmat_import(self.raw, &raw, repr.raw(), &mut out))?;
+        Ok(DMat { raw: out, _ctx: PhantomData })
+    }
+
+    /// [`Context::import_device`] for a rank of a [`LocalGroup`]: every rank passes a view of the whole matrix on its own device,
+    /// and of a trace tall enough to be split only this rank's run of rows is read.
+    ///
+    /// # Safety
+    /// As for [`Context::import_device`].
+    pub unsafe fn import_device_rows(&self, src: &DeviceView, repr: Repr) -> Result<DMat<'_>> {
+        let raw = src.raw();
+        let mut out: *mut vgpu_dmat = ptr::null_mut();
+        self.check(sys::vgpu_dmat_import_rows(self.raw, &raw, repr.raw(), &mut out))?;
+        Ok(DMat { raw: out, _ctx: PhantomData })
+    }
+
+    /// Zero-copy: the caller's column-major Montgomery buffer (element `(r, c)` at `data[c * col_stride + r]`, `col_stride >=
+    /// height`, 4-byte aligned) is proven from in place.  One read pass checks every word is below p; nothing is copied.
+    ///
+    /// # Safety
+    /// The library never writes or frees `data`, but reads it whenever a call takes the returned [`DMat`].  The caller keeps the
+    /// buffer allocated and unchanged until the `DMat` is dropped AND every call that took it has returned; writes to it before the
+    /// borrow must be ordered before the context's stream.
+    pub unsafe fn borrow_device(&self, data: *mut u32, height: u64, width: u64, col_stride: u64) -> Result<DMat<'_>> {
+        let mut out: *mut vgpu_dmat = ptr::null_mut();
+        self.check(sys::vgpu_dmat_borrow(self.raw, data, height, width, col_stride, &mut out))?;
+        Ok(DMat { raw: out, _ctx: PhantomData })
+    }
+
+    /// The context's stream waits for `cuda_event` (a `cudaEvent_t` the caller recorded on a producer stream).
+    ///
+    /// # Safety
+    /// `cuda_event` must be a valid CUDA event of this context's device.
+    pub unsafe fn wait_event(&self, cuda_event: *mut c_void) -> Result<()> {
+        self.check(sys::vgpu_ctx_wait_event(self.raw, cuda_event))
+    }
+
+    /// Records `cuda_event` on the context's stream, for a consumer stream to wait for (after [`DMat::export_device`]).
+    ///
+    /// # Safety
+    /// As for [`Context::wait_event`].
+    pub unsafe fn record_event(&self, cuda_event: *mut c_void) -> Result<()> {
+        self.check(sys::vgpu_ctx_record_event(self.raw, cuda_event))
+    }
+
+    /// `Machine::prove` from traces already on the device (imported or borrowed): the same bytes as [`Context::prove_bytes`].
+    pub fn prove_device_bytes(&self, main: &[&DMat<'_>; sys::VGPU_NUM_CHIPS], prep: &[&DMat<'_>; 2]) -> Result<Vec<u8>> {
+        let main_raw: Vec<*const vgpu_dmat> = main.iter().map(|m| m.as_ptr()).collect();
+        let prep_raw: Vec<*const vgpu_dmat> = prep.iter().map(|m| m.as_ptr()).collect();
+        let (mut bytes, mut len) = (ptr::null_mut::<u8>(), 0u64);
+        let code = unsafe { sys::vgpu_prove_device(self.raw, main_raw.as_ptr(), prep_raw.as_ptr(), &mut bytes, &mut len) };
+        self.check(code)?;
+        let proof = unsafe { std::slice::from_raw_parts(bytes, len as usize) }.to_vec();
+        unsafe { sys::vgpu_free_bytes(bytes) };
+        Ok(proof)
     }
 
     /// Kernels launched by this context so far.

@@ -8,6 +8,8 @@ from .api import (  # noqa: F401
     BABYBEAR_P,
     MERKLE_KECCAK256,
     MERKLE_POSEIDON16,
+    REPR_CANONICAL,
+    REPR_MONTY_R32,
     Context,
     DeviceMatrix,
     ProverData,

@@ -31,6 +31,11 @@ class _Matrix(C.Structure):
     _fields_ = [("data", C.POINTER(C.c_uint32)), ("height", C.c_uint64), ("width", C.c_uint64)]
 
 
+class _DevMatrix(C.Structure):
+    """vgpu_dev_matrix: a strided view of device memory (strides in elements)."""
+    _fields_ = [("data", C.c_void_p), ("height", C.c_uint64), ("width", C.c_uint64), ("row_stride", C.c_uint64), ("col_stride", C.c_uint64)]
+
+
 def _load():
     if not os.path.exists(lib_path):
         raise VgpuError(
@@ -43,6 +48,8 @@ def _load():
         "vgpu_ctx_destroy": (None, [vp]),
         "vgpu_last_error": (C.c_char_p, [vp]),
         "vgpu_ctx_synchronize": (C.c_int32, [vp]),
+        "vgpu_ctx_wait_event": (C.c_int32, [vp, vp]),
+        "vgpu_ctx_record_event": (C.c_int32, [vp, vp]),
         "vgpu_ctx_launch_count": (u64, [vp]),
         "vgpu_ctx_release_cached": (C.c_int32, [vp]),
         "vgpu_ctx_memory_stats": (C.c_int32, [vp, C.POINTER(u64), C.c_int32]),
@@ -54,6 +61,10 @@ def _load():
         "vgpu_dmat_upload_rows": (C.c_int32, [vp, C.POINTER(_Matrix), C.c_int32, C.POINTER(vp)]),
         "vgpu_dmat_local_rows": (C.c_int32, [vp, C.POINTER(u64), C.POINTER(u64)]),
         "vgpu_dmat_download": (C.c_int32, [vp, vp, C.c_int32, u32p]),
+        "vgpu_dmat_import": (C.c_int32, [vp, C.POINTER(_DevMatrix), C.c_int32, C.POINTER(vp)]),
+        "vgpu_dmat_import_rows": (C.c_int32, [vp, C.POINTER(_DevMatrix), C.c_int32, C.POINTER(vp)]),
+        "vgpu_dmat_borrow": (C.c_int32, [vp, vp, u64, u64, u64, C.POINTER(vp)]),
+        "vgpu_dmat_export": (C.c_int32, [vp, vp, C.c_int32, C.POINTER(_DevMatrix)]),
         "vgpu_dmat_dims": (C.c_int32, [vp, C.POINTER(u64), C.POINTER(u64)]),
         "vgpu_dmat_free": (None, [vp]),
         "vgpu_ntt_batch": (C.c_int32, [vp, vp, C.c_int32]),
@@ -130,6 +141,7 @@ class Context:
     """One context per device/stream (single-threaded)."""
 
     def __init__(self, device=0, stream=None):
+        self.device = device
         self._children = weakref.WeakSet()      # handles that point into this context: released before the context goes
         self._h = C.c_void_p()
         rc = lib().vgpu_ctx_create(device, C.c_void_p(stream) if stream else None, C.byref(self._h))
@@ -216,6 +228,57 @@ class Context:
         self.check(lib().vgpu_dmat_upload_rows(self._h, C.byref(m), repr, C.byref(out)))
         return DeviceMatrix(self, out)
 
+    # ---- caller device memory: torch tensors in, torch tensors out (include/valida_b200.h, vgpu_dmat_import / _borrow / _export) ----
+    def _wait_for_torch(self, device):
+        """The context's stream waits for torch's current stream on `device` (what it enqueued so far wrote the tensor)."""
+        import torch
+
+        ev = torch.cuda.Event()
+        ev.record(torch.cuda.current_stream(device))
+        self.check(lib().vgpu_ctx_wait_event(self._h, C.c_void_p(ev.cuda_event)))
+
+    def _torch_waits(self, device):
+        """torch's current stream on `device` waits for what the context's stream has enqueued so far."""
+        import torch
+
+        stream = torch.cuda.current_stream(device)
+        ev = torch.cuda.Event()
+        ev.record(stream)                       # creates the event on the device; the context's stream records it again
+        self.check(lib().vgpu_ctx_record_event(self._h, C.c_void_p(ev.cuda_event)))
+        stream.wait_event(ev)
+
+    def _import_tensor(self, fn, what, t, repr):
+        v = _tensor_view(self, t, what)
+        self._wait_for_torch(t.device)
+        out = C.c_void_p()
+        self.check(fn(self._h, C.byref(v), repr, C.byref(out)))
+        return DeviceMatrix(self, out)
+
+    def import_tensor(self, t, repr=REPR_CANONICAL):
+        """A 2-D CUDA tensor (torch.int32 or torch.uint32 bits, any non-negative strides, on this context's device) -> a
+        library-owned DeviceMatrix, equal to upload() of the same words.  Ordered after torch's current stream; every word must be
+        below p (VgpuError names the first that is not).  The tensor may change once this returns."""
+        return self._import_tensor(lib().vgpu_dmat_import, "import_tensor", t, repr)
+
+    def import_tensor_rows(self, t, repr=REPR_CANONICAL):
+        """Split proof: import_tensor of this rank's run of rows of a trace tall enough to be split (every rank passes the whole
+        tensor on its own device); otherwise like import_tensor."""
+        return self._import_tensor(lib().vgpu_dmat_import_rows, "import_tensor_rows", t, repr)
+
+    def borrow_tensor(self, t):
+        """Zero-copy: a column-major tensor of Montgomery words (stride(0) == 1, stride(1) >= shape(0)) becomes a DeviceMatrix read in
+        place.  Its words are checked once (below p); it is never written, and the DeviceMatrix keeps a reference to it.  Leave it
+        unchanged while the DeviceMatrix is alive."""
+        v = _tensor_view(self, t, "borrow_tensor")
+        if v.row_stride != 1:
+            raise ValueError("borrow_tensor: the tensor is not column-major (stride(0) = %d, must be 1)" % v.row_stride)
+        self._wait_for_torch(t.device)
+        out = C.c_void_p()
+        self.check(lib().vgpu_dmat_borrow(self._h, v.data, v.height, v.width, v.col_stride, C.byref(out)))
+        m = DeviceMatrix(self, out)
+        m._tensor = t
+        return m
+
     def host_register(self, array):
         """Page-lock a numpy array the caller will prove from repeatedly (its uploads then overlap the commits)."""
         self.check(lib().vgpu_host_register(self._h, C.c_void_p(array.ctypes.data), array.nbytes))
@@ -251,9 +314,35 @@ class Context:
             pass
 
 
+def _tensor_view(ctx, t, what):
+    """_DevMatrix of a 2-D CUDA tensor of 32-bit words on the context's device.  Strides of a dimension of size 1 are never used to
+    address an element; they are normalised so that a column (h x 1) and a row (1 x w) read as column-major views."""
+    import torch
+
+    if not isinstance(t, torch.Tensor):
+        raise TypeError("%s: expected a torch.Tensor, got %s" % (what, type(t).__name__))
+    if t.device.type != "cuda":
+        raise ValueError("%s: the tensor is on %s; a CUDA tensor on cuda:%d is needed" % (what, t.device, ctx.device))
+    if t.device.index != ctx.device:
+        raise ValueError("%s: the tensor is on %s, the context on cuda:%d" % (what, t.device, ctx.device))
+    if t.dtype not in (torch.int32, torch.uint32):
+        raise TypeError("%s: dtype %s; torch.int32 or torch.uint32 words are needed" % (what, t.dtype))
+    if t.dim() != 2:
+        raise ValueError("%s: a 2-D tensor is needed, got %d dimensions" % (what, t.dim()))
+    (h, w), (rs, cs) = t.shape, t.stride()
+    if rs < 0 or cs < 0:
+        raise ValueError("%s: negative strides %s" % (what, t.stride()))
+    if h <= 1:
+        rs = 1
+    if w <= 1:
+        cs = max(cs, h)
+    return _DevMatrix(t.data_ptr(), h, w, rs, cs)
+
+
 class DeviceMatrix:
     def __init__(self, ctx, handle, owned=True):
         self.ctx, self._h, self._owned = ctx, handle, owned
+        self._tensor = None                      # borrow_tensor: the caller's tensor the matrix reads in place
         ctx._children.add(self)
 
     @property
@@ -274,10 +363,31 @@ class DeviceMatrix:
         self.ctx.check(lib().vgpu_dmat_download(self.ctx._h, self._h, repr, out.ctypes.data_as(C.POINTER(C.c_uint32))))
         return out
 
+    def to_tensor(self, repr=REPR_CANONICAL, out=None):
+        """The matrix as a (h, w) torch.int32 CUDA tensor on the context's device (natural row order, `repr` words), or written into
+        `out` (int32 or uint32, any strides).  Enqueued on the context's stream; torch's current stream waits for it.  Of a row shard
+        only this rank's rows are written."""
+        import torch
+
+        h, w = self.shape
+        dev = torch.device("cuda", self.ctx.device)
+        if out is None:
+            out = torch.empty((h, w), dtype=torch.int32, device=dev)
+        v = _tensor_view(self.ctx, out, "to_tensor")
+        if (v.height, v.width) != (h, w):
+            raise ValueError("to_tensor: out has shape %s, the matrix is %d x %d" % (tuple(out.shape), h, w))
+        self.ctx._wait_for_torch(dev)            # out may have been allocated or last used on torch's stream
+        self.ctx.check(lib().vgpu_dmat_export(self.ctx._h, self._h, repr, C.byref(v)))
+        self.ctx._torch_waits(dev)
+        return out
+
     def free(self):
         if self._h and self._owned and self.ctx._h:
             lib().vgpu_dmat_free(self._h)
+            if self._tensor is not None:         # torch may reuse the tensor's memory only after the context's reads of it
+                self.ctx._torch_waits(self._tensor.device)
         self._h = None
+        self._tensor = None
 
     def __del__(self):
         try:

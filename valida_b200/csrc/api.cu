@@ -168,6 +168,18 @@ void vgpu_ctx_destroy(vgpu_ctx* ctx) {
 
 const char* vgpu_last_error(const vgpu_ctx* ctx) { return ctx ? ctx->err.c_str() : "null context"; }
 int32_t vgpu_ctx_synchronize(vgpu_ctx* ctx) { VG_CUDA(ctx, cudaStreamSynchronize(ctx->stream)); return 0; }
+int32_t vgpu_ctx_wait_event(vgpu_ctx* ctx, void* cuda_event) {
+    if (!cuda_event) VG_FAIL(ctx, "ctx_wait_event: null event");
+    VG_TRY(vg_enter(ctx));
+    VG_CUDA(ctx, cudaStreamWaitEvent(ctx->stream, (cudaEvent_t)cuda_event, 0));
+    return 0;
+}
+int32_t vgpu_ctx_record_event(vgpu_ctx* ctx, void* cuda_event) {
+    if (!cuda_event) VG_FAIL(ctx, "ctx_record_event: null event");
+    VG_TRY(vg_enter(ctx));
+    VG_CUDA(ctx, cudaEventRecord((cudaEvent_t)cuda_event, ctx->stream));
+    return 0;
+}
 uint64_t vgpu_ctx_launch_count(const vgpu_ctx* ctx) { return ctx->launches; }
 int32_t vgpu_ctx_release_cached(vgpu_ctx* ctx) {
     VG_TRY(vg_enter(ctx));
@@ -192,7 +204,7 @@ int32_t vgpu_ctx_set_merkle_hash(vgpu_ctx* ctx, int32_t hash) {
 static const char* KCLASS_NAMES[KC_COUNT] = {"ntt_pass_kernel", "leaf_hash_kernel", "compress_layer_kernel", "fri_leaf_hash_kernel", "transpose (rm<->cm)",
                                              "perm trace kernels", "quotient_kernel", "inverse denominators", "bary_kernel", "reduced_opening_kernel", "fri_fold_kernel", "peer-store exchange", "all-gathers + barriers (incl. waiting for the slowest rank)", "other",
                                              "check_kernel", "query_path_kernel", "p16_leaf_kernel", "p16_layer_kernel + p16_tail_kernel", "p16_fri_leaf_kernel",
-                                             "p16_path_kernel"};
+                                             "p16_path_kernel", "import_kernel / export_kernel (caller device memory)"};
 uint32_t vgpu_ctx_kernel_stats(vgpu_ctx* ctx, const char** names, uint32_t* launches, float* ms, double* bytes, uint32_t cap) {
     cudaStreamSynchronize(ctx->stream);
     uint32_t n[KC_COUNT] = {0}; float t[KC_COUNT] = {0}; double b[KC_COUNT] = {0};
@@ -271,6 +283,78 @@ int32_t vgpu_dmat_download(vgpu_ctx* ctx, const vgpu_dmat* m, int32_t repr, uint
     }
     return 0;
 }
+// ---- caller device memory ----------------------------------------------------------------------------
+// A caller's view must lie in device memory of the context's device (first and last word), hold whole words, and address its h x w
+// elements, their row-major index r * w + c and their bytes without 64-bit overflow.  Checked before anything is enqueued.
+static int32_t check_device_view(vgpu_ctx* ctx, const char* what, const uint32_t* p, uint64_t h, uint64_t w, uint64_t rs, uint64_t cs) {
+    uint64_t a, b, last, n;
+    if (__builtin_mul_overflow(h - 1, rs, &a) || __builtin_mul_overflow(w - 1, cs, &b) || __builtin_add_overflow(a, b, &last) ||
+        last > (UINT64_MAX >> 2) || (uintptr_t)p + 4 * last < (uintptr_t)p || __builtin_mul_overflow(h, w, &n) || n > (UINT64_MAX >> 2))
+        VG_FAIL(ctx, "%s: a %llu x %llu view with strides (%llu, %llu) overflows 64-bit addressing", what, (unsigned long long)h, (unsigned long long)w,
+                (unsigned long long)rs, (unsigned long long)cs);
+    if ((uintptr_t)p % 4) VG_FAIL(ctx, "%s: the device pointer %p is not 4-byte aligned", what, (const void*)p);
+    for (const uint32_t* q : {p, p + last}) {
+        cudaPointerAttributes at{};
+        if (cudaPointerGetAttributes(&at, q) != cudaSuccess) { cudaGetLastError(); at.type = cudaMemoryTypeUnregistered; }
+        if (at.type != cudaMemoryTypeDevice || at.device != ctx->device)
+            VG_FAIL(ctx, "%s: %p is not device memory of the context's device %d", what, (const void*)q, ctx->device);
+    }
+    return 0;
+}
+static int32_t import_view(vgpu_ctx* ctx, const char* what, const vgpu_dev_matrix* src, int32_t repr, bool rows, vgpu_dmat** out) {
+    if (!src || !out) VG_FAIL(ctx, "%s: null argument", what);
+    VG_TRY(vg_enter(ctx));
+    const uint64_t h = src->height, w = src->width;
+    if (h && w) VG_TRY(check_device_view(ctx, what, src->data, h, w, src->row_stride, src->col_stride));
+    vgpu_dmat* m = nullptr;
+    VG_TRY(rows && vg_split_rows(ctx, 2 * h) ? vg_dmat_alloc_dist(ctx, VG_ROWS, h, w, false, &m) : vg_dmat_alloc(ctx, h, w, &m));
+    unsigned long long bad = ~0ull;
+    int32_t rc = vg_import_strided(ctx, src->data + m->row0 * src->row_stride, m->h, m->w, src->row_stride, src->col_stride, repr, m, &bad);
+    const uint64_t row0 = m->row0;
+    if (rc == 0 && bad == ~0ull) { *out = m; return 0; }
+    vgpu_dmat_free(m);
+    if (rc) return rc;
+    VG_FAIL(ctx, "%s: the word at row %llu, column %llu is not below p = %u (neither a canonical nor a Montgomery BabyBear word)", what,
+            (unsigned long long)(row0 + bad / w), (unsigned long long)(bad % w), bb::P);
+}
+int32_t vgpu_dmat_import(vgpu_ctx* ctx, const vgpu_dev_matrix* src, int32_t repr, vgpu_dmat** out) {
+    return import_view(ctx, "dmat_import", src, repr, false, out);
+}
+int32_t vgpu_dmat_import_rows(vgpu_ctx* ctx, const vgpu_dev_matrix* src, int32_t repr, vgpu_dmat** out) {
+    return import_view(ctx, "dmat_import_rows", src, repr, true, out);
+}
+int32_t vgpu_dmat_borrow(vgpu_ctx* ctx, uint32_t* data, uint64_t height, uint64_t width, uint64_t col_stride, vgpu_dmat** out) {
+    if (!out) VG_FAIL(ctx, "dmat_borrow: null argument");
+    VG_TRY(vg_enter(ctx));
+    if (col_stride < height) VG_FAIL(ctx, "dmat_borrow: column stride %llu is below the height %llu", (unsigned long long)col_stride, (unsigned long long)height);
+    if (height && width) {
+        VG_TRY(check_device_view(ctx, "dmat_borrow", data, height, width, 1, col_stride));
+        unsigned long long bad = ~0ull;
+        VG_TRY(vg_import_strided(ctx, data, height, width, 1, col_stride, VGPU_REPR_MONTY_R32, nullptr, &bad));
+        if (bad != ~0ull)
+            VG_FAIL(ctx, "dmat_borrow: the word at row %llu, column %llu is not below p = %u (not a Montgomery BabyBear word)",
+                    (unsigned long long)(bad / width), (unsigned long long)(bad % width), bb::P);
+    }
+    vgpu_dmat* m = new (std::nothrow) vgpu_dmat();
+    if (!m) VG_FAIL(ctx, "out of host memory");
+    m->ctx = ctx; m->d = data; m->h = m->gh = height; m->w = m->gw = width; m->col_stride = col_stride;
+    m->owns = false;
+    *out = m;
+    return 0;
+}
+int32_t vgpu_dmat_export(vgpu_ctx* ctx, const vgpu_dmat* m, int32_t repr, const vgpu_dev_matrix* dst) {
+    if (!m || !dst) VG_FAIL(ctx, "dmat_export: null argument");
+    VG_TRY(vg_enter(ctx));
+    if (m->dist == VG_COLS) VG_FAIL(ctx, "dmat_export: column shares are internal to a commit");
+    if (m->dist == VG_ROWS && m->bitrev_rows) VG_FAIL(ctx, "dmat_export: a bit-reversed row shard has no contiguous natural-order image");
+    if (dst->height != m->gh || dst->width != m->gw)
+        VG_FAIL(ctx, "dmat_export: the view is %llu x %llu, the matrix %llu x %llu", (unsigned long long)dst->height, (unsigned long long)dst->width,
+                (unsigned long long)m->gh, (unsigned long long)m->gw);
+    if (m->h == 0 || m->w == 0) return 0;
+    VG_TRY(check_device_view(ctx, "dmat_export", dst->data, dst->height, dst->width, dst->row_stride, dst->col_stride));
+    VG_TRY(vg_dmat_materialize(ctx, m));
+    return vg_export_strided(ctx, m, repr, const_cast<uint32_t*>(dst->data), dst->row_stride, dst->col_stride);
+}
 int32_t vgpu_dmat_dims(const vgpu_dmat* m, uint64_t* height, uint64_t* width) { *height = m->gh; *width = m->gw; return 0; }
 int32_t vgpu_dmat_local_rows(const vgpu_dmat* m, uint64_t* row0, uint64_t* rows) { *row0 = m->row0; *rows = m->h; return m->dist; }
 void vgpu_dmat_free(vgpu_dmat* m) {
@@ -290,6 +374,7 @@ void vgpu_dmat_free(vgpu_dmat* m) {
 int32_t vgpu_ntt_batch(vgpu_ctx* ctx, vgpu_dmat* m, int32_t inverse) {
     VG_TRY(vg_enter(ctx));
     if (m->dist != VG_FULL) VG_FAIL(ctx, "ntt_batch: the matrix is a shard of a split proof");
+    if (!m->owns) VG_FAIL(ctx, "ntt_batch: the matrix is a borrowed caller buffer, which the library never writes");
     int log_n = 0;
     while ((1ull << log_n) < m->h) log_n++;
     if ((1ull << log_n) != m->h) VG_FAIL(ctx, "ntt_batch: height %llu is not a power of two", (unsigned long long)m->h);

@@ -27,7 +27,8 @@ __device__ __forceinline__ uint32_t vg_pow_lookup(const uint32_t* lo, const uint
 
 // kernel classes for the optional per-launch CUDA-event timing (bench.py's roofline line)
 enum KClass { KC_NTT = 0, KC_LEAF_HASH, KC_COMPRESS, KC_FRI_LEAF, KC_TRANSPOSE, KC_PERM, KC_QUOTIENT, KC_INVDEN, KC_BARY, KC_REDUCED_OPENING, KC_FRI_FOLD, KC_EXCHANGE, KC_COLLECTIVE, KC_OTHER, KC_CHECK, KC_TREE_PATH,
-             KC_P16_LEAF, KC_P16_COMPRESS, KC_P16_FRI_LEAF, KC_P16_PATH, KC_COUNT };   // KC_P16_*: the Poseidon-16 Merkle kernels (merkle.cu)
+             KC_P16_LEAF, KC_P16_COMPRESS, KC_P16_FRI_LEAF, KC_P16_PATH,   // KC_P16_*: the Poseidon-16 Merkle kernels (merkle.cu)
+             KC_DEVICE_IO, KC_COUNT };                                     // KC_DEVICE_IO: import / borrow check / export of caller device memory (staging.cu)
 struct KTimer { cudaEvent_t a, b; int cls; double bytes; };
 
 struct vgpu_ctx {
@@ -185,3 +186,6 @@ void vg_stager_free(vgpu_ctx* ctx);
 int32_t vg_dmat_materialize(vgpu_ctx* ctx, const vgpu_dmat* m);                                                       // no-op unless an upload is pending
 int32_t vg_upload_rowmajor(vgpu_ctx* ctx, const uint32_t* host, uint64_t h, uint64_t w, int32_t repr, vgpu_dmat* dst);
 int32_t vg_download_rowmajor(vgpu_ctx* ctx, const vgpu_dmat* src, int32_t repr, uint32_t* host);
+int32_t vg_import_strided(vgpu_ctx* ctx, const uint32_t* src, uint64_t h, uint64_t w, uint64_t rs, uint64_t cs, int32_t repr, vgpu_dmat* dst_or_null,
+                          unsigned long long* bad_key);                                                                    // synchronises
+int32_t vg_export_strided(vgpu_ctx* ctx, const vgpu_dmat* src, int32_t repr, uint32_t* dst, uint64_t rs, uint64_t cs);       // no host sync

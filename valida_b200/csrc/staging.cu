@@ -243,3 +243,126 @@ int32_t vg_download_rowmajor(vgpu_ctx* ctx, const vgpu_dmat* src, int32_t repr, 
     vg_free(ctx, stage);
     return 0;
 }
+
+// ---- caller device memory (vgpu_dmat_import / _borrow / _export) -----------------------------------------------------------
+// A caller matrix is any strided view: element (r, c) at v[r * rs + c * cs].  One CTA moves a tile of up to 128 columns and
+// `tr` rows through shared memory: it reads along whichever stride is the unit one (row-major: runs of a row; column-major: runs
+// of a column), so the loads are coalesced either way, and writes the library's columns as runs of consecutive rows.  Narrow
+// matrices get taller tiles (tr = 4096 rows of one column), so every CTA moves about 8 K words.
+namespace {
+constexpr uint32_t IO_TILE_WORDS = TR * (TW + 1);
+
+struct IoTiles {
+    uint64_t h, w;          // rows and columns moved
+    uint32_t tr;            // rows per tile (a power of two)
+    uint64_t row_tiles;     // ceil(h / tr); tile t covers row tile t % row_tiles of column tile t / row_tiles
+};
+__device__ __forceinline__ void io_tile(const IoTiles& g, uint64_t& r0, uint64_t& c0, uint32_t& rows, uint32_t& wc, uint32_t& wp) {
+    const uint64_t t = blockIdx.x;
+    r0 = (t % g.row_tiles) * g.tr;
+    c0 = (t / g.row_tiles) * TW;
+    rows = (uint32_t)(g.h - r0 < g.tr ? g.h - r0 : g.tr);
+    wc = (uint32_t)(g.w - c0 < TW ? g.w - c0 : TW);
+    wp = wc | 1;            // odd row pitch: a walk down a tile column touches 32 different banks
+}
+
+// Import (STORE) and the borrow check (!STORE).  Every word must be below p in either representation; the smallest row-major
+// index r * w + c of a word that is not goes to *bad with ONE atomicMin per warp that holds one (a clean matrix costs no atomic).
+template <bool STORE>
+__global__ void __launch_bounds__(256) import_kernel(const __grid_constant__ IoTiles g, const uint32_t* __restrict__ src, uint64_t rs, uint64_t cs,
+                                                     uint32_t* __restrict__ cm, uint64_t dcs, int to_monty, unsigned long long* __restrict__ bad) {
+    __shared__ uint32_t tile[IO_TILE_WORDS];
+    uint64_t r0, c0; uint32_t rows, wc, wp;
+    io_tile(g, r0, c0, rows, wc, wp);
+    const uint32_t tot = rows * wc;
+    const bool row_runs = cs <= rs;      // the unit (or smaller) stride is along a row
+    unsigned long long mine = ~0ull;
+    for (uint32_t i = threadIdx.x; i < tot; i += blockDim.x) {
+        uint32_t r, c;
+        if (row_runs) { r = i / wc; c = i % wc; } else { c = i / rows; r = i % rows; }
+        const uint32_t v = src[(r0 + r) * rs + (c0 + c) * cs];
+        if (v >= bb::P) mine = min(mine, (unsigned long long)((r0 + r) * g.w + c0 + c));
+        if (STORE) tile[r * wp + c] = v;
+    }
+    const unsigned vote = __ballot_sync(0xffffffffu, mine != ~0ull);
+    if (vote) {                          // rare: the warp's smallest key, then one atomic
+        for (int o = 16; o; o >>= 1) mine = min(mine, __shfl_xor_sync(0xffffffffu, mine, o));
+        if ((threadIdx.x & 31) == 0) atomicMin(bad, mine);
+    }
+    if (!STORE) return;
+    __syncthreads();
+    for (uint32_t i = threadIdx.x; i < tot; i += blockDim.x) {
+        const uint32_t c = i / rows, r = i % rows;
+        const uint32_t v = tile[r * wp + c];
+        cm[(c0 + c) * dcs + r0 + r] = to_monty ? bb::to_monty(v) : v;
+    }
+}
+
+// Export: the mirror image.  Stored row r of the local part is logical row row0 + r, or reverse_bits(r) of a bit-reversed matrix.
+__global__ void __launch_bounds__(256) export_kernel(const __grid_constant__ IoTiles g, const uint32_t* __restrict__ cm, uint64_t scs, int from_monty,
+                                                     uint32_t* __restrict__ dst, uint64_t rs, uint64_t cs, uint64_t row0, int log_bitrev) {
+    __shared__ uint32_t tile[IO_TILE_WORDS];
+    uint64_t r0, c0; uint32_t rows, wc, wp;
+    io_tile(g, r0, c0, rows, wc, wp);
+    const uint32_t tot = rows * wc;
+    for (uint32_t i = threadIdx.x; i < tot; i += blockDim.x) {
+        const uint32_t c = i / rows, r = i % rows;
+        const uint32_t v = cm[(c0 + c) * scs + r0 + r];
+        tile[r * wp + c] = from_monty ? bb::from_monty(v) : v;
+    }
+    __syncthreads();
+    const bool row_runs = cs <= rs;
+    for (uint32_t i = threadIdx.x; i < tot; i += blockDim.x) {
+        uint32_t r, c;
+        if (row_runs) { r = i / wc; c = i % wc; } else { c = i / rows; r = i % rows; }
+        const uint64_t lr = log_bitrev >= 0 ? (uint64_t)bb::reverse_bits((uint32_t)(r0 + r), log_bitrev) : row0 + r0 + r;
+        dst[lr * rs + (c0 + c) * cs] = tile[r * wp + c];
+    }
+}
+
+IoTiles io_tiles(uint64_t h, uint64_t w) {
+    const uint32_t wp = (uint32_t)(w < TW ? w : TW) | 1;
+    uint32_t tr = 1;
+    while (tr < 4096 && 2 * tr * wp <= IO_TILE_WORDS) tr *= 2;
+    return IoTiles{h, w, tr, (h + tr - 1) / tr};
+}
+}  // namespace
+
+// Enqueues the import of h x w words at src (strides rs, cs) into dst (null: check only) and reads the verdict: synchronises the
+// context's stream once.  *bad_key: ~0 when every word is below p, else the smallest row-major index r * w + c of one that is not.
+int32_t vg_import_strided(vgpu_ctx* ctx, const uint32_t* src, uint64_t h, uint64_t w, uint64_t rs, uint64_t cs, int32_t repr, vgpu_dmat* dst,
+                          unsigned long long* bad_key) {
+    *bad_key = ~0ull;
+    if (h == 0 || w == 0) return 0;
+    unsigned long long* d_bad = nullptr;
+    VG_TRY(vg_alloc(ctx, (void**)&d_bad, sizeof *d_bad));
+    struct Free { vgpu_ctx* c; void* p; ~Free() { vg_free(c, p); } } fr{ctx, d_bad};
+    VG_CUDA(ctx, cudaMemsetAsync(d_bad, 0xff, sizeof *d_bad, ctx->stream));
+    const IoTiles g = io_tiles(h, w);
+    const uint64_t tiles = g.row_tiles * ((w + TW - 1) / TW);
+    if (tiles > 0x7fffffffull) VG_FAIL(ctx, "import: %llu x %llu words exceed one launch", (unsigned long long)h, (unsigned long long)w);
+    {
+        KScope ks(ctx, KC_DEVICE_IO, (dst ? 8.0 : 4.0) * (double)h * (double)w);
+        if (dst) import_kernel<true><<<(unsigned)tiles, 256, 0, ctx->stream>>>(g, src, rs, cs, dst->d, dst->col_stride, repr == VGPU_REPR_CANONICAL, d_bad);
+        else import_kernel<false><<<(unsigned)tiles, 256, 0, ctx->stream>>>(g, src, rs, cs, nullptr, 0, 0, d_bad);
+        VG_LAUNCH_CHECK(ctx);
+    }
+    VG_CUDA(ctx, cudaMemcpyAsync(bad_key, d_bad, sizeof *d_bad, cudaMemcpyDeviceToHost, ctx->stream));
+    VG_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
+    return 0;
+}
+
+// The local rows of src into the caller's view at dst (strides rs, cs; logical row i at dst[i * rs]), on the context's stream.
+int32_t vg_export_strided(vgpu_ctx* ctx, const vgpu_dmat* src, int32_t repr, uint32_t* dst, uint64_t rs, uint64_t cs) {
+    const uint64_t h = src->h, w = src->w;
+    if (h == 0 || w == 0) return 0;
+    int lg = -1;
+    if (src->bitrev_rows) { lg = 0; while ((1ull << lg) < h) lg++; }
+    const IoTiles g = io_tiles(h, w);
+    const uint64_t tiles = g.row_tiles * ((w + TW - 1) / TW);
+    if (tiles > 0x7fffffffull) VG_FAIL(ctx, "export: %llu x %llu words exceed one launch", (unsigned long long)h, (unsigned long long)w);
+    KScope ks(ctx, KC_DEVICE_IO, 8.0 * (double)h * (double)w);
+    export_kernel<<<(unsigned)tiles, 256, 0, ctx->stream>>>(g, src->d, src->col_stride, repr == VGPU_REPR_CANONICAL, dst, rs, cs, src->row0, lg);
+    VG_LAUNCH_CHECK(ctx);
+    return 0;
+}
