@@ -4,6 +4,9 @@ The device sweep is held to two texts of the reference's debug-build check: the 
 test_check_constraints_restatement.py (first failing row and constraint, and the count of failing rows) and the oracle's
 check_constraints.  Clean witnesses report nothing, the witnesses the CPU AIR rejects are located exactly, random and tampered
 traces agree row for row, and the debug mode leaves the proof bytes alone."""
+import os
+import sys
+
 import numpy as np
 import pytest
 
@@ -11,6 +14,9 @@ import programs
 from test_check_constraints_restatement import (PREP_CHIPS, as_oracle_code, check_py, fib_traces, oracle_check,  # noqa: F401
                                                 random_case, tamper_cases, tampered)
 from test_perm_trace_restatement import CHIPS, P
+
+sys.path.insert(0, os.path.join(os.path.dirname(os.path.abspath(__file__)), "golden"))
+from make_large_proof_digests import assert_matches_golden  # noqa: E402
 
 pytestmark = pytest.mark.gpu
 
@@ -199,9 +205,10 @@ def test_split_contexts_refuse_the_debug_mode(oracle):
 
 
 def test_full_size_fibonacci(ctx, oracle):
-    """Fibonacci with 2^22 CPU rows (memory chip 2^24): the debug mode passes and leaves the bytes alone; one CPU cell changed at a
-    row r is found on rows r - 1 and r only, as the Python checker computes on those rows, and the cumulative sums no longer cancel
-    when row r sends on the memory bus (the last row is padding and sends nothing)."""
+    """Fibonacci with 2^22 CPU rows (memory chip 2^24) from the device witness: the bytes are the recorded oracle proof's; the debug
+    mode passes and leaves the bytes alone; one CPU cell changed at a row r is found on rows r - 1 and r only, as the Python checker
+    computes on those rows, and the cumulative sums no longer cancel when row r sends on the memory bus (the last row is padding and
+    sends nothing)."""
     import valida_b200 as vb
 
     n = ((1 << 22) - 17) // 7
@@ -211,6 +218,7 @@ def test_full_size_fibonacci(ctx, oracle):
     h = dm[0].shape[0]
     assert h == 1 << 22
     off = vb.prove_machine(cfg, None, device_resident=(dm, dp))
+    assert_matches_golden(off, "fib_2p22")
     ctx.set_debug_checks(True)
     try:
         on = vb.prove_machine(cfg, None, device_resident=(dm, dp))

@@ -3,11 +3,16 @@
 host traces and the oracle's; every import equals upload() of the same words; refusals name the offending word and launch nothing
 when they are decided on the host."""
 import ctypes as C
+import os
+import sys
 
 import numpy as np
 import pytest
 
 from programs import mixed_program, static_data_program
+
+sys.path.insert(0, os.path.join(os.path.dirname(os.path.abspath(__file__)), "golden"))
+from make_large_proof_digests import assert_matches_golden  # noqa: E402
 
 pytestmark = pytest.mark.gpu
 P = 2013265921
@@ -342,7 +347,8 @@ def test_split_import_rows(oracle, fib15, nranks):
 
 
 def test_full_size_borrow_saves_the_traces(ctx, oracle, cfg):
-    """Fibonacci 2^22 from borrowed tensors: the uploaded traces' bytes, and a peak that is lower by the traces' device copy."""
+    """Fibonacci 2^22 from borrowed tensors: the uploaded traces' bytes, which are the recorded oracle proof's, and a peak that is
+    lower by the traces' device copy."""
     import valida_b200 as vb
 
     torch = _torch()
@@ -356,6 +362,7 @@ def test_full_size_borrow_saves_the_traces(ctx, oracle, cfg):
         ctx.memory_stats(reset=True)
         proof = vb.prove_machine(cfg, t, device_resident=(dm, dp))
         peak_uploaded = ctx.memory_stats()["peak"]
+        assert_matches_golden(proof, "fib_2p22")
     finally:
         for m in dm + dp:
             m.free()

@@ -1,8 +1,14 @@
 """GPU Machine::prove parity: proof bytes identical to the oracle's, accepted by the oracle verifier,
 tampering rejected; plus size-independent properties on a larger trace."""
+import os
+import sys
+
 import cbor2
 import numpy as np
 import pytest
+
+sys.path.insert(0, os.path.join(os.path.dirname(os.path.abspath(__file__)), "golden"))
+from make_large_proof_digests import assert_matches_golden  # noqa: E402
 
 P = 2013265921
 pytestmark = pytest.mark.gpu
@@ -80,12 +86,13 @@ def test_prove_larger_trace_verifies_and_matches(ctx, oracle):
 
 
 def test_prove_2_16_rows_verifies(ctx, oracle):
-    """Size-independent check at a size the oracle prover would take long on: the verifier accepts."""
+    """65537 cycles (2^17 CPU rows): the verifier accepts, and the bytes are the recorded oracle proof's."""
     import valida_b200 as vb
 
     t = vb.run_program(vb.fib_program(9360), initial_fp=0x1000)   # 65537 cycles -> 2^17 CPU rows
     proof = gpu_prove(ctx, oracle, t)
     assert oracle.verify(proof, t.preprocessed) == 0
+    assert_matches_golden(proof, "fib_2p17")
 
 
 import json
@@ -180,11 +187,12 @@ def test_prove_mixed_chip_program(ctx, oracle):
     proof = gpu_prove(ctx, oracle, t)
     assert proof == ref.cbor()
     assert oracle.verify(proof, t.preprocessed) == 0
-    # larger instance: verifier accepts (oracle prover not run)
+    # larger instance: verifier accepts, bytes equal to the recorded oracle proof
     t2 = vb.run_program(mixed_program(20000), initial_fp=0x1000)
     assert t2.main[0].shape[0] == 1 << 18
     p2 = gpu_prove(ctx, oracle, t2)
     assert oracle.verify(p2, t2.preprocessed) == 0
+    assert_matches_golden(p2, "mixed_20000")
 
 
 def test_prove_config5_program(ctx, oracle):
@@ -202,11 +210,13 @@ def test_prove_config5_program(ctx, oracle):
     assert t2.main[0].shape[0] == 1 << 18
     p2 = gpu_prove(ctx, oracle, t2)
     assert oracle.verify(p2, t2.preprocessed) == 0
+    assert_matches_golden(p2, "config5_16000")
 
 
 def test_prove_full_size_2p22_verifies(ctx, oracle):
-    """BASELINE config 3 at full size (Fibonacci, 2^22 CPU rows, 2^24 memory rows): both verifiers accept the proof,
-    and a second run yields the same bytes (the proof is a pure function of the traces and the challenger)."""
+    """BASELINE config 3 at full size (Fibonacci, 2^22 CPU rows, 2^24 memory rows): both verifiers accept the proof, its
+    bytes are the recorded oracle proof's, and a second run yields the same bytes (the proof is a pure function of the traces
+    and the challenger)."""
     import valida_b200 as vb
 
     n = ((1 << 22) - 17) // 7
@@ -216,6 +226,7 @@ def test_prove_full_size_2p22_verifies(ctx, oracle):
     proof = vb.prove_machine(cfg, t)
     assert oracle.verify(proof, t.preprocessed) == 0
     vb.verify_machine(cfg, proof, t.preprocessed)
+    assert_matches_golden(proof, "fib_2p22")
     assert vb.prove_machine(cfg, t) == proof
 
 
