@@ -98,7 +98,8 @@ int32_t vgpu_dmat_download(vgpu_ctx* ctx, const vgpu_dmat* m, int32_t repr, uint
  * 4-byte aligned, and a view whose element indices or byte addresses overflow 64 bits.  4 bytes is all the kernels that read
  * traces assume: the LDE's NTT passes, the LogUp sweeps, the check sweep and the import / export kernels load and store single
  * 32-bit words at any column stride; the vector loads of the library (leaf hashing, openings, row-shard exchanges) read only
- * buffers the library allocated itself.  Empty views (height or width 0) are handled as the uploads handle empty matrices. */
+ * buffers the library allocated itself (a borrowed row shard that is not 16-byte aligned, or whose column stride is not a multiple
+ * of 4, is handed over by an exchange kernel that loads single words).  Empty views (height or width 0) are handled as the uploads handle empty matrices. */
 typedef struct vgpu_dev_matrix {
     const uint32_t* data;      /* device pointer on the context's device */
     uint64_t height, width;
@@ -115,12 +116,33 @@ int32_t vgpu_dmat_import_rows(vgpu_ctx* ctx, const vgpu_dev_matrix* src, int32_t
 /* Zero-copy: the caller's column-major Montgomery buffer (element (r, c) at data[c * col_stride + r], col_stride >= height) becomes
  * a matrix that the library reads in place.  One read pass checks that every word is below p (synchronises once, copies nothing).
  * The library never writes or frees the buffer (vgpu_ntt_batch refuses a borrowed matrix); the caller keeps it alive and unchanged
- * until vgpu_dmat_free of the handle AND until every call that read it has returned.  Whole matrices only (not a rank's row shard). */
+ * until vgpu_dmat_free of the handle AND until every call that read it has returned.  Whole matrices only (a rank's row shard:
+ * vgpu_dmat_borrow_local). */
 int32_t vgpu_dmat_borrow(vgpu_ctx* ctx, uint32_t* data, uint64_t height, uint64_t width, uint64_t col_stride, vgpu_dmat** out);
 /* Device twin of vgpu_dmat_download: writes the rows this rank holds at their place in the caller's height x width view, in natural
  * row order (a bit-reversed matrix, e.g. quotient chunks, is mapped by the kernel), on the context's stream with no host
  * synchronisation (vgpu_ctx_record_event orders a consumer after it).  Refuses what the download refuses. */
 int32_t vgpu_dmat_export(vgpu_ctx* ctx, const vgpu_dmat* m, int32_t repr, const vgpu_dev_matrix* dst);
+/* Row shards in caller device memory: each rank of a split proof holds only its LOCAL rows of a matrix of logical height `height`,
+ * [r * height / N, (r + 1) * height / N) on rank r of N when the trace is tall enough to be split (the rule of vgpu_dmat_upload_rows
+ * and vgpu_dmat_import_rows), otherwise all of [0, height) (a short trace, a context without a communicator, sharding off).  So
+ * code written against these calls runs unchanged on one GPU and on N.
+ *   vgpu_ctx_local_rows: the rows this rank must supply for a matrix of this height, before anything exists; equal to what
+ *     vgpu_dmat_local_rows reports of the matrices the calls below create.
+ *   vgpu_dmat_import_local: `local` views this rank's rows only (local->height == rows, any strides; local row i is global row
+ *     row0 + i).  A copy into a library-owned matrix, equal word for word to vgpu_dmat_import_rows of a whole-matrix view of the same
+ *     words.  Synchronises once, to read the verdict.
+ *   vgpu_dmat_borrow_local: zero-copy, as vgpu_dmat_borrow: local row i of column c at data[c * col_stride + i], col_stride >= rows,
+ *     Montgomery words, 4-byte alignment; the same lifetime contract (never written or freed by the library).
+ *   vgpu_dmat_export_local: writes the rows this rank holds into a rows x width view (local row i at row i), on the context's stream
+ *     with no host synchronisation; of a whole matrix it is vgpu_dmat_export.  Refuses what vgpu_dmat_export refuses.
+ * Before anything is enqueued the calls refuse a view whose height is not this rank's row count (the message names the expected row0
+ * and rows), col_stride < rows for a borrow, and whatever the calls above refuse of a view.  A word not below p fails the call on the
+ * rank that holds it, naming its GLOBAL row (row0 + local row) and column; the verdict is not collective. */
+int32_t vgpu_ctx_local_rows(const vgpu_ctx* ctx, uint64_t height, uint64_t* row0, uint64_t* rows);
+int32_t vgpu_dmat_import_local(vgpu_ctx* ctx, const vgpu_dev_matrix* local, uint64_t height, int32_t repr, vgpu_dmat** out);
+int32_t vgpu_dmat_borrow_local(vgpu_ctx* ctx, uint32_t* data, uint64_t height, uint64_t width, uint64_t col_stride, vgpu_dmat** out);
+int32_t vgpu_dmat_export_local(vgpu_ctx* ctx, const vgpu_dmat* m, int32_t repr, const vgpu_dev_matrix* dst);
 /* Logical dimensions (of the whole matrix, also for a shard). */
 int32_t vgpu_dmat_dims(const vgpu_dmat* m, uint64_t* height, uint64_t* width);
 /* The rows held here; returns 0 = whole matrix, 1 = row shard, 2 = column share. */

@@ -124,6 +124,10 @@ extern "C" {
     pub fn vgpu_dmat_import_rows(ctx: *mut vgpu_ctx, src: *const vgpu_dev_matrix, repr: i32, out: *mut *mut vgpu_dmat) -> i32;
     pub fn vgpu_dmat_borrow(ctx: *mut vgpu_ctx, data: *mut u32, height: u64, width: u64, col_stride: u64, out: *mut *mut vgpu_dmat) -> i32;
     pub fn vgpu_dmat_export(ctx: *mut vgpu_ctx, m: *const vgpu_dmat, repr: i32, dst: *const vgpu_dev_matrix) -> i32;
+    pub fn vgpu_ctx_local_rows(ctx: *const vgpu_ctx, height: u64, row0: *mut u64, rows: *mut u64) -> i32;
+    pub fn vgpu_dmat_import_local(ctx: *mut vgpu_ctx, local: *const vgpu_dev_matrix, height: u64, repr: i32, out: *mut *mut vgpu_dmat) -> i32;
+    pub fn vgpu_dmat_borrow_local(ctx: *mut vgpu_ctx, data: *mut u32, height: u64, width: u64, col_stride: u64, out: *mut *mut vgpu_dmat) -> i32;
+    pub fn vgpu_dmat_export_local(ctx: *mut vgpu_ctx, m: *const vgpu_dmat, repr: i32, dst: *const vgpu_dev_matrix) -> i32;
     pub fn vgpu_dmat_dims(m: *const vgpu_dmat, height: *mut u64, width: *mut u64) -> i32;
     pub fn vgpu_dmat_local_rows(m: *const vgpu_dmat, row0: *mut u64, rows: *mut u64) -> i32;
     pub fn vgpu_dmat_free(m: *mut vgpu_dmat);

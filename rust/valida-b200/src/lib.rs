@@ -145,6 +145,23 @@ impl DMat<'_> {
         let raw = dst.raw();
         ctx.check(sys::vgpu_dmat_export(ctx.raw, self.raw, repr.raw(), &raw))
     }
+
+    /// The rows held on this rank (`row0`, `rows`): all of them unless the matrix is a row shard of a split proof.
+    pub fn local_rows(&self) -> (u64, u64) {
+        let (mut row0, mut rows) = (0u64, 0u64);
+        unsafe { sys::vgpu_dmat_local_rows(self.raw, &mut row0, &mut rows) };
+        (row0, rows)
+    }
+
+    /// Writes the rows held on this rank into the caller's `rows x width` view (local row `i` at row `i`), in `repr` words, on the
+    /// context's stream without a host synchronisation; of a whole matrix the same as [`DMat::export_device`].
+    ///
+    /// # Safety
+    /// As for [`DMat::export_device`].
+    pub unsafe fn export_device_local(&self, ctx: &Context, repr: Repr, dst: &DeviceView) -> Result<()> {
+        let raw = dst.raw();
+        ctx.check(sys::vgpu_dmat_export_local(ctx.raw, self.raw, repr.raw(), &raw))
+    }
 }
 
 impl Drop for DMat<'_> {
@@ -287,6 +304,41 @@ impl Context {
     pub unsafe fn borrow_device(&self, data: *mut u32, height: u64, width: u64, col_stride: u64) -> Result<DMat<'_>> {
         let mut out: *mut vgpu_dmat = ptr::null_mut();
         self.check(sys::vgpu_dmat_borrow(self.raw, data, height, width, col_stride, &mut out))?;
+        Ok(DMat { raw: out, _ctx: PhantomData })
+    }
+
+    /// The rows `(row0, rows)` this rank holds of a matrix of logical height `height`, and so must supply to
+    /// [`Context::import_device_local`] and [`Context::borrow_device_local`]: its run of a trace tall enough to be split, otherwise
+    /// `(0, height)`.  Known before any matrix exists, so each rank can fill only its own rows.
+    pub fn local_rows(&self, height: u64) -> (u64, u64) {
+        let (mut row0, mut rows) = (0u64, 0u64);
+        unsafe { sys::vgpu_ctx_local_rows(self.raw, height, &mut row0, &mut rows) };
+        (row0, rows)
+    }
+
+    /// [`Context::import_device`] of this rank's rows only: `local` views the `rows` of [`Context::local_rows`]`(height)` (any
+    /// strides), local row `i` being row `row0 + i` of the matrix.  The result equals [`Context::import_device_rows`] of a view of
+    /// the whole matrix; a word not below p fails on this rank only, naming its row in the whole matrix.
+    ///
+    /// # Safety
+    /// As for [`Context::import_device`].
+    pub unsafe fn import_device_local(&self, local: &DeviceView, height: u64, repr: Repr) -> Result<DMat<'_>> {
+        let raw = local.raw();
+        let mut out: *mut vgpu_dmat = ptr::null_mut();
+        self.check(sys::vgpu_dmat_import_local(self.raw, &raw, height, repr.raw(), &mut out))?;
+        Ok(DMat { raw: out, _ctx: PhantomData })
+    }
+
+    /// [`Context::borrow_device`] of this rank's rows only: `data` holds the `rows` of [`Context::local_rows`]`(height)`, column-major
+    /// Montgomery (local row `i` of column `c` at `data[c * col_stride + i]`, `col_stride >= rows`, 4-byte aligned), and is proven
+    /// from in place.
+    ///
+    /// # Safety
+    /// As for [`Context::borrow_device`]: the library never writes or frees `data`; the caller keeps it allocated and unchanged until
+    /// the `DMat` is dropped AND every call that took it has returned, and orders writes to it before the context's stream.
+    pub unsafe fn borrow_device_local(&self, data: *mut u32, height: u64, width: u64, col_stride: u64) -> Result<DMat<'_>> {
+        let mut out: *mut vgpu_dmat = ptr::null_mut();
+        self.check(sys::vgpu_dmat_borrow_local(self.raw, data, height, width, col_stride, &mut out))?;
         Ok(DMat { raw: out, _ctx: PhantomData })
     }
 

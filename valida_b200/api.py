@@ -65,6 +65,10 @@ def _load():
         "vgpu_dmat_import_rows": (C.c_int32, [vp, C.POINTER(_DevMatrix), C.c_int32, C.POINTER(vp)]),
         "vgpu_dmat_borrow": (C.c_int32, [vp, vp, u64, u64, u64, C.POINTER(vp)]),
         "vgpu_dmat_export": (C.c_int32, [vp, vp, C.c_int32, C.POINTER(_DevMatrix)]),
+        "vgpu_ctx_local_rows": (C.c_int32, [vp, u64, C.POINTER(u64), C.POINTER(u64)]),
+        "vgpu_dmat_import_local": (C.c_int32, [vp, C.POINTER(_DevMatrix), u64, C.c_int32, C.POINTER(vp)]),
+        "vgpu_dmat_borrow_local": (C.c_int32, [vp, vp, u64, u64, u64, C.POINTER(vp)]),
+        "vgpu_dmat_export_local": (C.c_int32, [vp, vp, C.c_int32, C.POINTER(_DevMatrix)]),
         "vgpu_dmat_dims": (C.c_int32, [vp, C.POINTER(u64), C.POINTER(u64)]),
         "vgpu_dmat_free": (None, [vp]),
         "vgpu_ntt_batch": (C.c_int32, [vp, vp, C.c_int32]),
@@ -265,19 +269,48 @@ class Context:
         tensor on its own device); otherwise like import_tensor."""
         return self._import_tensor(lib().vgpu_dmat_import_rows, "import_tensor_rows", t, repr)
 
+    def _borrow_tensor(self, what, t, call):
+        v = _tensor_view(self, t, what)
+        if v.row_stride != 1:
+            raise ValueError("%s: the tensor is not column-major (stride(0) = %d, must be 1)" % (what, v.row_stride))
+        self._wait_for_torch(t.device)
+        out = C.c_void_p()
+        self.check(call(v, out))
+        m = DeviceMatrix(self, out)
+        m._tensor = t
+        return m
+
     def borrow_tensor(self, t):
         """Zero-copy: a column-major tensor of Montgomery words (stride(0) == 1, stride(1) >= shape(0)) becomes a DeviceMatrix read in
         place.  Its words are checked once (below p); it is never written, and the DeviceMatrix keeps a reference to it.  Leave it
         unchanged while the DeviceMatrix is alive."""
-        v = _tensor_view(self, t, "borrow_tensor")
-        if v.row_stride != 1:
-            raise ValueError("borrow_tensor: the tensor is not column-major (stride(0) = %d, must be 1)" % v.row_stride)
-        self._wait_for_torch(t.device)
-        out = C.c_void_p()
-        self.check(lib().vgpu_dmat_borrow(self._h, v.data, v.height, v.width, v.col_stride, C.byref(out)))
-        m = DeviceMatrix(self, out)
-        m._tensor = t
-        return m
+        return self._borrow_tensor("borrow_tensor", t,
+                                   lambda v, out: lib().vgpu_dmat_borrow(self._h, v.data, v.height, v.width, v.col_stride, C.byref(out)))
+
+    # ---- row shards in caller device memory: each rank holds only its own rows (include/valida_b200.h, vgpu_dmat_*_local) ----
+    def local_rows(self, height):
+        """(row0, rows): the rows of a matrix of logical height `height` that this rank holds, and so must supply to
+        import_tensor_local / borrow_tensor_local: its run of a trace tall enough to be split, otherwise (0, height)."""
+        r0, n = C.c_uint64(), C.c_uint64()
+        self.check(lib().vgpu_ctx_local_rows(self._h, height, C.byref(r0), C.byref(n)))
+        return int(r0.value), int(n.value)
+
+    def import_tensor_local(self, t, height, repr=REPR_CANONICAL):
+        """import_tensor of this rank's rows only: `t` has local_rows(height)[1] rows (any strides), local row i being row row0 + i of
+        the matrix.  Equal to import_tensor_rows of the whole tensor; a word not below p is named by its row in the whole matrix."""
+        return self._import_tensor(lambda h, v, r, out: lib().vgpu_dmat_import_local(h, v, height, r, out), "import_tensor_local", t, repr)
+
+    def borrow_tensor_local(self, t, height):
+        """borrow_tensor of this rank's rows only: a column-major Montgomery tensor of local_rows(height)[1] rows (stride(0) == 1,
+        stride(1) >= its rows, 4-byte alignment).  Read in place and never written; the DeviceMatrix keeps a reference to it."""
+        def call(v, out):
+            row0, rows = self.local_rows(height)
+            if v.height != rows:
+                raise ValueError("borrow_tensor_local: the tensor has %d rows, but of a matrix of height %d this rank holds rows = %d "
+                                 "starting at row0 = %d" % (v.height, height, rows, row0))
+            return lib().vgpu_dmat_borrow_local(self._h, v.data, height, v.width, v.col_stride, C.byref(out))
+
+        return self._borrow_tensor("borrow_tensor_local", t, call)
 
     def host_register(self, array):
         """Page-lock a numpy array the caller will prove from repeatedly (its uploads then overlap the commits)."""
@@ -378,6 +411,22 @@ class DeviceMatrix:
             raise ValueError("to_tensor: out has shape %s, the matrix is %d x %d" % (tuple(out.shape), h, w))
         self.ctx._wait_for_torch(dev)            # out may have been allocated or last used on torch's stream
         self.ctx.check(lib().vgpu_dmat_export(self.ctx._h, self._h, repr, C.byref(v)))
+        self.ctx._torch_waits(dev)
+        return out
+
+    def local_to_tensor(self, repr=REPR_CANONICAL, out=None):
+        """The rows held on this rank (local_rows()) as a (rows, w) torch.int32 CUDA tensor, local row i at row i, or written into
+        `out` (int32 or uint32, any strides); of a whole matrix the same as to_tensor.  Ordered as to_tensor."""
+        import torch
+
+        _, rows = self.local_rows()
+        w = self.shape[1]
+        dev = torch.device("cuda", self.ctx.device)
+        if out is None:
+            out = torch.empty((rows, w), dtype=torch.int32, device=dev)
+        v = _tensor_view(self.ctx, out, "local_to_tensor")
+        self.ctx._wait_for_torch(dev)
+        self.ctx.check(lib().vgpu_dmat_export_local(self.ctx._h, self._h, repr, C.byref(v)))
         self.ctx._torch_waits(dev)
         return out
 

@@ -301,15 +301,35 @@ static int32_t check_device_view(vgpu_ctx* ctx, const char* what, const uint32_t
     }
     return 0;
 }
-static int32_t import_view(vgpu_ctx* ctx, const char* what, const vgpu_dev_matrix* src, int32_t repr, bool rows, vgpu_dmat** out) {
+// The rows this rank holds of a matrix of logical height h: its run of a trace tall enough to be split (where vg_dmat_alloc_dist
+// puts a VG_ROWS shard, the rule of vgpu_dmat_upload_rows), otherwise all of them.  Returns whether the matrix is split.
+static bool local_rows_of(const vgpu_ctx* ctx, uint64_t h, uint64_t* row0, uint64_t* rows) {
+    const bool split = vg_split_rows(ctx, 2 * h);
+    *rows = split ? h / (uint64_t)ctx->comm_size : h;
+    *row0 = split ? *rows * (uint64_t)ctx->comm_rank : 0;
+    return split;
+}
+static int32_t check_local_height(vgpu_ctx* ctx, const char* what, uint64_t view_rows, uint64_t h) {
+    uint64_t row0, rows;
+    local_rows_of(ctx, h, &row0, &rows);
+    if (view_rows != rows)
+        VG_FAIL(ctx, "%s: the view has %llu rows, but of a matrix of height %llu rank %d holds rows = %llu starting at row0 = %llu", what,
+                (unsigned long long)view_rows, (unsigned long long)h, ctx->comm_rank, (unsigned long long)rows, (unsigned long long)row0);
+    return 0;
+}
+// rows: keep this rank's run of a trace tall enough to be split.  local: `src` views those rows only (of a matrix of height h);
+// otherwise it views the whole matrix (h == src->height).
+static int32_t import_view(vgpu_ctx* ctx, const char* what, const vgpu_dev_matrix* src, uint64_t h, int32_t repr, bool rows, bool local, vgpu_dmat** out) {
     if (!src || !out) VG_FAIL(ctx, "%s: null argument", what);
     VG_TRY(vg_enter(ctx));
-    const uint64_t h = src->height, w = src->width;
-    if (h && w) VG_TRY(check_device_view(ctx, what, src->data, h, w, src->row_stride, src->col_stride));
+    const uint64_t w = src->width;
+    if (local) VG_TRY(check_local_height(ctx, what, src->height, h));
+    if (src->height && w) VG_TRY(check_device_view(ctx, what, src->data, src->height, w, src->row_stride, src->col_stride));
     vgpu_dmat* m = nullptr;
     VG_TRY(rows && vg_split_rows(ctx, 2 * h) ? vg_dmat_alloc_dist(ctx, VG_ROWS, h, w, false, &m) : vg_dmat_alloc(ctx, h, w, &m));
     unsigned long long bad = ~0ull;
-    int32_t rc = vg_import_strided(ctx, src->data + m->row0 * src->row_stride, m->h, m->w, src->row_stride, src->col_stride, repr, m, &bad);
+    const uint32_t* first = local ? src->data : src->data + m->row0 * src->row_stride;
+    int32_t rc = vg_import_strided(ctx, first, m->h, m->w, src->row_stride, src->col_stride, repr, m, &bad);
     const uint64_t row0 = m->row0;
     if (rc == 0 && bad == ~0ull) { *out = m; return 0; }
     vgpu_dmat_free(m);
@@ -318,42 +338,73 @@ static int32_t import_view(vgpu_ctx* ctx, const char* what, const vgpu_dev_matri
             (unsigned long long)(row0 + bad / w), (unsigned long long)(bad % w), bb::P);
 }
 int32_t vgpu_dmat_import(vgpu_ctx* ctx, const vgpu_dev_matrix* src, int32_t repr, vgpu_dmat** out) {
-    return import_view(ctx, "dmat_import", src, repr, false, out);
+    return import_view(ctx, "dmat_import", src, src ? src->height : 0, repr, false, false, out);
 }
 int32_t vgpu_dmat_import_rows(vgpu_ctx* ctx, const vgpu_dev_matrix* src, int32_t repr, vgpu_dmat** out) {
-    return import_view(ctx, "dmat_import_rows", src, repr, true, out);
+    return import_view(ctx, "dmat_import_rows", src, src ? src->height : 0, repr, true, false, out);
 }
-int32_t vgpu_dmat_borrow(vgpu_ctx* ctx, uint32_t* data, uint64_t height, uint64_t width, uint64_t col_stride, vgpu_dmat** out) {
-    if (!out) VG_FAIL(ctx, "dmat_borrow: null argument");
+int32_t vgpu_dmat_import_local(vgpu_ctx* ctx, const vgpu_dev_matrix* local, uint64_t height, int32_t repr, vgpu_dmat** out) {
+    return import_view(ctx, "dmat_import_local", local, height, repr, true, true, out);
+}
+// local: `data` holds this rank's rows of a matrix of height `height` (a VG_ROWS shard when the matrix is split), else all of it.
+static int32_t borrow_view(vgpu_ctx* ctx, const char* what, uint32_t* data, uint64_t height, uint64_t width, uint64_t col_stride, bool local, vgpu_dmat** out) {
+    if (!out) VG_FAIL(ctx, "%s: null argument", what);
     VG_TRY(vg_enter(ctx));
-    if (col_stride < height) VG_FAIL(ctx, "dmat_borrow: column stride %llu is below the height %llu", (unsigned long long)col_stride, (unsigned long long)height);
-    if (height && width) {
-        VG_TRY(check_device_view(ctx, "dmat_borrow", data, height, width, 1, col_stride));
+    uint64_t row0 = 0, rows = height;
+    const bool split = local && local_rows_of(ctx, height, &row0, &rows);
+    if (col_stride < rows) VG_FAIL(ctx, "%s: column stride %llu is below the height %llu", what, (unsigned long long)col_stride, (unsigned long long)rows);
+    if (rows && width) {
+        VG_TRY(check_device_view(ctx, what, data, rows, width, 1, col_stride));
         unsigned long long bad = ~0ull;
-        VG_TRY(vg_import_strided(ctx, data, height, width, 1, col_stride, VGPU_REPR_MONTY_R32, nullptr, &bad));
+        VG_TRY(vg_import_strided(ctx, data, rows, width, 1, col_stride, VGPU_REPR_MONTY_R32, nullptr, &bad));
         if (bad != ~0ull)
-            VG_FAIL(ctx, "dmat_borrow: the word at row %llu, column %llu is not below p = %u (not a Montgomery BabyBear word)",
-                    (unsigned long long)(bad / width), (unsigned long long)(bad % width), bb::P);
+            VG_FAIL(ctx, "%s: the word at row %llu, column %llu is not below p = %u (not a Montgomery BabyBear word)", what,
+                    (unsigned long long)(row0 + bad / width), (unsigned long long)(bad % width), bb::P);
     }
     vgpu_dmat* m = new (std::nothrow) vgpu_dmat();
     if (!m) VG_FAIL(ctx, "out of host memory");
-    m->ctx = ctx; m->d = data; m->h = m->gh = height; m->w = m->gw = width; m->col_stride = col_stride;
+    m->ctx = ctx; m->d = data; m->h = rows; m->gh = height; m->w = m->gw = width; m->col_stride = col_stride;
+    m->row0 = row0; m->dist = split ? VG_ROWS : VG_FULL;
     m->owns = false;
     *out = m;
     return 0;
 }
-int32_t vgpu_dmat_export(vgpu_ctx* ctx, const vgpu_dmat* m, int32_t repr, const vgpu_dev_matrix* dst) {
-    if (!m || !dst) VG_FAIL(ctx, "dmat_export: null argument");
+int32_t vgpu_dmat_borrow(vgpu_ctx* ctx, uint32_t* data, uint64_t height, uint64_t width, uint64_t col_stride, vgpu_dmat** out) {
+    return borrow_view(ctx, "dmat_borrow", data, height, width, col_stride, false, out);
+}
+int32_t vgpu_dmat_borrow_local(vgpu_ctx* ctx, uint32_t* data, uint64_t height, uint64_t width, uint64_t col_stride, vgpu_dmat** out) {
+    return borrow_view(ctx, "dmat_borrow_local", data, height, width, col_stride, true, out);
+}
+// local: the view holds this rank's rows only (local row i at view row i); otherwise the whole matrix, each row at its logical place.
+static int32_t export_view(vgpu_ctx* ctx, const char* what, const vgpu_dmat* m, int32_t repr, const vgpu_dev_matrix* dst, bool local) {
+    if (!m || !dst) VG_FAIL(ctx, "%s: null argument", what);
     VG_TRY(vg_enter(ctx));
-    if (m->dist == VG_COLS) VG_FAIL(ctx, "dmat_export: column shares are internal to a commit");
-    if (m->dist == VG_ROWS && m->bitrev_rows) VG_FAIL(ctx, "dmat_export: a bit-reversed row shard has no contiguous natural-order image");
-    if (dst->height != m->gh || dst->width != m->gw)
-        VG_FAIL(ctx, "dmat_export: the view is %llu x %llu, the matrix %llu x %llu", (unsigned long long)dst->height, (unsigned long long)dst->width,
+    if (m->dist == VG_COLS) VG_FAIL(ctx, "%s: column shares are internal to a commit", what);
+    if (m->dist == VG_ROWS && m->bitrev_rows) VG_FAIL(ctx, "%s: a bit-reversed row shard has no contiguous natural-order image", what);
+    if (local && (dst->height != m->h || dst->width != m->w))
+        VG_FAIL(ctx, "%s: the view is %llu x %llu, but of the %llu x %llu matrix rank %d holds rows = %llu starting at row0 = %llu", what,
+                (unsigned long long)dst->height, (unsigned long long)dst->width, (unsigned long long)m->gh, (unsigned long long)m->gw, ctx->comm_rank,
+                (unsigned long long)m->h, (unsigned long long)m->row0);
+    if (!local && (dst->height != m->gh || dst->width != m->gw))
+        VG_FAIL(ctx, "%s: the view is %llu x %llu, the matrix %llu x %llu", what, (unsigned long long)dst->height, (unsigned long long)dst->width,
                 (unsigned long long)m->gh, (unsigned long long)m->gw);
     if (m->h == 0 || m->w == 0) return 0;
-    VG_TRY(check_device_view(ctx, "dmat_export", dst->data, dst->height, dst->width, dst->row_stride, dst->col_stride));
+    VG_TRY(check_device_view(ctx, what, dst->data, dst->height, dst->width, dst->row_stride, dst->col_stride));
     VG_TRY(vg_dmat_materialize(ctx, m));
-    return vg_export_strided(ctx, m, repr, const_cast<uint32_t*>(dst->data), dst->row_stride, dst->col_stride);
+    vgpu_dmat at = *m;                  // export_kernel writes stored row r at view row at.row0 + r
+    if (local) at.row0 = 0;
+    return vg_export_strided(ctx, &at, repr, const_cast<uint32_t*>(dst->data), dst->row_stride, dst->col_stride);
+}
+int32_t vgpu_dmat_export(vgpu_ctx* ctx, const vgpu_dmat* m, int32_t repr, const vgpu_dev_matrix* dst) {
+    return export_view(ctx, "dmat_export", m, repr, dst, false);
+}
+int32_t vgpu_dmat_export_local(vgpu_ctx* ctx, const vgpu_dmat* m, int32_t repr, const vgpu_dev_matrix* dst) {
+    return export_view(ctx, "dmat_export_local", m, repr, dst, true);
+}
+int32_t vgpu_ctx_local_rows(const vgpu_ctx* ctx, uint64_t height, uint64_t* row0, uint64_t* rows) {
+    if (!ctx || !row0 || !rows) return -1;
+    local_rows_of(ctx, height, row0, rows);
+    return 0;
 }
 int32_t vgpu_dmat_dims(const vgpu_dmat* m, uint64_t* height, uint64_t* width) { *height = m->gh; *width = m->gw; return 0; }
 int32_t vgpu_dmat_local_rows(const vgpu_dmat* m, uint64_t* row0, uint64_t* rows) { *row0 = m->row0; *rows = m->h; return m->dist; }

@@ -30,6 +30,19 @@ __global__ void __launch_bounds__(256) rows_to_cols_kernel(const __grid_constant
     uint4* o = reinterpret_cast<uint4*>(p.dst[d] + (uint64_t)(c - p.c0[d]) * p.gh + p.row0);
     for (uint64_t i = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x; i < n4; i += (uint64_t)gridDim.x * blockDim.x) o[i] = __ldg(s + i);
 }
+// The same hand-over from a row shard whose columns are not 16-byte aligned (a borrowed caller buffer: 4-byte alignment, any column
+// stride): four 32-bit loads per 16-byte chunk of a column, one 16-byte store into the peer's column buffer, which is aligned (a
+// symmetric-heap allocation, gh and row0 multiples of 4).
+__global__ void __launch_bounds__(256) rows_to_cols_scalar_kernel(const __grid_constant__ R2CParams p) {
+    const uint32_t c = blockIdx.y;
+    uint32_t d = 0;
+    while (d + 1 < p.nranks && c >= p.c0[d + 1]) d++;
+    const uint64_t n4 = p.hl >> 2;
+    const uint32_t* s = p.src + (uint64_t)c * p.scs;
+    uint4* o = reinterpret_cast<uint4*>(p.dst[d] + (uint64_t)(c - p.c0[d]) * p.gh + p.row0);
+    for (uint64_t i = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x; i < n4; i += (uint64_t)gridDim.x * blockDim.x)
+        o[i] = make_uint4(__ldg(s + 4 * i), __ldg(s + 4 * i + 1), __ldg(s + 4 * i + 2), __ldg(s + 4 * i + 3));
+}
 
 struct C2RParams {
     const uint32_t* src; uint64_t H, hs;        // local columns [c0, c1) at stride H; shard height hs = H / nranks
@@ -49,9 +62,12 @@ __global__ void __launch_bounds__(256) cols_to_rows_kernel(const __grid_constant
 
 // rows: this rank's row shard (VG_ROWS) of a gh x gw matrix.  cols_symm: a symmetric-heap buffer (the same size on every rank, room
 // for the widest share); after the barrier that follows, it holds this rank's columns [col_begin[rank], col_begin[rank + 1]) at stride gh.
+// A shard the library allocated has 16-byte aligned columns and is read with vector loads; a borrowed one may have any column stride
+// and a 4-byte aligned base, and is read a word at a time.
 int32_t vg_exchange_rows_to_cols(vgpu_ctx* ctx, const vgpu_dmat* rows, uint32_t* cols_symm, const uint32_t* col_begin /* comm_size + 1 */) {
     const int G = ctx->comm_size;
-    if (rows->dist != VG_ROWS || (rows->h & 3) || (rows->row0 & 3) || (rows->col_stride & 3)) VG_FAIL(ctx, "exchange: row shard of %llu rows at %llu is not 16-byte aligned", (unsigned long long)rows->h, (unsigned long long)rows->row0);
+    if (rows->dist != VG_ROWS || (rows->h & 3) || (rows->row0 & 3)) VG_FAIL(ctx, "exchange: row shard of %llu rows at %llu is not 16-byte aligned", (unsigned long long)rows->h, (unsigned long long)rows->row0);
+    const bool vec = ((uintptr_t)rows->d & 15) == 0 && (rows->col_stride & 3) == 0;
     R2CParams p{};
     p.src = rows->d; p.scs = rows->col_stride; p.hl = rows->h; p.gh = rows->gh; p.row0 = rows->row0; p.nranks = (uint32_t)G;
     for (int d = 0; d <= G; d++) p.c0[d] = col_begin[d];
@@ -60,7 +76,8 @@ int32_t vg_exchange_rows_to_cols(vgpu_ctx* ctx, const vgpu_dmat* rows, uint32_t*
     unsigned gx = (unsigned)((n4 + 255) / 256);
     if (gx > 64) gx = 64;
     KScope ks(ctx, KC_EXCHANGE, 8.0 * (double)rows->h * (double)rows->gw);
-    rows_to_cols_kernel<<<dim3(gx, (unsigned)rows->gw), 256, 0, ctx->stream>>>(p);
+    if (vec) rows_to_cols_kernel<<<dim3(gx, (unsigned)rows->gw), 256, 0, ctx->stream>>>(p);
+    else rows_to_cols_scalar_kernel<<<dim3(gx, (unsigned)rows->gw), 256, 0, ctx->stream>>>(p);
     VG_LAUNCH_CHECK(ctx);
     ctx->stat_exchange.calls++; ctx->stat_exchange.bytes += 4.0 * (double)rows->h * (double)rows->gw * (G - 1) / G;
     return 0;
