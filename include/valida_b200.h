@@ -90,7 +90,10 @@ int32_t vgpu_dmat_upload(vgpu_ctx* ctx, const vgpu_matrix* host, int32_t repr, v
 /* Split proof (multi-GPU section below): of a trace tall enough to be split a rank keeps ITS contiguous run of rows only;
  * every rank passes the same host matrix.  Shorter traces, and any trace on a lone GPU, are uploaded whole. */
 int32_t vgpu_dmat_upload_rows(vgpu_ctx* ctx, const vgpu_matrix* host, int32_t repr, vgpu_dmat** out);
-/* Writes the rows this rank holds at their place in the caller's height x width row-major buffer. */
+/* Writes the rows this rank holds at their place in the caller's height x width row-major buffer, in natural row order, and leaves
+ * the other rows untouched.  Of a matrix stored with bit-reversed rows (quotient chunks) stored row s goes to row
+ * reverse_bits(s, log2 height); of a row shard of such a matrix (a split proof's quotient chunks) that places this rank's rows
+ * all over the buffer. */
 int32_t vgpu_dmat_download(vgpu_ctx* ctx, const vgpu_dmat* m, int32_t repr, uint32_t* host_row_major_out);
 /* View of caller DEVICE memory (a torch tensor, the output of the caller's own kernels), strides counted in words: row-major is
  * (width, 1), column-major is (1, height), a sub-matrix of a larger buffer has larger strides.  Every call below refuses, before
@@ -121,7 +124,8 @@ int32_t vgpu_dmat_import_rows(vgpu_ctx* ctx, const vgpu_dev_matrix* src, int32_t
 int32_t vgpu_dmat_borrow(vgpu_ctx* ctx, uint32_t* data, uint64_t height, uint64_t width, uint64_t col_stride, vgpu_dmat** out);
 /* Device twin of vgpu_dmat_download: writes the rows this rank holds at their place in the caller's height x width view, in natural
  * row order (a bit-reversed matrix, e.g. quotient chunks, is mapped by the kernel), on the context's stream with no host
- * synchronisation (vgpu_ctx_record_event orders a consumer after it).  Refuses what the download refuses. */
+ * synchronisation (vgpu_ctx_record_event orders a consumer after it).  Refuses what the download refuses, and also a row shard
+ * with bit-reversed rows (its rows have no contiguous natural-order image). */
 int32_t vgpu_dmat_export(vgpu_ctx* ctx, const vgpu_dmat* m, int32_t repr, const vgpu_dev_matrix* dst);
 /* Row shards in caller device memory: each rank of a split proof holds only its LOCAL rows of a matrix of logical height `height`,
  * [r * height / N, (r + 1) * height / N) on rank r of N when the trace is tall enough to be split (the rule of vgpu_dmat_upload_rows

@@ -390,9 +390,15 @@ class DeviceMatrix:
         lib().vgpu_dmat_local_rows(self._h, C.byref(r0), C.byref(n))
         return int(r0.value), int(n.value)
 
-    def download(self, repr=REPR_CANONICAL):
+    def download(self, repr=REPR_CANONICAL, out=None):
+        """The matrix as an (h, w) numpy uint32 array in natural row order, `repr` words.  Of a row shard only the rows this rank holds
+        are written, at their natural rows (those of a bit-reversed shard, such as a split quotient's chunks, are scattered); the other
+        rows are left as they were in `out`, or uninitialised without it."""
         h, w = self.shape
-        out = np.empty((h, w), dtype=np.uint32)
+        if out is None:
+            out = np.empty((h, w), dtype=np.uint32)
+        elif out.shape != (h, w) or out.dtype != np.uint32 or not out.flags.c_contiguous:
+            raise ValueError("download: out must be a C-contiguous (%d, %d) uint32 array" % (h, w))
         self.ctx.check(lib().vgpu_dmat_download(self.ctx._h, self._h, repr, out.ctypes.data_as(C.POINTER(C.c_uint32))))
         return out
 

@@ -263,24 +263,19 @@ int32_t vgpu_dmat_upload_rows(vgpu_ctx* ctx, const vgpu_matrix* host, int32_t re
     return 0;
 }
 // Writes the rows this rank holds (all of them unless the matrix is a row shard) at their place in the caller's
-// gh x gw row-major buffer.
+// gh x gw row-major buffer, in natural row order: stored row s of a matrix with bit-reversed rows (quotient chunks, also their row
+// shards) lands at row reverse_bits(s, log2 gh).  Rows another rank holds are left untouched.
 int32_t vgpu_dmat_download(vgpu_ctx* ctx, const vgpu_dmat* m, int32_t repr, uint32_t* host_row_major_out) {
     VG_TRY(vg_enter(ctx));
     VG_TRY(vg_dmat_materialize(ctx, m));
     if (m->dist == VG_COLS) VG_FAIL(ctx, "dmat_download: column shares are internal to a commit");
-    if (m->dist == VG_ROWS && m->bitrev_rows) VG_FAIL(ctx, "dmat_download: a bit-reversed row shard has no contiguous natural-order image");
-    VG_TRY(vg_download_rowmajor(ctx, m, repr, host_row_major_out + m->row0 * m->gw));
-    if (m->bitrev_rows && m->h > 1) {   // present the logical (natural) row order to the caller
-        int lg = 0; while ((1ull << lg) < m->h) lg++;
-        std::vector<uint32_t> tmp(m->w);
-        for (uint64_t i = 0; i < m->h; i++) {
-            uint64_t j = bb::reverse_bits((uint32_t)i, lg);
-            if (i < j) {
-                uint32_t* a = host_row_major_out + i * m->w; uint32_t* b = host_row_major_out + j * m->w;
-                std::memcpy(tmp.data(), a, m->w * 4); std::memcpy(a, b, m->w * 4); std::memcpy(b, tmp.data(), m->w * 4);
-            }
-        }
-    }
+    if (!m->bitrev_rows || m->gh < 2) return vg_download_rowmajor(ctx, m, repr, host_row_major_out + m->row0 * m->gw);
+    std::vector<uint32_t> stored;
+    try { stored.resize(m->h * m->w); } catch (const std::bad_alloc&) { VG_FAIL(ctx, "out of host memory"); }
+    VG_TRY(vg_download_rowmajor(ctx, m, repr, stored.data()));
+    int lg = 0; while ((1ull << lg) < m->gh) lg++;
+    for (uint64_t i = 0; i < m->h; i++)
+        std::memcpy(host_row_major_out + bb::reverse_bits((uint32_t)(m->row0 + i), lg) * m->w, stored.data() + i * m->w, m->w * 4);
     return 0;
 }
 // ---- caller device memory ----------------------------------------------------------------------------
