@@ -149,7 +149,7 @@ int32_t vgpu_dmat_borrow_local(vgpu_ctx* ctx, uint32_t* data, uint64_t height, u
 int32_t vgpu_dmat_export_local(vgpu_ctx* ctx, const vgpu_dmat* m, int32_t repr, const vgpu_dev_matrix* dst);
 /* Logical dimensions (of the whole matrix, also for a shard). */
 int32_t vgpu_dmat_dims(const vgpu_dmat* m, uint64_t* height, uint64_t* width);
-/* The rows held here; returns 0 = whole matrix, 1 = row shard, 2 = column share. */
+/* The rows held here; returns 0 = whole matrix, 1 = row shard. */
 int32_t vgpu_dmat_local_rows(const vgpu_dmat* m, uint64_t* row0, uint64_t* rows);
 void vgpu_dmat_free(vgpu_dmat* m);
 

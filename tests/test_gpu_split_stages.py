@@ -40,6 +40,8 @@ def _src(name):
 # ---- the host-side rules, restated ---------------------------------------------------------------------------------------
 SPLIT_MIN = int(re.search(r"inline bool vg_split_rows\(const vgpu_ctx\* ctx, uint64_t n\) \{ return vg_sharded\(ctx\) && "
                           r"n >= \(uint64_t\)ctx->comm_size \* (\d+); \}", _src("ctx.h")).group(1))
+TRACE_FACTOR = int(re.search(r"inline VgRun vg_trace_run\(const vgpu_ctx\* ctx, uint64_t h\) \{ return vg_run\(h, ctx->comm_size, "
+                             r"ctx->comm_rank, vg_split_rows\(ctx, (\d+) \* h\)\); \}", _src("ctx.h")).group(1))
 RO_MAXW = int(re.search(r"\bRO_MAXW = (\d+);", _src("open.cu")).group(1))
 
 
@@ -87,17 +89,27 @@ def fri_whole_from(log_max, nranks):
     return n
 
 
-def test_model_matches_the_source():
-    assert SPLIT_MIN == 4096 and RO_MAXW == 96
+def test_model_matches_the_single_definition():
+    assert SPLIT_MIN == 4096 and TRACE_FACTOR == 2 and RO_MAXW == 96
+    # rank r holds stored rows [r n/N, (r+1) n/N) of a split matrix (shard_natural_rows), all n of a whole one
+    assert "return split ? VgRun{rank * (n / nranks), n / nranks, true} : VgRun{0, n, false};" in _src("ctx.h")
+    # the rule is defined in ctx.h alone: every other site asks it, and no column-share distribution is left
+    for d, _, files in os.walk(CSRC):
+        for f in files:
+            path = os.path.join(d, f)
+            if os.path.relpath(path, CSRC) != "ctx.h":
+                src = open(path).read()
+                for name in ("vg_split_rows(", "VG_COLS", "col0", "vg_dmat_alloc_dist"):
+                    assert name not in src, (path, name)
     assert "uint32_t vg_eval_columns_first_coset(uint32_t w) { return (w + 1) / 2; }" in _src("open.cu")
-    assert "const bool split = vg_split_rows(ctx, 2 * main->gh);" in _src("perm.cu")
-    assert "if (!vg_split_rows(ctx, 2 * host->height)) return vgpu_dmat_upload(ctx, host, repr, out);" in _src("api.cu")
-    assert "if (vg_split_rows(ctx, heights[i])) tall.push_back(i);" in _src("api.cu")            # commit: LDEs of 2h rows
+    assert "const VgRun run = vg_trace_run(ctx, main->gh);" in _src("perm.cu")
+    assert "if (!vg_trace_run(ctx, host->height).split) return vgpu_dmat_upload(ctx, host, repr, out);" in _src("api.cu")
+    assert "if (vg_trace_run(ctx, mats[i]->gh).split) tall.push_back(i);" in _src("api.cu")       # commit: LDEs of 2h rows
     assert "const bool split = main_lde->dist == VG_ROWS;" in _src("quotient.cu")
-    assert "VG_TRY(split ? vg_dmat_alloc_dist(ctx, VG_ROWS, h, 10, false, &out) : vg_dmat_alloc(ctx, h, 10, &out));" in _src("quotient.cu")
+    assert "VG_TRY(vg_dmat_alloc_run(ctx, h, 10, split, false, &out));" in _src("quotient.cu")
     assert "out->bitrev_rows = true;" in _src("quotient.cu")
     prover = _src(os.path.join("host", "prover.cc"))
-    assert "if (vg_split_rows(ctx, n)) { v->count = n / ctx->comm_size;" in prover
+    assert "int32_t rowvec_alloc(vgpu_ctx* ctx, uint64_t n, RowVec* v) {\n    const VgRun run = vg_row_run(ctx, n);" in prover
     assert "if (cur.shard() && !next.shard()) {" in prover
 
 

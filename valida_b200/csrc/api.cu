@@ -42,31 +42,14 @@ void vg_free(vgpu_ctx* ctx, void* p) {
     ctx->cached_bytes += bytes;
 }
 
-int32_t vg_dmat_alloc(vgpu_ctx* ctx, uint64_t h, uint64_t w, vgpu_dmat** out) {
+int32_t vg_dmat_alloc_run(vgpu_ctx* ctx, uint64_t gh, uint64_t gw, bool split, bool symm, vgpu_dmat** out) {
     vgpu_dmat* m = new (std::nothrow) vgpu_dmat();
     if (!m) VG_FAIL(ctx, "out of host memory");
-    m->ctx = ctx; m->h = h; m->w = w; m->col_stride = h; m->owns = true;
-    m->gh = h; m->gw = w;
-    int32_t rc = vg_alloc(ctx, (void**)&m->d, h * w * 4);
-    if (rc) { delete m; return rc; }
-    *out = m;
-    return 0;
-}
-
-// The local part of a gh x gw matrix: VG_FULL = all of it; VG_ROWS = this rank's run of gh / comm_size stored rows;
-// VG_COLS = this rank's column share (vg_shard_range of gw).  symm: taken from the symmetric heap (peers store into it).
-int32_t vg_dmat_alloc_dist(vgpu_ctx* ctx, int dist, uint64_t gh, uint64_t gw, bool symm, vgpu_dmat** out) {
-    vgpu_dmat* m = new (std::nothrow) vgpu_dmat();
-    if (!m) VG_FAIL(ctx, "out of host memory");
-    const uint64_t G = (uint64_t)ctx->comm_size, r = (uint64_t)ctx->comm_rank;
-    m->ctx = ctx; m->gh = gh; m->gw = gw; m->dist = dist; m->owns = true; m->symm = symm;
-    m->h = gh; m->w = gw;
-    if (dist == VG_ROWS) { m->h = gh / G; m->row0 = r * m->h; }
-    else if (dist == VG_COLS) { uint64_t a, b; vg_shard_range(gw, (int)G, (int)r, &a, &b); m->col0 = a; m->w = b - a; }
-    m->col_stride = m->h;
-    size_t words = m->h * m->w;
-    if (dist == VG_COLS) words = m->h * ((gw + G - 1) / G);       // the same size on every rank
-    int32_t rc = symm ? vg_symm_alloc(ctx, (void**)&m->d, words * 4) : vg_alloc(ctx, (void**)&m->d, words * 4);
+    const VgRun run = vg_run(gh, ctx->comm_size, ctx->comm_rank, split);
+    m->ctx = ctx; m->gh = gh; m->gw = gw; m->dist = split ? VG_ROWS : VG_FULL; m->owns = true; m->symm = symm;
+    m->h = m->col_stride = run.count; m->w = gw; m->row0 = run.begin;
+    const size_t bytes = m->h * m->w * 4;
+    int32_t rc = symm ? vg_symm_alloc(ctx, (void**)&m->d, bytes) : vg_alloc(ctx, (void**)&m->d, bytes);
     if (rc) { delete m; return rc; }
     *out = m;
     return 0;
@@ -253,10 +236,10 @@ int32_t vgpu_dmat_upload(vgpu_ctx* ctx, const vgpu_matrix* host, int32_t repr, v
 // matrix, or at least its own rows of it); shorter traces are uploaded whole.  The handle reports the logical dimensions.
 int32_t vgpu_dmat_upload_rows(vgpu_ctx* ctx, const vgpu_matrix* host, int32_t repr, vgpu_dmat** out) {
     if (!host || !out) VG_FAIL(ctx, "dmat_upload_rows: null argument");
-    if (!vg_split_rows(ctx, 2 * host->height)) return vgpu_dmat_upload(ctx, host, repr, out);
+    if (!vg_trace_run(ctx, host->height).split) return vgpu_dmat_upload(ctx, host, repr, out);
     VG_TRY(vg_enter(ctx));
     vgpu_dmat* m = nullptr;
-    VG_TRY(vg_dmat_alloc_dist(ctx, VG_ROWS, host->height, host->width, false, &m));
+    VG_TRY(vg_dmat_alloc_run(ctx, host->height, host->width, true, false, &m));
     int32_t rc = vg_upload_rowmajor(ctx, host->data + m->row0 * host->width, m->h, m->w, repr, m);
     if (rc) { vgpu_dmat_free(m); return rc; }
     *out = m;
@@ -268,7 +251,6 @@ int32_t vgpu_dmat_upload_rows(vgpu_ctx* ctx, const vgpu_matrix* host, int32_t re
 int32_t vgpu_dmat_download(vgpu_ctx* ctx, const vgpu_dmat* m, int32_t repr, uint32_t* host_row_major_out) {
     VG_TRY(vg_enter(ctx));
     VG_TRY(vg_dmat_materialize(ctx, m));
-    if (m->dist == VG_COLS) VG_FAIL(ctx, "dmat_download: column shares are internal to a commit");
     if (!m->bitrev_rows || m->gh < 2) return vg_download_rowmajor(ctx, m, repr, host_row_major_out + m->row0 * m->gw);
     std::vector<uint32_t> stored;
     try { stored.resize(m->h * m->w); } catch (const std::bad_alloc&) { VG_FAIL(ctx, "out of host memory"); }
@@ -296,20 +278,12 @@ static int32_t check_device_view(vgpu_ctx* ctx, const char* what, const uint32_t
     }
     return 0;
 }
-// The rows this rank holds of a matrix of logical height h: its run of a trace tall enough to be split (where vg_dmat_alloc_dist
-// puts a VG_ROWS shard, the rule of vgpu_dmat_upload_rows), otherwise all of them.  Returns whether the matrix is split.
-static bool local_rows_of(const vgpu_ctx* ctx, uint64_t h, uint64_t* row0, uint64_t* rows) {
-    const bool split = vg_split_rows(ctx, 2 * h);
-    *rows = split ? h / (uint64_t)ctx->comm_size : h;
-    *row0 = split ? *rows * (uint64_t)ctx->comm_rank : 0;
-    return split;
-}
+// The rows this rank holds of a trace of height h: vg_trace_run, the rule of vgpu_dmat_upload_rows.
 static int32_t check_local_height(vgpu_ctx* ctx, const char* what, uint64_t view_rows, uint64_t h) {
-    uint64_t row0, rows;
-    local_rows_of(ctx, h, &row0, &rows);
-    if (view_rows != rows)
+    const VgRun run = vg_trace_run(ctx, h);
+    if (view_rows != run.count)
         VG_FAIL(ctx, "%s: the view has %llu rows, but of a matrix of height %llu rank %d holds rows = %llu starting at row0 = %llu", what,
-                (unsigned long long)view_rows, (unsigned long long)h, ctx->comm_rank, (unsigned long long)rows, (unsigned long long)row0);
+                (unsigned long long)view_rows, (unsigned long long)h, ctx->comm_rank, (unsigned long long)run.count, (unsigned long long)run.begin);
     return 0;
 }
 // rows: keep this rank's run of a trace tall enough to be split.  local: `src` views those rows only (of a matrix of height h);
@@ -321,7 +295,7 @@ static int32_t import_view(vgpu_ctx* ctx, const char* what, const vgpu_dev_matri
     if (local) VG_TRY(check_local_height(ctx, what, src->height, h));
     if (src->height && w) VG_TRY(check_device_view(ctx, what, src->data, src->height, w, src->row_stride, src->col_stride));
     vgpu_dmat* m = nullptr;
-    VG_TRY(rows && vg_split_rows(ctx, 2 * h) ? vg_dmat_alloc_dist(ctx, VG_ROWS, h, w, false, &m) : vg_dmat_alloc(ctx, h, w, &m));
+    VG_TRY(vg_dmat_alloc_run(ctx, h, w, rows && vg_trace_run(ctx, h).split, false, &m));
     unsigned long long bad = ~0ull;
     const uint32_t* first = local ? src->data : src->data + m->row0 * src->row_stride;
     int32_t rc = vg_import_strided(ctx, first, m->h, m->w, src->row_stride, src->col_stride, repr, m, &bad);
@@ -345,8 +319,8 @@ int32_t vgpu_dmat_import_local(vgpu_ctx* ctx, const vgpu_dev_matrix* local, uint
 static int32_t borrow_view(vgpu_ctx* ctx, const char* what, uint32_t* data, uint64_t height, uint64_t width, uint64_t col_stride, bool local, vgpu_dmat** out) {
     if (!out) VG_FAIL(ctx, "%s: null argument", what);
     VG_TRY(vg_enter(ctx));
-    uint64_t row0 = 0, rows = height;
-    const bool split = local && local_rows_of(ctx, height, &row0, &rows);
+    const VgRun run = local ? vg_trace_run(ctx, height) : VgRun{0, height, false};
+    const uint64_t row0 = run.begin, rows = run.count;
     if (col_stride < rows) VG_FAIL(ctx, "%s: column stride %llu is below the height %llu", what, (unsigned long long)col_stride, (unsigned long long)rows);
     if (rows && width) {
         VG_TRY(check_device_view(ctx, what, data, rows, width, 1, col_stride));
@@ -359,7 +333,7 @@ static int32_t borrow_view(vgpu_ctx* ctx, const char* what, uint32_t* data, uint
     vgpu_dmat* m = new (std::nothrow) vgpu_dmat();
     if (!m) VG_FAIL(ctx, "out of host memory");
     m->ctx = ctx; m->d = data; m->h = rows; m->gh = height; m->w = m->gw = width; m->col_stride = col_stride;
-    m->row0 = row0; m->dist = split ? VG_ROWS : VG_FULL;
+    m->row0 = row0; m->dist = run.split ? VG_ROWS : VG_FULL;
     m->owns = false;
     *out = m;
     return 0;
@@ -374,7 +348,6 @@ int32_t vgpu_dmat_borrow_local(vgpu_ctx* ctx, uint32_t* data, uint64_t height, u
 static int32_t export_view(vgpu_ctx* ctx, const char* what, const vgpu_dmat* m, int32_t repr, const vgpu_dev_matrix* dst, bool local) {
     if (!m || !dst) VG_FAIL(ctx, "%s: null argument", what);
     VG_TRY(vg_enter(ctx));
-    if (m->dist == VG_COLS) VG_FAIL(ctx, "%s: column shares are internal to a commit", what);
     if (m->dist == VG_ROWS && m->bitrev_rows) VG_FAIL(ctx, "%s: a bit-reversed row shard has no contiguous natural-order image", what);
     if (local && (dst->height != m->h || dst->width != m->w))
         VG_FAIL(ctx, "%s: the view is %llu x %llu, but of the %llu x %llu matrix rank %d holds rows = %llu starting at row0 = %llu", what,
@@ -398,7 +371,8 @@ int32_t vgpu_dmat_export_local(vgpu_ctx* ctx, const vgpu_dmat* m, int32_t repr, 
 }
 int32_t vgpu_ctx_local_rows(const vgpu_ctx* ctx, uint64_t height, uint64_t* row0, uint64_t* rows) {
     if (!ctx || !row0 || !rows) return -1;
-    local_rows_of(ctx, height, row0, rows);
+    const VgRun run = vg_trace_run(ctx, height);
+    *row0 = run.begin; *rows = run.count;
     return 0;
 }
 int32_t vgpu_dmat_dims(const vgpu_dmat* m, uint64_t* height, uint64_t* width) { *height = m->gh; *width = m->gw; return 0; }
@@ -489,16 +463,22 @@ static std::vector<ColPlan> plan_columns(const int G, const std::vector<std::pai
     return plan;
 }
 
-// Symmetric-heap bytes one commit of matrices with these (height, width) puts there when they arrive as row shards (prover.cc sizes
-// the heap for a whole proof with it).
+// Symmetric-heap bytes of one split commit of the tall matrices dims[k] = (height, width), columns planned by `plan`: the row shard
+// of every LDE, and the column buffer of every matrix that arrives as row shards (as_rows[k]).
+static size_t commit_symm_bytes(int G, const std::vector<std::pair<uint64_t, uint64_t>>& dims, const std::vector<ColPlan>& plan, const std::vector<bool>& as_rows) {
+    size_t need = 0;
+    for (size_t k = 0; k < dims.size(); k++) {
+        need += vg_symm_round((2 * dims[k].first / (uint64_t)G) * dims[k].second * 4);
+        if (as_rows[k]) need += vg_symm_round(dims[k].first * plan[k].widest * 4);
+    }
+    return need;
+}
+// The same for matrices with these (height, width), all arriving as row shards when tall enough to be split (prover.cc sizes the
+// heap for a whole proof with it).
 extern "C++" size_t vg_commit_symm_need(const vgpu_ctx* ctx, const std::vector<std::pair<uint64_t, uint64_t>>& dims_all) {
     std::vector<std::pair<uint64_t, uint64_t>> dims;
-    for (auto& d : dims_all) if (vg_split_rows(ctx, 2 * d.first)) dims.push_back(d);
-    const std::vector<ColPlan> plan = plan_columns(ctx->comm_size, dims);
-    size_t need = 0;
-    for (size_t k = 0; k < dims.size(); k++)
-        need += vg_symm_round((2 * dims[k].first / (uint64_t)ctx->comm_size) * dims[k].second * 4) + vg_symm_round(dims[k].first * plan[k].widest * 4);
-    return need;
+    for (auto& d : dims_all) if (vg_trace_run(ctx, d.first).split) dims.push_back(d);
+    return commit_symm_bytes(ctx->comm_size, dims, plan_columns(ctx->comm_size, dims), std::vector<bool>(dims.size(), true));
 }
 
 // The column plan of a commit as data (tests; a host program that wants to know which rank extends what): matrices i = 0..n-1 of
@@ -514,25 +494,18 @@ void vgpu_split_column_plan(int32_t nranks, uint32_t n, const uint64_t* heights,
 // its columns; (2) every rank extends its column share and stores, through peer pointers, each rank's run of the committed
 // rows into that rank's shard.  After the closing barrier pd->ldes[i] holds rows [rank * H/G, (rank+1) * H/G) of all columns.
 static int32_t extend_split(vgpu_ctx* ctx, vgpu_prover_data* pd, const vgpu_dmat* const* mats, const std::vector<size_t>& tall, const uint32_t* coset_shifts_or_null) {
-    const uint64_t G = (uint64_t)ctx->comm_size;
     std::vector<std::pair<uint64_t, uint64_t>> dims;
-    for (size_t i : tall) dims.push_back({mats[i]->gh, mats[i]->gw});
+    std::vector<bool> as_rows;
+    for (size_t i : tall) { dims.push_back({mats[i]->gh, mats[i]->gw}); as_rows.push_back(mats[i]->dist == VG_ROWS); }
     const std::vector<ColPlan> plan = plan_columns(ctx->comm_size, dims);
-    size_t need = 0;
-    for (size_t k = 0; k < tall.size(); k++) {
-        const vgpu_dmat* m = mats[tall[k]];
-        need += vg_symm_round((2 * m->gh / G) * m->gw * 4);
-        if (m->dist == VG_ROWS) need += vg_symm_round(m->gh * plan[k].widest * 4);
-    }
-    VG_TRY(vg_symm_reserve(ctx, need));
+    VG_TRY(vg_symm_reserve(ctx, commit_symm_bytes(ctx->comm_size, dims, plan, as_rows)));
     std::vector<uint32_t*> cols(tall.size(), nullptr);      // column buffers of the matrices that arrive as row shards (symmetric heap)
     struct Guard { vgpu_ctx* c; std::vector<uint32_t*>& v; ~Guard() { for (auto* p : v) vg_symm_free(c, p); } } guard{ctx, cols};
     bool moved = false;
     for (size_t k = 0; k < tall.size(); k++) {
         const vgpu_dmat* m = mats[tall[k]];
         VG_TRY(vg_dmat_materialize(ctx, m));
-        if (m->dist == VG_COLS) VG_FAIL(ctx, "commit: column shares are internal to a commit");
-        if (m->dist != VG_ROWS) continue;
+        if (!as_rows[k]) continue;
         VG_TRY(vg_symm_alloc(ctx, (void**)&cols[k], m->gh * plan[k].widest * 4));
         VG_TRY(vg_exchange_rows_to_cols(ctx, m, cols[k], plan[k].begin));
         moved = true;
@@ -558,7 +531,7 @@ static int32_t extend_split(vgpu_ctx* ctx, vgpu_prover_data* pd, const vgpu_dmat
         const vgpu_dmat* m = mats[i];
         const uint64_t h = m->gh, H = 2 * h;
         const uint64_t c0 = plan[k].begin[ctx->comm_rank], c1 = plan[k].begin[ctx->comm_rank + 1];
-        VG_TRY(vg_dmat_alloc_dist(ctx, VG_ROWS, H, m->gw, true, &pd->ldes[i]));
+        VG_TRY(vg_dmat_alloc_run(ctx, H, m->gw, true, true, &pd->ldes[i]));
         pd->ldes[i]->bitrev_rows = false;        // committed order IS the stored order of an LDE (rows at reverse_bits)
         if (c1 <= c0) continue;
         const uint32_t* src; uint64_t scs;
@@ -594,7 +567,7 @@ int32_t vgpu_commit_batches(vgpu_ctx* ctx, const vgpu_dmat* const* mats, uint32_
     for (uint32_t i = 0; i < n; i++) {
         if (!mats[i]) { vgpu_prover_data_free(pd); VG_FAIL(ctx, "commit: matrix %u is null", i); }
         heights[i] = mats[i]->gh * 2;
-        if (vg_split_rows(ctx, heights[i])) tall.push_back(i);
+        if (vg_trace_run(ctx, mats[i]->gh).split) tall.push_back(i);
         else if (mats[i]->dist != VG_FULL) { vgpu_prover_data_free(pd); VG_FAIL(ctx, "commit: matrix %u is a shard but too short to be split", i); }
     }
     int32_t rc = tall.empty() ? 0 : extend_split(ctx, pd, mats, tall, coset_shifts_or_null);

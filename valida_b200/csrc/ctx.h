@@ -90,13 +90,13 @@ struct vgpu_ctx {
 
 // Distribution of a matrix over the ranks of a split proof.  FULL: every rank holds all of it (also the only kind on a lone
 // GPU).  ROWS: this rank holds the contiguous run [row0, row0 + h) of the STORED row order (natural rows for traces,
-// bit-reversed rows for committed LDEs / quotient chunks) of a gh x gw matrix.  COLS: columns [col0, col0 + w), all rows.
-enum VgDist { VG_FULL = 0, VG_ROWS = 1, VG_COLS = 2 };
+// bit-reversed rows for committed LDEs / quotient chunks) of a gh x gw matrix (vg_dmat_alloc_run).
+enum VgDist { VG_FULL = 0, VG_ROWS = 1 };
 struct vgpu_dmat {
     vgpu_ctx* ctx = nullptr;
     uint32_t* d = nullptr;       // column-major: LOCAL element (r, c) at d[c * col_stride + r], Montgomery form
     uint64_t h = 0, w = 0, col_stride = 0;     // local extent
-    uint64_t gh = 0, gw = 0, row0 = 0, col0 = 0;   // logical extent and the position of the local part in it
+    uint64_t gh = 0, gw = 0, row0 = 0;         // logical extent and the first local row in it
     int dist = VG_FULL;
     bool symm = false;           // d lives in the symmetric heap
     bool owns = true;
@@ -140,17 +140,34 @@ struct KScope {
 int32_t vg_enter(vgpu_ctx* ctx);                          // make ctx->device current on the calling thread
 int32_t vg_alloc(vgpu_ctx* ctx, void** p, size_t bytes);
 void vg_free(vgpu_ctx* ctx, void* p);
-int32_t vg_dmat_alloc(vgpu_ctx* ctx, uint64_t h, uint64_t w, vgpu_dmat** out);
 // pow.cu: the context's Poseidon-16 constants on the device (poseidon.cuh layout), uploaded on first use; an error before vgpu_set_challenger
 int32_t vg_poseidon_consts(vgpu_ctx* ctx, uint32_t** out);
 int32_t vg_get_shift_table(vgpu_ctx* ctx, uint32_t shift_canonical, uint32_t scale_canonical, uint64_t max_exp, const PowTable** out);
 
-// host/comm.cc — every rank calls these in the same order with the same sizes
 inline bool vg_sharded(const vgpu_ctx* ctx) { return ctx->sharding && ctx->comm_size > 1; }
+// Which rows each rank of a split proof holds.  Every rank must reach the same answer at every allocation, upload, sweep and query
+// answer (or the proof hangs at a barrier or comes out wrong), so this is the one place that decides it.
+// A run of stored rows: this rank holds [begin, begin + count) of them; split = they are cut into one equal run per rank.
+struct VgRun { uint64_t begin, count; bool split; };
+inline VgRun vg_run(uint64_t n, uint64_t nranks, uint64_t rank, bool split) {
+    return split ? VgRun{rank * (n / nranks), n / nranks, true} : VgRun{0, n, false};
+}
 // A matrix / vector of `n` stored rows is cut into comm_size contiguous row shards when every shard keeps >= 4096 rows;
 // shorter ones are replicated (every rank computes and holds all of them).
 inline bool vg_split_rows(const vgpu_ctx* ctx, uint64_t n) { return vg_sharded(ctx) && n >= (uint64_t)ctx->comm_size * 4096; }
-void vg_shard_range(uint64_t total, int nranks, int rank, uint64_t* begin, uint64_t* end);   // contiguous, balanced
+inline VgRun vg_row_run(const vgpu_ctx* ctx, uint64_t n) { return vg_run(n, ctx->comm_size, ctx->comm_rank, vg_split_rows(ctx, n)); }
+// A trace of h rows is split when its LDE of 2h rows is: its rank r holds natural rows [r h / comm_size, (r + 1) h / comm_size).
+inline VgRun vg_trace_run(const vgpu_ctx* ctx, uint64_t h) { return vg_run(h, ctx->comm_size, ctx->comm_rank, vg_split_rows(ctx, 2 * h)); }
+// A Merkle tree layer of `len` nodes is cut into runs when every one of the nranks > 1 ranks gets a node (merkle.h).
+inline VgRun vg_layer_run(uint64_t len, int nranks, int rank) { return vg_run(len, nranks, rank, nranks > 1 && len >= (uint64_t)nranks); }
+// A query answer is summed over the ranks, so of data every rank holds only rank 0 reports its words.
+inline bool vg_reports_replicated(const vgpu_ctx* ctx) { return ctx->comm_rank == 0 || !vg_sharded(ctx); }
+// The part of a gh x gw matrix this rank holds: its run of gh / comm_size stored rows when `split` (VG_ROWS), else all of it
+// (VG_FULL).  symm: taken from the symmetric heap (peers store into it).
+int32_t vg_dmat_alloc_run(vgpu_ctx* ctx, uint64_t gh, uint64_t gw, bool split, bool symm, vgpu_dmat** out);
+inline int32_t vg_dmat_alloc(vgpu_ctx* ctx, uint64_t h, uint64_t w, vgpu_dmat** out) { return vg_dmat_alloc_run(ctx, h, w, false, false, out); }
+
+// host/comm.cc — every rank calls these in the same order with the same sizes
 // buf holds comm_size consecutive blocks of `words_per_rank` u32; this rank's block is already filled
 int32_t vg_comm_allgather_inplace(vgpu_ctx* ctx, uint32_t* buf, uint64_t words_per_rank);
 // stream-ordered barrier: everything enqueued before it on ANY rank's stream completes before anything enqueued after it
@@ -171,7 +188,6 @@ template <class T> inline T* vg_peer_ptr(const vgpu_ctx* ctx, T* mine, int peer)
 int32_t vg_exchange_rows_to_cols(vgpu_ctx* ctx, const vgpu_dmat* rows, uint32_t* cols_symm, const uint32_t* col_begin);
 int32_t vg_exchange_cols_to_rows(vgpu_ctx* ctx, const uint32_t* lde_cols, uint64_t H, uint64_t c0, uint64_t c1, vgpu_dmat* shard, cudaStream_t on = nullptr);
 size_t vg_commit_symm_need(const vgpu_ctx* ctx, const std::vector<std::pair<uint64_t, uint64_t>>& dims_all);
-int32_t vg_dmat_alloc_dist(vgpu_ctx* ctx, int dist, uint64_t gh, uint64_t gw, bool symm, vgpu_dmat** out);
 
 // ntt.cu
 int32_t vg_ntt_nat2nat(vgpu_ctx* ctx, const uint32_t* src, uint64_t src_cs, uint32_t* dst, uint64_t dst_cs, int log_n, uint64_t w,

@@ -110,13 +110,6 @@ int32_t local_barrier(vgpu_ctx* ctx) {
 
 }  // namespace
 
-void vg_shard_range(uint64_t total, int nranks, int rank, uint64_t* begin, uint64_t* end) {
-    // the first (total % nranks) ranks take one extra unit
-    const uint64_t q = total / (uint64_t)nranks, r = total % (uint64_t)nranks, k = (uint64_t)rank;
-    *begin = k * q + (k < r ? k : r);
-    *end = *begin + q + (k < r ? 1 : 0);
-}
-
 int32_t vg_comm_group_begin(vgpu_ctx* ctx) { if (ctx->nccl) VG_NCCL(ctx, nccl().GroupStart()); return 0; }
 int32_t vg_comm_group_end(vgpu_ctx* ctx) { if (ctx->nccl) VG_NCCL(ctx, nccl().GroupEnd()); return 0; }
 
@@ -350,10 +343,15 @@ void vgpu_comm_stats(vgpu_ctx* ctx, uint32_t calls[3], double bytes[3], int32_t 
 // the share of a tree layer of `len` nodes that rank `rank` derives itself (merkle.cu); *split = 0 when the
 // layer is shorter than the communicator and every rank computes all of it
 void vgpu_tree_share(uint64_t len, int32_t nranks, int32_t rank, uint64_t* begin, uint64_t* count, int32_t* split) {
-    if (nranks > 1 && len >= (uint64_t)nranks) { *count = len / (uint64_t)nranks; *begin = *count * (uint64_t)rank; *split = 1; }
-    else { *begin = 0; *count = len; *split = 0; }
+    const VgRun run = vg_layer_run(len, nranks, rank);
+    *begin = run.begin; *count = run.count; *split = run.split;
 }
 
-void vgpu_shard_range(uint64_t total, int32_t nranks, int32_t rank, uint64_t* begin, uint64_t* end) { vg_shard_range(total, nranks, rank, begin, end); }
+void vgpu_shard_range(uint64_t total, int32_t nranks, int32_t rank, uint64_t* begin, uint64_t* end) {
+    // the first (total % nranks) ranks take one extra unit
+    const uint64_t q = total / (uint64_t)nranks, r = total % (uint64_t)nranks, k = (uint64_t)rank;
+    *begin = k * q + (k < r ? k : r);
+    *end = *begin + q + (k < r ? 1 : 0);
+}
 
 }  // extern "C"

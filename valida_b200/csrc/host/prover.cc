@@ -58,13 +58,13 @@ struct RowVec {
     uint64_t n = 0, begin = 0, count = 0;      // whole length; stored run (limb stride = count)
     bool shard() const { return count != n; }
     const uint32_t* at(const vgpu_ctx* ctx, int limb, uint64_t i) const {   // null: another rank reports this element (see VgTree::node)
-        if (!shard()) return ctx->comm_rank == 0 || !vg_sharded(ctx) ? d + (uint64_t)limb * count + i : nullptr;
+        if (!shard()) return vg_reports_replicated(ctx) ? d + (uint64_t)limb * count + i : nullptr;
         return i >= begin && i < begin + count ? d + (uint64_t)limb * count + (i - begin) : nullptr;
     }
 };
 int32_t rowvec_alloc(vgpu_ctx* ctx, uint64_t n, RowVec* v) {
-    v->n = n;
-    if (vg_split_rows(ctx, n)) { v->count = n / ctx->comm_size; v->begin = v->count * ctx->comm_rank; } else { v->count = n; v->begin = 0; }
+    const VgRun run = vg_row_run(ctx, n);
+    v->n = n; v->begin = run.begin; v->count = run.count;
     return vg_alloc(ctx, (void**)&v->d, 5 * v->count * 4);
 }
 
@@ -117,7 +117,7 @@ int32_t open_multi_batches(vgpu_ctx* ctx, const std::vector<OpenRound>& rounds, 
             Job j{};
             j.lde = rd.pd->ldes[mi]; j.log_H = (uint32_t)log2u(j.lde->gh); j.w = (uint32_t)j.lde->gw; j.pts = &rd.points[mi];
             if (j.pts->empty() || j.pts->size() > 2) VG_FAIL(ctx, "open: 1 or 2 points per matrix are supported");
-            if ((j.lde->dist == VG_ROWS) != vg_split_rows(ctx, j.lde->gh)) VG_FAIL(ctx, "open: a committed matrix is not distributed as its height demands");
+            if ((j.lde->dist == VG_ROWS) != vg_row_run(ctx, j.lde->gh).split) VG_FAIL(ctx, "open: a committed matrix is not distributed as its height demands");
             j.sums_at = sums_words; sums_words += vg_eval_columns_words(j.w);
             jobs.push_back(j);
         }
@@ -278,7 +278,7 @@ int32_t open_multi_batches(vgpu_ctx* ctx, const std::vector<OpenRound>& rounds, 
             uint64_t bidx = index >> (log_max - lg);
             for (auto* m : rd.pd->ldes) {
                 const uint64_t row = bidx >> (lg - log2u(m->gh));
-                const bool mine = m->dist == VG_ROWS ? (row >= m->row0 && row < m->row0 + m->h) : (ctx->comm_rank == 0 || !vg_sharded(ctx));
+                const bool mine = m->dist == VG_ROWS ? (row >= m->row0 && row < m->row0 + m->h) : vg_reports_replicated(ctx);
                 for (uint64_t c = 0; c < m->w; c++) *o++ = mine ? m->d + c * m->col_stride + (row - m->row0) : nullptr;
             }
             push_path(S.layers.size() + r);
@@ -593,7 +593,7 @@ int32_t vgpu_prove(vgpu_ctx* ctx, const vgpu_matrix main[VGPU_NUM_CHIPS], const 
     auto t0 = std::chrono::steady_clock::now();
     dm.v.assign(VGPU_NUM_CHIPS, nullptr); dp.v.assign(2, nullptr);
     auto alloc_for = [&](const vgpu_matrix& hm, vgpu_dmat** out) {
-        return vg_split_rows(ctx, 2 * hm.height) ? vg_dmat_alloc_dist(ctx, VG_ROWS, hm.height, hm.width, false, out) : vg_dmat_alloc(ctx, hm.height, hm.width, out);
+        return vg_dmat_alloc_run(ctx, hm.height, hm.width, vg_trace_run(ctx, hm.height).split, false, out);
     };
     auto begin_upload = [&](const vgpu_matrix& hm, vgpu_dmat* m) { return vg_upload_begin(ctx, hm.data + m->row0 * hm.width, m->h, m->w, repr, m); };
     for (int i = 0; i < 2; i++) VG_TRY(alloc_for(prep[i], &dp.v[i]));

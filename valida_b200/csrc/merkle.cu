@@ -559,14 +559,14 @@ __global__ void __launch_bounds__(PATH_THREADS) p16_path_kernel(const PathTree* 
 // Layer plan of a tree over `leaves` leaves (merkle.h): which run of every layer this rank computes and which it keeps.
 struct LayerPlan { uint64_t len, cbegin, ccount, sbegin, scount; bool gather; };
 static std::vector<LayerPlan> plan_tree(const vgpu_ctx* ctx, uint64_t leaves, bool split) {
-    const uint64_t G = split ? (uint64_t)ctx->comm_size : 1, r = split ? (uint64_t)ctx->comm_rank : 0;
+    const int G = split ? ctx->comm_size : 1, r = split ? ctx->comm_rank : 0;
     std::vector<LayerPlan> plan;
     for (uint64_t len = leaves; len >= 1; len >>= 1) {
+        const VgRun run = vg_layer_run(len, G, r);
         LayerPlan p{};
-        p.len = len;
-        if (G > 1 && len >= G) { p.ccount = len / G; p.cbegin = r * p.ccount; } else { p.cbegin = 0; p.ccount = len; }
-        if (G > 1 && len > G) { p.sbegin = p.cbegin; p.scount = p.ccount; } else { p.sbegin = 0; p.scount = len; }
-        p.gather = G > 1 && len == G;          // the sub-roots: one node per rank, completed by the all-gather
+        p.len = len; p.cbegin = run.begin; p.ccount = run.count;
+        p.gather = run.split && len == (uint64_t)G;     // the sub-roots: one node per rank, completed by the all-gather
+        if (run.split && !p.gather) { p.sbegin = p.cbegin; p.scount = p.ccount; } else { p.sbegin = 0; p.scount = len; }
         plan.push_back(p);
         if (len == 1) break;
     }
@@ -740,7 +740,7 @@ int32_t vg_merkle_build(vgpu_ctx* ctx, vgpu_prover_data* pd, const std::vector<u
     uint64_t max_h = heights[order[0]];
     if (max_h & (max_h - 1)) VG_FAIL(ctx, "commit: heights must be powers of two");
     pd->max_height = max_h;
-    const std::vector<LayerPlan> plan = plan_tree(ctx, max_h, vg_split_rows(ctx, max_h));
+    const std::vector<LayerPlan> plan = plan_tree(ctx, max_h, vg_row_run(ctx, max_h).split);
     LowerLayers low{ctx, &pd->tree};
     VG_TRY(alloc_tree(ctx, plan, &pd->tree, &low));
     pd->tree.hash = ctx->merkle_hash;

@@ -26,9 +26,9 @@ struct VgTree {
     // the levels of an authentication path that are not stored: vg_tree_paths rebuilds them
     size_t rebuilt() const { return std::min(depth(), VG_TREE_DROP); }
     // whether THIS rank is the one that reports node `j` of layer `lvl` in a query answer (the owner of a split layer's run;
-    // rank 0 for the layers every rank holds)
+    // vg_reports_replicated for the layers every rank holds)
     bool reports(const vgpu_ctx* ctx, size_t lvl, uint64_t j) const {
-        if (layer_count[lvl] == layer_len[lvl]) return ctx->comm_rank == 0 || !vg_sharded(ctx);
+        if (layer_count[lvl] == layer_len[lvl]) return vg_reports_replicated(ctx);
         return j >= layer_begin[lvl] && j < layer_begin[lvl] + layer_count[lvl];
     }
     // address of node `j` of a kept layer `lvl` if this rank reports it, else null

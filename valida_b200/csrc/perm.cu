@@ -229,7 +229,6 @@ int32_t vg_perm_trace_enqueue(vgpu_ctx* ctx, const vgpu_chip_desc* chip, const v
     if (!chip || !main || !out_perm) VG_FAIL(ctx, "perm_trace: null argument");
     if (main->bitrev_rows) VG_FAIL(ctx, "perm_trace: main trace rows are stored bit-reversed");
     if (main->gw != chip->width) VG_FAIL(ctx, "perm_trace: main width %llu != chip width %u", (unsigned long long)main->gw, chip->width);
-    if (main->dist == VG_COLS || (prep_or_null && prep_or_null->dist == VG_COLS)) VG_FAIL(ctx, "perm_trace: column shares are internal to a commit");
     if (chip->preprocessed_width && (!prep_or_null || prep_or_null->gw != chip->preprocessed_width || prep_or_null->gh != main->gh)) {
         // interactions of BasicMachine never read preprocessed columns, but the shape must still be coherent when given
         if (prep_or_null) VG_FAIL(ctx, "perm_trace: preprocessed trace shape mismatch");
@@ -239,13 +238,13 @@ int32_t vg_perm_trace_enqueue(vgpu_ctx* ctx, const vgpu_chip_desc* chip, const v
     auto dchip_h = std::make_unique<DevChip>();
     VG_TRY(vg_build_devchip(ctx, chip, challenges, dchip_h.get()));
     const DevChip& dchip = *dchip_h;
-    const bool split = vg_split_rows(ctx, 2 * main->gh);
+    const VgRun run = vg_trace_run(ctx, main->gh);
+    const bool split = run.split;
     if (!split && main->dist != VG_FULL) VG_FAIL(ctx, "perm_trace: the trace is a shard but too short to be split");
-    const uint64_t h = split ? main->gh / ctx->comm_size : main->gh;          // rows swept here
-    const uint64_t row0 = split ? h * ctx->comm_rank : 0;
+    const uint64_t h = run.count, row0 = run.begin;          // rows swept here
     uint32_t k = chip->n_interactions;
     vgpu_dmat* perm = nullptr;
-    VG_TRY(split ? vg_dmat_alloc_dist(ctx, VG_ROWS, main->gh, 5 * (k + 1), false, &perm) : vg_dmat_alloc(ctx, h, 5 * (k + 1), &perm));
+    VG_TRY(vg_dmat_alloc_run(ctx, main->gh, 5 * (k + 1), split, false, &perm));
     struct Undo { vgpu_dmat* m; ~Undo() { vgpu_dmat_free(m); } } undo{perm};       // released on every failing exit below
     // first swept row of a matrix: a shard starts there, a whole trace is entered at row0
     auto rows_of = [&](const vgpu_dmat* m) { return m->d + (m->dist == VG_ROWS ? 0 : row0); };

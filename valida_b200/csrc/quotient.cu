@@ -195,7 +195,6 @@ extern "C" int32_t vgpu_quotient(vgpu_ctx* ctx, const vgpu_chip_desc* chip, uint
     // split proof: the committed LDEs of a tall chip are row shards (all three the same run of rows), of a short chip whole
     const bool split = main_lde->dist == VG_ROWS;
     if ((perm_lde->dist == VG_ROWS) != split || (prep_lde && (prep_lde->dist == VG_ROWS) != split)) VG_FAIL(ctx, "quotient: the LDEs are not distributed alike");
-    if (main_lde->dist == VG_COLS) VG_FAIL(ctx, "quotient: column shares are internal to a commit");
     // alpha powers for N = base + k + 3 constraints
     const uint32_t N = vg_chip_base_constraints(chip->chip_id) + chip->n_interactions + 3;
     if (N > Q_MAX_CONSTRAINTS) { VG_FAIL(ctx, "quotient: %u constraints exceed the parameter table (%u)", N, Q_MAX_CONSTRAINTS); }
@@ -222,7 +221,7 @@ extern "C" int32_t vgpu_quotient(vgpu_ctx* ctx, const vgpu_chip_desc* chip, uint
         return vg_peer_ptr(ctx, m->d, next_rank) - (uint64_t)next_rank * m->h;
     };
     vgpu_dmat* out = nullptr;
-    VG_TRY(split ? vg_dmat_alloc_dist(ctx, VG_ROWS, h, 10, false, &out) : vg_dmat_alloc(ctx, h, 10, &out));
+    VG_TRY(vg_dmat_alloc_run(ctx, h, 10, split, false, &out));
     out->bitrev_rows = true;
     p.main = base_of(main_lde); p.main_n = next_of(main_lde); p.mcs = main_lde->col_stride;
     p.prep = prep_lde ? base_of(prep_lde) : nullptr; p.prep_n = prep_lde ? next_of(prep_lde) : nullptr; p.pcs = prep_lde ? prep_lde->col_stride : 0;

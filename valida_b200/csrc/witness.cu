@@ -340,7 +340,7 @@ int32_t vgpu_witness_device(vgpu_ctx* ctx, const vgpu_vmlog* log, vgpu_dmat* mai
     if (!L.n_cpu) VG_FAIL(ctx, "witness: the run has no cycles");
     // a tall chip's trace: whole, or this rank's run of rows (split proof)
     auto alloc_rows = [&](uint64_t h, uint64_t w, vgpu_dmat** out, RowRange* rr) -> int32_t {
-        if (vg_split_rows(ctx, 2 * h)) VG_TRY(vg_dmat_alloc_dist(ctx, VG_ROWS, h, w, false, out)); else VG_TRY(vg_dmat_alloc(ctx, h, w, out));
+        VG_TRY(vg_dmat_alloc_run(ctx, h, w, vg_trace_run(ctx, h).split, false, out));
         rr->row0 = (*out)->row0; rr->rows = (*out)->h; rr->out = (*out)->d; rr->cs = (*out)->col_stride;
         return 0;
     };
