@@ -261,7 +261,7 @@ void build_cpu(const Vm& vm, Traces& t) {
         const CpuRec& r = vm.cpu[i];
         uint32_t* row = &v[(size_t)i * W];
         const int32_t* w = vm.prog + 6 * (size_t)r.instr;
-        row[0] = (uint32_t)i; row[1] = r.pc; row[2] = r.fp;
+        row[0] = (uint32_t)i; row[1] = r.pc; row[2] = r.fp % P;      // from_canonical_u32 (cpu/src/lib.rs:171-172) reduces mod p
         row[3] = (uint32_t)w[0];
         for (int k = 0; k < 5; k++) row[4 + k] = from_i32(w[1 + k]);
         bool left_imm = false;
@@ -295,7 +295,7 @@ void build_cpu(const Vm& vm, Traces& t) {
             if (m.is_write) ch = 43;
             else if (first_read && !left_imm) { ch = 29; first_read = false; }
             else ch = 36;
-            row[ch] = 1; row[ch + 2] = m.addr; word_be(m.value, &row[ch + 3]);
+            row[ch] = 1; row[ch + 2] = m.addr % P; word_be(m.value, &row[ch + 3]);     // cpu/src/lib.rs:263-276
         }
         uint64_t dsum = 0;
         for (int k = 0; k < 4; k++) { int64_t dd = (int64_t)row[32 + k] - (int64_t)row[39 + k]; dsum += (uint64_t)(dd * dd); }
@@ -320,7 +320,7 @@ void build_cpu(const Vm& vm, Traces& t) {
     // pad_to_power_of_two (cpu/src/lib.rs:318-353)
     if (n) {
         const uint32_t* last = &v[(n - 1) * W];
-        uint32_t pc = last[1], fp = last[2], clk = last[0];
+        uint32_t pc = last[1], fp = last[2], clk = last[0];        // fp already reduced
 #pragma omp parallel for schedule(static)
         for (long i = (long)n; i < (long)h; i++) {
             uint32_t* row = &v[(size_t)i * W];
@@ -386,7 +386,7 @@ void build_mem(const Vm& vm, Traces& t) {
     for (size_t i = 0; i < n0; i++) {
         uint32_t* row = &v[i * W];
         std::memset(row, 0, W * sizeof(uint32_t));
-        row[0] = vm.static_cells[i].first; word_be(vm.static_cells[i].second, &row[1]);
+        row[0] = vm.static_cells[i].first % P; word_be(vm.static_cells[i].second, &row[1]);     // memory/src/lib.rs:276
         row[6] = 1; row[8] = 1; row[12] = (uint32_t)i;
     }
     // every word of the n operation rows is written here and the padding rows are cleared below: no zero fill of the
@@ -394,7 +394,7 @@ void build_mem(const Vm& vm, Traces& t) {
 #pragma omp parallel for schedule(static)
     for (long i = 0; i < (long)n; i++) {
         uint32_t* row = &v[(n0 + (size_t)i) * W];
-        row[0] = ops[i].addr; word_be(ops[i].value, &row[1]);
+        row[0] = ops[i].addr % P; word_be(ops[i].value, &row[1]);      // sorted by the u32 address, stored reduced (memory/src/lib.rs:247-262)
         row[5] = ops[i].clk; row[6] = 0;
         row[7] = ops[i].is_write ? 0 : 1; row[8] = ops[i].is_write ? 1 : 0;
         row[9] = 0; row[10] = 0; row[11] = 0;
@@ -529,7 +529,8 @@ static vgpu_traces* build_traces_host(Vm& vm) {
         for (size_t i = 0; i < h; i++) {
             uint32_t* row = &t.store[14][i * 7];
             row[0] = (uint32_t)i;
-            if (i < n_instr) { row[1] = (uint32_t)program_words[6 * i]; for (int k = 0; k < 5; k++) row[2 + k] = from_i32(program_words[6 * i + 1 + k]); }
+            // every row of the program, executed or not: InstructionWord::flatten takes the opcode from_canonical_u32 (machine/src/program.rs:44)
+            if (i < n_instr) { row[1] = (uint32_t)program_words[6 * i] % P; for (int k = 0; k < 5; k++) row[2 + k] = from_i32(program_words[6 * i + 1 + k]); }
         }
         t.prep[0] = {t.store[14].data(), h, 7};
     }
@@ -557,7 +558,7 @@ static vgpu_traces* build_traces_host(Vm& vm) {
         t.store[13].zeros(h * 6);
         for (size_t i = 0; i < n0; i++) {
             uint32_t* row = &t.store[13][i * 6];
-            row[0] = vm.static_cells[i].first; word_be(vm.static_cells[i].second, &row[1]); row[5] = 1;
+            row[0] = vm.static_cells[i].first % P; word_be(vm.static_cells[i].second, &row[1]); row[5] = 1;    // static_data/src/lib.rs:67
         }
         t.main[13] = {t.store[13].data(), h, 6};
     }
