@@ -42,7 +42,7 @@ void vg_free(vgpu_ctx* ctx, void* p) {
     ctx->cached_bytes += bytes;
 }
 
-int32_t vg_dmat_alloc_run(vgpu_ctx* ctx, uint64_t gh, uint64_t gw, bool split, bool symm, vgpu_dmat** out) {
+int32_t vg_dmat_alloc_run(vgpu_ctx* ctx, uint64_t gh, uint64_t gw, bool split, bool symm, VgMat* out) {
     vgpu_dmat* m = new (std::nothrow) vgpu_dmat();
     if (!m) VG_FAIL(ctx, "out of host memory");
     const VgRun run = vg_run(gh, ctx->comm_size, ctx->comm_rank, split);
@@ -51,7 +51,7 @@ int32_t vg_dmat_alloc_run(vgpu_ctx* ctx, uint64_t gh, uint64_t gw, bool split, b
     const size_t bytes = m->h * m->w * 4;
     int32_t rc = symm ? vg_symm_alloc(ctx, (void**)&m->d, bytes) : vg_alloc(ctx, (void**)&m->d, bytes);
     if (rc) { delete m; return rc; }
-    *out = m;
+    out->reset(m);
     return 0;
 }
 
@@ -63,11 +63,12 @@ static int32_t build_pow_table(vgpu_ctx* ctx, uint32_t base_monty, uint32_t scal
     uint32_t step = a;  // base^4096
     a = scale_monty;
     for (uint64_t j = 0; j < hi_len; j++) { hi[j] = a; a = bb::mul(a, step); }
-    VG_TRY(vg_alloc(ctx, (void**)&t->lo, lo.size() * 4));
-    VG_TRY(vg_alloc(ctx, (void**)&t->hi, hi.size() * 4));
-    VG_CUDA(ctx, cudaMemcpyAsync(t->lo, lo.data(), lo.size() * 4, cudaMemcpyHostToDevice, ctx->stream));
-    VG_CUDA(ctx, cudaMemcpyAsync(t->hi, hi.data(), hi.size() * 4, cudaMemcpyHostToDevice, ctx->stream));
+    VgBuf dlo(ctx), dhi(ctx);
+    VG_TRY(dlo.upload(lo.data(), lo.size()));
+    VG_TRY(dhi.upload(hi.data(), hi.size()));
     VG_CUDA(ctx, cudaStreamSynchronize(ctx->stream));   // host vectors go out of scope
+    t->lo = (uint32_t*)dlo.release();                    // the caller's table owns them from here on
+    t->hi = (uint32_t*)dhi.release();
     t->hi_len = (uint32_t)hi_len;
     t->base = base_monty;
     return 0;
@@ -225,11 +226,10 @@ int32_t vgpu_host_unregister(vgpu_ctx* ctx, const void* p) {
 int32_t vgpu_dmat_upload(vgpu_ctx* ctx, const vgpu_matrix* host, int32_t repr, vgpu_dmat** out) {
     if (!host || !out) VG_FAIL(ctx, "dmat_upload: null argument");
     VG_TRY(vg_enter(ctx));
-    vgpu_dmat* m = nullptr;
+    VgMat m;
     VG_TRY(vg_dmat_alloc(ctx, host->height, host->width, &m));
-    int32_t rc = vg_upload_rowmajor(ctx, host->data, host->height, host->width, repr, m);
-    if (rc) { vgpu_dmat_free(m); return rc; }
-    *out = m;
+    VG_TRY(vg_upload_rowmajor(ctx, host->data, host->height, host->width, repr, m.get()));
+    *out = m.release();
     return 0;
 }
 // Split proof: a rank keeps only ITS run of rows of a trace tall enough to be split (every rank passes the same host
@@ -238,11 +238,10 @@ int32_t vgpu_dmat_upload_rows(vgpu_ctx* ctx, const vgpu_matrix* host, int32_t re
     if (!host || !out) VG_FAIL(ctx, "dmat_upload_rows: null argument");
     if (!vg_trace_run(ctx, host->height).split) return vgpu_dmat_upload(ctx, host, repr, out);
     VG_TRY(vg_enter(ctx));
-    vgpu_dmat* m = nullptr;
+    VgMat m;
     VG_TRY(vg_dmat_alloc_run(ctx, host->height, host->width, true, false, &m));
-    int32_t rc = vg_upload_rowmajor(ctx, host->data + m->row0 * host->width, m->h, m->w, repr, m);
-    if (rc) { vgpu_dmat_free(m); return rc; }
-    *out = m;
+    VG_TRY(vg_upload_rowmajor(ctx, host->data + m->row0 * host->width, m->h, m->w, repr, m.get()));
+    *out = m.release();
     return 0;
 }
 // Writes the rows this rank holds (all of them unless the matrix is a row shard) at their place in the caller's
@@ -294,17 +293,16 @@ static int32_t import_view(vgpu_ctx* ctx, const char* what, const vgpu_dev_matri
     const uint64_t w = src->width;
     if (local) VG_TRY(check_local_height(ctx, what, src->height, h));
     if (src->height && w) VG_TRY(check_device_view(ctx, what, src->data, src->height, w, src->row_stride, src->col_stride));
-    vgpu_dmat* m = nullptr;
+    VgMat m;
     VG_TRY(vg_dmat_alloc_run(ctx, h, w, rows && vg_trace_run(ctx, h).split, false, &m));
     unsigned long long bad = ~0ull;
     const uint32_t* first = local ? src->data : src->data + m->row0 * src->row_stride;
-    int32_t rc = vg_import_strided(ctx, first, m->h, m->w, src->row_stride, src->col_stride, repr, m, &bad);
-    const uint64_t row0 = m->row0;
-    if (rc == 0 && bad == ~0ull) { *out = m; return 0; }
-    vgpu_dmat_free(m);
-    if (rc) return rc;
-    VG_FAIL(ctx, "%s: the word at row %llu, column %llu is not below p = %u (neither a canonical nor a Montgomery BabyBear word)", what,
-            (unsigned long long)(row0 + bad / w), (unsigned long long)(bad % w), bb::P);
+    VG_TRY(vg_import_strided(ctx, first, m->h, m->w, src->row_stride, src->col_stride, repr, m.get(), &bad));
+    if (bad != ~0ull)
+        VG_FAIL(ctx, "%s: the word at row %llu, column %llu is not below p = %u (neither a canonical nor a Montgomery BabyBear word)", what,
+                (unsigned long long)(m->row0 + bad / w), (unsigned long long)(bad % w), bb::P);
+    *out = m.release();
+    return 0;
 }
 int32_t vgpu_dmat_import(vgpu_ctx* ctx, const vgpu_dev_matrix* src, int32_t repr, vgpu_dmat** out) {
     return import_view(ctx, "dmat_import", src, src ? src->height : 0, repr, false, false, out);
@@ -401,11 +399,9 @@ int32_t vgpu_ntt_batch(vgpu_ctx* ctx, vgpu_dmat* m, int32_t inverse) {
     if (log_n > VG_LOG_NMAX) VG_FAIL(ctx, "ntt_batch: height exceeds two-adicity");
     if (m->bitrev_rows) VG_FAIL(ctx, "ntt_batch: matrix rows are stored bit-reversed");
     VG_TRY(vg_dmat_materialize(ctx, m));
-    uint32_t* tmp = nullptr;
-    VG_TRY(vg_alloc(ctx, (void**)&tmp, m->h * m->w * 4));
-    int32_t rc = vg_ntt_nat2nat(ctx, m->d, m->col_stride, m->d, m->col_stride, log_n, m->w, inverse != 0, nullptr, tmp, m->h);
-    vg_free(ctx, tmp);
-    return rc;
+    VgBuf tmp(ctx);
+    VG_TRY(tmp.alloc(m->h * m->w * 4));
+    return vg_ntt_nat2nat(ctx, m->d, m->col_stride, m->d, m->col_stride, log_n, m->w, inverse != 0, nullptr, tmp.as<uint32_t>(), m->h);
 }
 
 int32_t vgpu_coset_lde_batch(vgpu_ctx* ctx, const vgpu_dmat* in, uint32_t log_blowup, uint32_t shift_canonical, int32_t bit_reversed, vgpu_dmat** out) {
@@ -413,22 +409,20 @@ int32_t vgpu_coset_lde_batch(vgpu_ctx* ctx, const vgpu_dmat* in, uint32_t log_bl
     VG_TRY(vg_enter(ctx));
     if (in->dist != VG_FULL) VG_FAIL(ctx, "coset_lde: the matrix is a shard of a split proof");
     VG_TRY(vg_dmat_materialize(ctx, in));
-    vgpu_dmat* o = nullptr;
+    VgMat o;
     VG_TRY(vg_dmat_alloc(ctx, in->h << log_blowup, in->w, &o));
-    int32_t rc = vg_coset_lde(ctx, in->d, in->col_stride, in->h, in->w, shift_canonical, o->d, o->col_stride, bit_reversed != 0, in->bitrev_rows, log_blowup);
-    if (rc) { vgpu_dmat_free(o); return rc; }
-    *out = o;
+    VG_TRY(vg_coset_lde(ctx, in->d, in->col_stride, in->h, in->w, shift_canonical, o->d, o->col_stride, bit_reversed != 0, in->bitrev_rows, log_blowup));
+    *out = o.release();
     return 0;
 }
 
 int32_t vgpu_ntt_batch_host(vgpu_ctx* ctx, uint32_t* row_major, uint64_t height, uint64_t width, int32_t repr, int32_t inverse) {
     vgpu_matrix hm{row_major, height, width};
-    vgpu_dmat* m = nullptr;
-    VG_TRY(vgpu_dmat_upload(ctx, &hm, repr, &m));
-    int32_t rc = vgpu_ntt_batch(ctx, m, inverse);
-    if (rc == 0) rc = vgpu_dmat_download(ctx, m, repr, row_major);
-    vgpu_dmat_free(m);
-    return rc;
+    vgpu_dmat* raw = nullptr;
+    VG_TRY(vgpu_dmat_upload(ctx, &hm, repr, &raw));
+    VgMat m(raw);
+    VG_TRY(vgpu_ntt_batch(ctx, m.get(), inverse));
+    return vgpu_dmat_download(ctx, m.get(), repr, row_major);
 }
 
 // ---- commit ------------------------------------------------------------------------------------------
@@ -522,32 +516,33 @@ static int32_t extend_split(vgpu_ctx* ctx, vgpu_prover_data* pd, const vgpu_dmat
     size_t ext_words = 0;
     for (size_t k = 0; k < tall.size(); k++)
         ext_words = std::max<size_t>(ext_words, 2 * mats[tall[k]]->gh * (plan[k].begin[ctx->comm_rank + 1] - plan[k].begin[ctx->comm_rank]));
-    uint32_t* ext[2] = {nullptr, nullptr};
-    struct ExtGuard { vgpu_ctx* c; uint32_t** e; ~ExtGuard() { vg_free(c, e[0]); vg_free(c, e[1]); } } eg{ctx, ext};
-    if (ext_words) { VG_TRY(vg_alloc(ctx, (void**)&ext[0], ext_words * 4)); if (overlap) VG_TRY(vg_alloc(ctx, (void**)&ext[1], ext_words * 4)); }
+    VgBuf ext[2] = {VgBuf(ctx), VgBuf(ctx)};
+    if (ext_words) { VG_TRY(ext[0].alloc(ext_words * 4)); if (overlap) VG_TRY(ext[1].alloc(ext_words * 4)); }
     bool used[2] = {false, false};
     for (size_t k = 0; k < tall.size(); k++) {
         const size_t i = tall[k];
         const vgpu_dmat* m = mats[i];
         const uint64_t h = m->gh, H = 2 * h;
         const uint64_t c0 = plan[k].begin[ctx->comm_rank], c1 = plan[k].begin[ctx->comm_rank + 1];
-        VG_TRY(vg_dmat_alloc_run(ctx, H, m->gw, true, true, &pd->ldes[i]));
-        pd->ldes[i]->bitrev_rows = false;        // committed order IS the stored order of an LDE (rows at reverse_bits)
+        VgMat lde;
+        VG_TRY(vg_dmat_alloc_run(ctx, H, m->gw, true, true, &lde));
+        lde->bitrev_rows = false;                // committed order IS the stored order of an LDE (rows at reverse_bits)
+        pd->ldes[i] = lde.release();
         if (c1 <= c0) continue;
         const uint32_t* src; uint64_t scs;
         if (m->dist == VG_ROWS) { src = cols[k]; scs = h; }
         else { src = m->d + c0 * m->col_stride; scs = m->col_stride; }
         const int b = overlap ? (int)(k & 1) : 0;
         if (overlap && used[b]) VG_CUDA(ctx, cudaStreamWaitEvent(ctx->stream, ctx->xfer_ev[b], 0));
-        VG_TRY(vg_coset_lde(ctx, src, scs, h, c1 - c0, lde_shift_of(coset_shifts_or_null, (uint32_t)i), ext[b], H, true, m->bitrev_rows));
+        VG_TRY(vg_coset_lde(ctx, src, scs, h, c1 - c0, lde_shift_of(coset_shifts_or_null, (uint32_t)i), ext[b].as<uint32_t>(), H, true, m->bitrev_rows));
         if (overlap) {
             VG_CUDA(ctx, cudaEventRecord(ctx->xfer_ev[2], ctx->stream));
             VG_CUDA(ctx, cudaStreamWaitEvent(ctx->xfer_stream, ctx->xfer_ev[2], 0));
-            VG_TRY(vg_exchange_cols_to_rows(ctx, ext[b], H, c0, c1, pd->ldes[i], ctx->xfer_stream));
+            VG_TRY(vg_exchange_cols_to_rows(ctx, ext[b].as<uint32_t>(), H, c0, c1, pd->ldes[i], ctx->xfer_stream));
             VG_CUDA(ctx, cudaEventRecord(ctx->xfer_ev[b], ctx->xfer_stream));
             used[b] = true;
         } else {
-            VG_TRY(vg_exchange_cols_to_rows(ctx, ext[0], H, c0, c1, pd->ldes[i]));
+            VG_TRY(vg_exchange_cols_to_rows(ctx, ext[0].as<uint32_t>(), H, c0, c1, pd->ldes[i]));
         }
     }
     if (overlap) for (int b = 0; b < 2; b++) if (used[b]) VG_CUDA(ctx, cudaStreamWaitEvent(ctx->stream, ctx->xfer_ev[b], 0));
@@ -558,19 +553,19 @@ int32_t vgpu_commit_batches(vgpu_ctx* ctx, const vgpu_dmat* const* mats, uint32_
                             uint32_t digest_out[8], vgpu_prover_data** out) {
     VG_TRY(vg_enter(ctx));
     if (ctx->merkle_hash == VGPU_MERKLE_POSEIDON16 && !ctx->challenger_set) VG_FAIL(ctx, "commit: the Poseidon-16 Merkle hash needs vgpu_set_challenger first");
-    vgpu_prover_data* pd = new (std::nothrow) vgpu_prover_data();
+    VgPd pd(new (std::nothrow) vgpu_prover_data());
     if (!pd) VG_FAIL(ctx, "out of host memory");
     pd->ctx = ctx;
     pd->ldes.assign(n, nullptr);
     std::vector<uint64_t> heights(n);
     std::vector<size_t> tall;
     for (uint32_t i = 0; i < n; i++) {
-        if (!mats[i]) { vgpu_prover_data_free(pd); VG_FAIL(ctx, "commit: matrix %u is null", i); }
+        if (!mats[i]) VG_FAIL(ctx, "commit: matrix %u is null", i);
         heights[i] = mats[i]->gh * 2;
         if (vg_trace_run(ctx, mats[i]->gh).split) tall.push_back(i);
-        else if (mats[i]->dist != VG_FULL) { vgpu_prover_data_free(pd); VG_FAIL(ctx, "commit: matrix %u is a shard but too short to be split", i); }
+        else if (mats[i]->dist != VG_FULL) VG_FAIL(ctx, "commit: matrix %u is a shard but too short to be split", i);
     }
-    int32_t rc = tall.empty() ? 0 : extend_split(ctx, pd, mats, tall, coset_shifts_or_null);
+    if (!tall.empty()) VG_TRY(extend_split(ctx, pd.get(), mats, tall, coset_shifts_or_null));
     // The other matrices one height group at a time, when the tree reaches that height; a matrix whose upload is still in
     // flight is waited for here, not earlier.  (Split proof: short matrices are extended, whole, by every rank.)
     auto extend_group = [&](const std::vector<size_t>& group) -> int32_t {
@@ -581,21 +576,21 @@ int32_t vgpu_commit_batches(vgpu_ctx* ctx, const vgpu_dmat* const* mats, uint32_
         }
         return 0;
     };
-    if (rc == 0) rc = vg_merkle_build(ctx, pd, heights, extend_group);
-    if (rc) { vgpu_prover_data_free(pd); return rc; }
+    VG_TRY(vg_merkle_build(ctx, pd.get(), heights, extend_group));
     if (digest_out) std::memcpy(digest_out, pd->root, 32);
-    *out = pd;
+    *out = pd.release();
     return 0;
 }
 
 int32_t vgpu_commit_batches_host(vgpu_ctx* ctx, const vgpu_matrix* mats, uint32_t n, int32_t repr, const uint32_t* coset_shifts_or_null,
                                  uint32_t digest_out[8], vgpu_prover_data** out) {
-    std::vector<vgpu_dmat*> dm(n, nullptr);
-    int32_t rc = 0;
-    for (uint32_t i = 0; i < n && rc == 0; i++) rc = vgpu_dmat_upload_rows(ctx, &mats[i], repr, &dm[i]);   // a split proof uploads each rank's rows only
-    if (rc == 0) rc = vgpu_commit_batches(ctx, dm.data(), n, coset_shifts_or_null, digest_out, out);
-    for (auto* m : dm) vgpu_dmat_free(m);
-    return rc;
+    std::vector<VgMat> dm(n);
+    for (uint32_t i = 0; i < n; i++) {   // a split proof uploads each rank's rows only
+        vgpu_dmat* m = nullptr;
+        VG_TRY(vgpu_dmat_upload_rows(ctx, &mats[i], repr, &m));
+        dm[i].reset(m);
+    }
+    return vgpu_commit_batches(ctx, vg_handles(dm).data(), n, coset_shifts_or_null, digest_out, out);
 }
 
 int32_t vgpu_prover_data_lde(const vgpu_prover_data* pd, uint32_t i, const vgpu_dmat** view) {
@@ -606,8 +601,7 @@ int32_t vgpu_prover_data_lde(const vgpu_prover_data* pd, uint32_t i, const vgpu_
 void vgpu_prover_data_free(vgpu_prover_data* pd) {
     if (!pd) return;
     for (auto* m : pd->ldes) vgpu_dmat_free(m);
-    vg_tree_free(pd->ctx, &pd->tree);
-    delete pd;
+    delete pd;                                   // and with it the tree's digests
 }
 
 }  // extern "C"

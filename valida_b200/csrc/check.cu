@@ -120,9 +120,9 @@ extern "C" int32_t vgpu_check_constraints(vgpu_ctx* ctx, const vgpu_chip_desc* c
                                           int64_t* first_row, uint32_t* first_constraint, uint64_t* failing_rows) {
     if (!first_row || !first_constraint || !failing_rows) VG_FAIL(ctx, "check_constraints: null output");
     VG_TRY(vg_enter(ctx));
-    unsigned long long* d = nullptr;
-    VG_TRY(vg_alloc(ctx, (void**)&d, 2 * sizeof(unsigned long long)));
-    struct Free { vgpu_ctx* c; void* p; ~Free() { vg_free(c, p); } } fr{ctx, d};
+    VgBuf buf(ctx);
+    VG_TRY(buf.alloc(2 * sizeof(unsigned long long)));
+    unsigned long long* d = buf.as<unsigned long long>();
     VG_CUDA(ctx, cudaMemsetAsync(d, 0xff, sizeof(unsigned long long), ctx->stream));
     VG_CUDA(ctx, cudaMemsetAsync(d + 1, 0, sizeof(unsigned long long), ctx->stream));
     VG_TRY(vg_check_enqueue(ctx, chip, main, prep_or_null, perm, challenges, d, d + 1));

@@ -1,7 +1,9 @@
 // Internal context / device-matrix definitions shared by the kernels' host wrappers.
 #pragma once
+#include <algorithm>
 #include <cstdint>
 #include <cstdio>
+#include <memory>
 #include <string>
 #include <vector>
 #include <map>
@@ -140,6 +142,40 @@ struct KScope {
 int32_t vg_enter(vgpu_ctx* ctx);                          // make ctx->device current on the calling thread
 int32_t vg_alloc(vgpu_ctx* ctx, void** p, size_t bytes);
 void vg_free(vgpu_ctx* ctx, void* p);
+
+// The owner of one vg_alloc block: the block goes back to the context's cache when the owner does (or at reset()), on every
+// exit path, so a call that fails leaves nothing live.
+struct VgBuf {
+    vgpu_ctx* ctx = nullptr;
+    void* p = nullptr;
+    explicit VgBuf(vgpu_ctx* c = nullptr) : ctx(c) {}
+    VgBuf(VgBuf&& o) noexcept : ctx(o.ctx), p(o.release()) {}
+    VgBuf& operator=(VgBuf&& o) noexcept { if (this != &o) { reset(); ctx = o.ctx; p = o.release(); } return *this; }
+    ~VgBuf() { reset(); }
+    int32_t alloc(size_t bytes) { reset(); return vg_alloc(ctx, &p, bytes); }
+    // count elements copied from the host on the context's stream; a pageable `host` may go once this returns (the runtime
+    // stages such a copy before the call returns)
+    template <class T> int32_t upload(const T* host, size_t count) {
+        VG_TRY(alloc(std::max<size_t>(count, 1) * sizeof(T)));
+        if (count) VG_CUDA(ctx, cudaMemcpyAsync(p, host, count * sizeof(T), cudaMemcpyHostToDevice, ctx->stream));
+        return 0;
+    }
+    template <class T> T* as() const { return (T*)p; }
+    explicit operator bool() const { return p != nullptr; }
+    void reset() { vg_free(ctx, p); p = nullptr; }
+    void* release() { void* q = p; p = nullptr; return q; }
+};
+// Owners of the handles the entry points hand out; an entry point passes its result on with release() once it has succeeded.
+struct VgMatFree { void operator()(vgpu_dmat* m) const { vgpu_dmat_free(m); } };
+struct VgPdFree { void operator()(vgpu_prover_data* p) const { vgpu_prover_data_free(p); } };
+using VgMat = std::unique_ptr<vgpu_dmat, VgMatFree>;
+using VgPd = std::unique_ptr<vgpu_prover_data, VgPdFree>;
+// the handles of owned matrices, for the calls that take an array of them
+inline std::vector<vgpu_dmat*> vg_handles(const std::vector<VgMat>& v) {
+    std::vector<vgpu_dmat*> r;
+    for (const VgMat& m : v) r.push_back(m.get());
+    return r;
+}
 // pow.cu: the context's Poseidon-16 constants on the device (poseidon.cuh layout), uploaded on first use; an error before vgpu_set_challenger
 int32_t vg_poseidon_consts(vgpu_ctx* ctx, uint32_t** out);
 int32_t vg_get_shift_table(vgpu_ctx* ctx, uint32_t shift_canonical, uint32_t scale_canonical, uint64_t max_exp, const PowTable** out);
@@ -164,8 +200,8 @@ inline VgRun vg_layer_run(uint64_t len, int nranks, int rank) { return vg_run(le
 inline bool vg_reports_replicated(const vgpu_ctx* ctx) { return ctx->comm_rank == 0 || !vg_sharded(ctx); }
 // The part of a gh x gw matrix this rank holds: its run of gh / comm_size stored rows when `split` (VG_ROWS), else all of it
 // (VG_FULL).  symm: taken from the symmetric heap (peers store into it).
-int32_t vg_dmat_alloc_run(vgpu_ctx* ctx, uint64_t gh, uint64_t gw, bool split, bool symm, vgpu_dmat** out);
-inline int32_t vg_dmat_alloc(vgpu_ctx* ctx, uint64_t h, uint64_t w, vgpu_dmat** out) { return vg_dmat_alloc_run(ctx, h, w, false, false, out); }
+int32_t vg_dmat_alloc_run(vgpu_ctx* ctx, uint64_t gh, uint64_t gw, bool split, bool symm, VgMat* out);
+inline int32_t vg_dmat_alloc(vgpu_ctx* ctx, uint64_t h, uint64_t w, VgMat* out) { return vg_dmat_alloc_run(ctx, h, w, false, false, out); }
 
 // host/comm.cc — every rank calls these in the same order with the same sizes
 // buf holds comm_size consecutive blocks of `words_per_rank` u32; this rank's block is already filled

@@ -54,18 +54,20 @@ void phases_reset(vgpu_ctx* ctx) {
 // An ext5 vector over the rows of one LDE height (reduced openings, inverse denominators, FRI layers): limb-major.
 // Split proof: a vector of a height whose matrices are row shards holds this rank's run [begin, begin + count) only.
 struct RowVec {
-    uint32_t* d = nullptr;
+    VgBuf d;
     uint64_t n = 0, begin = 0, count = 0;      // whole length; stored run (limb stride = count)
+    uint32_t* data() const { return d.as<uint32_t>(); }
     bool shard() const { return count != n; }
     const uint32_t* at(const vgpu_ctx* ctx, int limb, uint64_t i) const {   // null: another rank reports this element (see VgTree::node)
-        if (!shard()) return vg_reports_replicated(ctx) ? d + (uint64_t)limb * count + i : nullptr;
-        return i >= begin && i < begin + count ? d + (uint64_t)limb * count + (i - begin) : nullptr;
+        if (!shard()) return vg_reports_replicated(ctx) ? data() + (uint64_t)limb * count + i : nullptr;
+        return i >= begin && i < begin + count ? data() + (uint64_t)limb * count + (i - begin) : nullptr;
     }
 };
 int32_t rowvec_alloc(vgpu_ctx* ctx, uint64_t n, RowVec* v) {
     const VgRun run = vg_row_run(ctx, n);
     v->n = n; v->begin = run.begin; v->count = run.count;
-    return vg_alloc(ctx, (void**)&v->d, 5 * v->count * 4);
+    v->d = VgBuf(ctx);
+    return v->d.alloc(5 * v->count * 4);
 }
 
 struct FriLayer { RowVec values; VgTree tree; };
@@ -77,26 +79,6 @@ struct PointKey {
 
 int log2u(uint64_t n) { int l = 0; while ((1ull << l) < n) l++; return l; }
 
-// Device buffers of open_multi_batches, released on every exit path.
-struct OpenScratch {
-    vgpu_ctx* ctx;
-    std::map<PointKey, uint32_t*> invden;       // (height, point) -> 1/(x - z) over this rank's rows of the coset
-    RowVec ro[32];
-    uint32_t* d_sums = nullptr;
-    RowVec current;
-    std::vector<FriLayer> layers;
-    uint32_t* paths = nullptr;                  // the rebuilt lower levels of the query paths (vg_tree_paths)
-    explicit OpenScratch(vgpu_ctx* c) : ctx(c) {}
-    void drop_invden() { for (auto& kv : invden) vg_free(ctx, kv.second); invden.clear(); vg_free(ctx, d_sums); d_sums = nullptr; }
-    ~OpenScratch() {
-        drop_invden();
-        vg_free(ctx, paths);
-        for (auto& r : ro) vg_free(ctx, r.d);
-        vg_free(ctx, current.d);
-        for (auto& L : layers) { vg_free(ctx, L.values.d); vg_tree_free(ctx, &L.tree); }
-    }
-};
-
 int32_t open_multi_batches(vgpu_ctx* ctx, const std::vector<OpenRound>& rounds, vgh::Challenger& ch, vgh::OpenedValues* values, vgh::PcsProof* out) {
     const E5 alpha = ch.sample_ext();
     // alpha^c table (host; the reduced-opening kernel takes its powers through the kernel parameters)
@@ -105,7 +87,12 @@ int32_t open_multi_batches(vgpu_ctx* ctx, const std::vector<OpenRound>& rounds, 
     std::vector<E5> apow(max_w + 1);
     { E5 a = bb::e5_one(); for (uint32_t c = 0; c <= max_w; c++) { apow[c] = a; a = bb::e5_mul(a, alpha); } }
 
-    OpenScratch S(ctx);
+    std::map<PointKey, VgBuf> invden;           // (height, point) -> 1/(x - z) over this rank's rows of the coset
+    RowVec ro[32];                              // reduced openings by log height
+    VgBuf d_sums(ctx);
+    RowVec current;                             // the FRI layer being folded
+    std::vector<FriLayer> layers;
+    VgBuf paths(ctx);                           // the rebuilt lower levels of the query paths (vg_tree_paths)
     uint64_t num_reduced[32] = {0};
     // Pass 1 — enqueue, for every matrix, the inverse denominators of its points and the column sums behind p_c(z_q); nothing
     // here waits for the device.  One copy brings the sums of all matrices back.
@@ -121,28 +108,27 @@ int32_t open_multi_batches(vgpu_ctx* ctx, const std::vector<OpenRound>& rounds, 
             j.sums_at = sums_words; sums_words += vg_eval_columns_words(j.w);
             jobs.push_back(j);
         }
-    VG_TRY(vg_alloc(ctx, (void**)&S.d_sums, sums_words * 4));
+    VG_TRY(d_sums.alloc(sums_words * 4));
     for (Job& j : jobs) {
-        RowVec& R = S.ro[j.log_H];
+        RowVec& R = ro[j.log_H];
         if (!R.d) {
             VG_TRY(rowvec_alloc(ctx, j.lde->gh, &R));
-            VG_CUDA(ctx, cudaMemsetAsync(R.d, 0, 5 * R.count * 4, ctx->stream));
+            VG_CUDA(ctx, cudaMemsetAsync(R.data(), 0, 5 * R.count * 4, ctx->stream));
         }
         for (size_t q = 0; q < j.pts->size(); q++) {
             PointKey key; key.log_H = j.log_H; std::memcpy(key.c, (*j.pts)[q].c, 20);
-            auto it = S.invden.find(key);
-            if (it == S.invden.end()) {
-                uint32_t* buf = nullptr;
-                VG_TRY(vg_alloc(ctx, (void**)&buf, 5 * R.count * 4));
-                it = S.invden.emplace(key, buf).first;
-                VG_TRY(vg_inverse_denominators(ctx, j.log_H, (*j.pts)[q], R.begin, R.count, buf));
+            auto it = invden.find(key);
+            if (it == invden.end()) {
+                it = invden.emplace(key, VgBuf(ctx)).first;
+                VG_TRY(it->second.alloc(5 * R.count * 4));
+                VG_TRY(vg_inverse_denominators(ctx, j.log_H, (*j.pts)[q], R.begin, R.count, it->second.as<uint32_t>()));
             }
-            j.dens[q] = it->second;
+            j.dens[q] = it->second.as<uint32_t>();
         }
-        VG_TRY(vg_eval_columns_enqueue(ctx, j.lde, (uint32_t)j.pts->size(), j.dens, R.count, S.d_sums + j.sums_at));
+        VG_TRY(vg_eval_columns_enqueue(ctx, j.lde, (uint32_t)j.pts->size(), j.dens, R.count, d_sums.as<uint32_t>() + j.sums_at));
     }
     std::vector<uint32_t> sums(sums_words);
-    VG_CUDA(ctx, cudaMemcpyAsync(sums.data(), S.d_sums, sums_words * 4, cudaMemcpyDeviceToHost, ctx->stream));
+    VG_CUDA(ctx, cudaMemcpyAsync(sums.data(), d_sums.p, sums_words * 4, cudaMemcpyDeviceToHost, ctx->stream));
     VG_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
     // Pass 2 — opened values on the host, then the reduced openings of every matrix (again without waiting)
     values->clear();
@@ -168,51 +154,51 @@ int32_t open_multi_batches(vgpu_ctx* ctx, const std::vector<OpenRound>& rounds, 
                 const E5 a_off = bb::e5_pow(alpha, num_reduced[j.log_H]);
                 num_reduced[j.log_H] += (uint64_t)w * np;
                 for (uint32_t c = 0; c < w; c++) apow_off[c] = bb::e5_mul(a_off, apow[c]);
-                VG_TRY(vg_reduced_opening_accumulate(ctx, j.lde, apow_off.data(), apow[w], np, j.dens, S.ro[j.log_H].count, sum_y, S.ro[j.log_H].d));
+                VG_TRY(vg_reduced_opening_accumulate(ctx, j.lde, apow_off.data(), apow[w], np, j.dens, ro[j.log_H].count, sum_y, ro[j.log_H].data()));
             }
         }
     }
-    S.drop_invden();
+    invden.clear();
+    d_sums.reset();
 
     // ---- p3-fri prove: commit phase --------------------------------------------------------------
     // Split proof: while a layer is long enough it stays in row shards — a fold pairs neighbours (2i, 2i+1), so a rank folds its
     // own run, hashes its own leaves and sub-tree, and only the sub-roots meet; the first layer too short to split is
     // all-gathered once and folded by every rank from there on.
     int log_max = 31;
-    while (log_max >= 0 && !S.ro[log_max].d) log_max--;
+    while (log_max >= 0 && !ro[log_max].d) log_max--;
     if (log_max < LOG_BLOWUP) VG_FAIL(ctx, "open: nothing to open");
-    S.current = S.ro[log_max];
-    S.ro[log_max] = RowVec();
+    current = std::move(ro[log_max]);
     for (int lfh = log_max - 1; lfh >= LOG_BLOWUP; lfh--) {
-        S.layers.emplace_back();
-        FriLayer& L = S.layers.back();
-        L.values = S.current; S.current = RowVec();
+        layers.emplace_back();
+        FriLayer& L = layers.back();
+        L.values = std::move(current);
         const RowVec& cur = L.values;
         const uint64_t npairs = cur.n / 2;
         Digest root;
-        VG_TRY(vg_fri_layer_commit(ctx, cur.d, cur.count, npairs, cur.shard(), &L.tree, root.data()));
+        VG_TRY(vg_fri_layer_commit(ctx, cur.data(), cur.count, npairs, cur.shard(), &L.tree, root.data()));
         ch.observe_digest_canonical(root.data());
         out->commit_phase_commits.push_back(root);
         E5 beta = ch.sample_ext();
         RowVec next;
         VG_TRY(rowvec_alloc(ctx, npairs, &next));
-        S.current = next;
-        const RowVec& add = S.ro[lfh];
+        const RowVec& add = ro[lfh];
         if (add.d && add.shard() != next.shard()) VG_FAIL(ctx, "open: reduced openings and FRI layer of height 2^%d are distributed differently", lfh);
         const uint64_t i0 = cur.shard() ? cur.begin / 2 : 0, cnt = cur.count / 2;      // outputs folded here
-        VG_TRY(vg_fri_fold(ctx, cur.d, cur.count, cur.n, i0, cnt, beta, add.d ? add.d - add.begin : nullptr, add.count, next.d - next.begin, next.count));
+        VG_TRY(vg_fri_fold(ctx, cur.data(), cur.count, cur.n, i0, cnt, beta, add.d ? add.data() - add.begin : nullptr, add.count, next.data() - next.begin, next.count));
         if (cur.shard() && !next.shard()) {   // every rank folded its run into the whole-length buffer: complete it
             VG_TRY(vg_comm_group_begin(ctx));
-            for (int l = 0; l < 5; l++) VG_TRY(vg_comm_allgather_inplace(ctx, next.d + (uint64_t)l * next.count, cnt));
+            for (int l = 0; l < 5; l++) VG_TRY(vg_comm_allgather_inplace(ctx, next.data() + (uint64_t)l * next.count, cnt));
             VG_TRY(vg_comm_group_end(ctx));
         }
-        if (S.ro[lfh].d) { vg_free(ctx, S.ro[lfh].d); S.ro[lfh] = RowVec(); }
+        current = std::move(next);
+        ro[lfh] = RowVec();
     }
     {
-        const RowVec& cur = S.current;
+        const RowVec& cur = current;
         if (cur.shard()) VG_FAIL(ctx, "open: the final FRI layer is still distributed");
         std::vector<uint32_t> fin(5 * cur.n);
-        VG_CUDA(ctx, cudaMemcpyAsync(fin.data(), cur.d, fin.size() * 4, cudaMemcpyDeviceToHost, ctx->stream));
+        VG_CUDA(ctx, cudaMemcpyAsync(fin.data(), cur.data(), fin.size() * 4, cudaMemcpyDeviceToHost, ctx->stream));
         VG_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
         E5 f0;
         for (int l = 0; l < 5; l++) f0.c[l] = fin[l * cur.n];
@@ -233,17 +219,17 @@ int32_t open_multi_batches(vgpu_ctx* ctx, const std::vector<OpenRound>& rounds, 
     // every query asks for the same NUMBER of words (its index only selects which): the 40 pointer lists, and later the 40 answers,
     // are filled by the host threads in parallel
     size_t per_query = 0;
-    for (auto& L : S.layers) per_query += 5 + 8 * (L.tree.layer_ptr.size() - 1);
+    for (auto& L : layers) per_query += 5 + 8 * (L.tree.layer_ptr.size() - 1);
     for (const OpenRound& rd : rounds) { for (auto* m : rd.pd->ldes) per_query += m->w; per_query += 8 * (size_t)log2u(rd.pd->max_height); }
     const long nq = (long)indices.size();
     // the path levels below the kept tree layers: every tree's, of every query, rebuilt in one launch (merkle.h) — by the rank that
     // reports the leaf, as for the stored levels; tree t of query qi writes slot qi * trees + t
     std::vector<VgPathTree> trees;
-    for (const FriLayer& L : S.layers) trees.push_back({&L.tree, nullptr, L.values.d - L.values.begin, L.values.count});
+    for (const FriLayer& L : layers) trees.push_back({&L.tree, nullptr, L.values.data() - L.values.begin, L.values.count});
     for (const OpenRound& rd : rounds) trees.push_back({&rd.pd->tree, rd.pd, nullptr, 0});
     auto leaf_of = [&](size_t t, uint64_t index) -> uint64_t {     // the leaf of tree t a query index opens
-        if (t < S.layers.size()) return index >> (t + 1);
-        return index >> (log_max - log2u(rounds[t - S.layers.size()].pd->max_height));
+        if (t < layers.size()) return index >> (t + 1);
+        return index >> (log_max - log2u(rounds[t - layers.size()].pd->max_height));
     };
     std::vector<VgPathReq> reqs;
     for (long qi = 0; qi < nq; qi++)
@@ -251,8 +237,8 @@ int32_t open_multi_batches(vgpu_ctx* ctx, const std::vector<OpenRound>& rounds, 
             const uint64_t leaf = leaf_of(t, indices[qi]);
             if (trees[t].tree->rebuilt() && trees[t].tree->reports(ctx, 0, leaf)) reqs.push_back({(uint32_t)t, (uint32_t)(qi * trees.size() + t), leaf});
         }
-    VG_TRY(vg_tree_paths(ctx, trees, reqs, (size_t)nq * trees.size(), &S.paths));
-    const uint32_t* paths = S.paths;
+    VG_TRY(vg_tree_paths(ctx, trees, reqs, (size_t)nq * trees.size(), &paths));
+    const uint32_t* path_words = paths.as<uint32_t>();
     std::vector<const uint32_t*> ptrs(per_query * (size_t)nq);
 #pragma omp parallel for schedule(static) num_threads(8)
     for (long qi = 0; qi < nq; qi++) {
@@ -262,12 +248,12 @@ int32_t open_multi_batches(vgpu_ctx* ctx, const std::vector<OpenRound>& rounds, 
         auto push_path = [&](size_t t) {     // the sibling digests of tree t's path, leaf level first
             const VgTree& tr = *trees[t].tree;
             const uint64_t leaf = leaf_of(t, index);
-            const uint32_t* rebuilt = tr.reports(ctx, 0, leaf) ? paths + ((size_t)qi * trees.size() + t) * VG_TREE_DROP * 8 : nullptr;
+            const uint32_t* rebuilt = tr.reports(ctx, 0, leaf) ? path_words + ((size_t)qi * trees.size() + t) * VG_TREE_DROP * 8 : nullptr;
             for (size_t lvl = 0; lvl < tr.depth(); lvl++)
                 push_digest(lvl < tr.rebuilt() ? (rebuilt ? rebuilt + lvl * 8 : nullptr) : tr.node(ctx, lvl, (leaf >> lvl) ^ 1));
         };
-        for (size_t i = 0; i < S.layers.size(); i++) {
-            const FriLayer& L = S.layers[i];
+        for (size_t i = 0; i < layers.size(); i++) {
+            const FriLayer& L = layers[i];
             uint64_t sib = (index >> i) ^ 1;
             for (int l = 0; l < 5; l++) *o++ = L.values.at(ctx, l, sib);
             push_path(i);
@@ -281,7 +267,7 @@ int32_t open_multi_batches(vgpu_ctx* ctx, const std::vector<OpenRound>& rounds, 
                 const bool mine = m->dist == VG_ROWS ? (row >= m->row0 && row < m->row0 + m->h) : vg_reports_replicated(ctx);
                 for (uint64_t c = 0; c < m->w; c++) *o++ = mine ? m->d + c * m->col_stride + (row - m->row0) : nullptr;
             }
-            push_path(S.layers.size() + r);
+            push_path(layers.size() + r);
         }
     }
     std::vector<uint32_t> words;
@@ -293,11 +279,11 @@ int32_t open_multi_batches(vgpu_ctx* ctx, const std::vector<OpenRound>& rounds, 
         size_t pos = per_query * (size_t)qi;
         auto take_digest = [&]() { Digest d; for (int k = 0; k < 8; k++) d[k] = words[pos++]; return d; };
         std::vector<vgh::CommitPhaseStep>& steps = out->query_proofs[qi];
-        steps.reserve(S.layers.size());
-        for (size_t i = 0; i < S.layers.size(); i++) {
+        steps.reserve(layers.size());
+        for (size_t i = 0; i < layers.size(); i++) {
             vgh::CommitPhaseStep st;
             for (int l = 0; l < 5; l++) st.sibling_value.c[l] = words[pos++];
-            const size_t depth = S.layers[i].tree.layer_ptr.size() - 1;
+            const size_t depth = layers[i].tree.layer_ptr.size() - 1;
             st.opening_proof.reserve(depth);
             for (size_t lvl = 0; lvl < depth; lvl++) st.opening_proof.push_back(take_digest());
             steps.push_back(std::move(st));
@@ -333,10 +319,6 @@ vgh::Poseidon16* poseidon_of(vgpu_ctx* ctx) {
     }
     return (vgh::Poseidon16*)ctx->poseidon;
 }
-
-struct PdGuard { vgpu_prover_data* p = nullptr; ~PdGuard() { if (p) vgpu_prover_data_free(p); } };
-struct BufGuard { vgpu_ctx* ctx; void* p = nullptr; explicit BufGuard(vgpu_ctx* c) : ctx(c) {} ~BufGuard() { vg_free(ctx, p); } };
-struct MatGuard { std::vector<vgpu_dmat*> v; ~MatGuard() { for (auto* m : v) vgpu_dmat_free(m); } };
 
 // The debug mode checks whole traces; a split proof holds row shards, whose last row's "next" row lives on another rank.  Every rank
 // refuses alike, before any collective.
@@ -465,46 +447,53 @@ static int32_t prove_device(vgpu_ctx* ctx, const vgpu_dmat* const main[VGPU_NUM_
     { delete (vgh::Poseidon16*)ctx->poseidon; ctx->poseidon = nullptr; }
     ch.perm = poseidon_of(ctx);
 
-    PdGuard prep_pd, main_pd, perm_pd, quot_pd;
+    // a commit's prover data, owned here from the moment the commit hands it out
+    auto commit = [&](const vgpu_dmat* const* mats, uint32_t n, const uint32_t* shifts, uint32_t digest_out[8], VgPd* pd) -> int32_t {
+        vgpu_prover_data* p = nullptr;
+        VG_TRY(vgpu_commit_batches(ctx, mats, n, shifts, digest_out, &p));
+        pd->reset(p);
+        return 0;
+    };
+    VgPd prep_pd, main_pd, perm_pd, quot_pd;
     uint32_t digest[8];
     {   // preprocessed commit (derive:299-311)
         Phase ph(ctx, "commit preprocessed");
-        VG_TRY(vgpu_commit_batches(ctx, prep, 2, nullptr, digest, &prep_pd.p));
+        VG_TRY(commit(prep, 2, nullptr, digest, &prep_pd));
         ch.observe_digest_canonical(digest);
     }
     vgh::MachineProof mp;
     mp.chip_proofs.resize(VGPU_NUM_CHIPS);
     {   // main commit (313-332)
         Phase ph(ctx, "commit main");
-        VG_TRY(vgpu_commit_batches(ctx, main, VGPU_NUM_CHIPS, nullptr, mp.main_trace.data(), &main_pd.p));
+        VG_TRY(commit(main, VGPU_NUM_CHIPS, nullptr, mp.main_trace.data(), &main_pd));
         ch.observe_digest_canonical(mp.main_trace.data());
     }
     uint32_t perm_challenges[15];
     for (int i = 0; i < 3; i++) { E5 e = ch.sample_ext(); for (int l = 0; l < 5; l++) perm_challenges[5 * i + l] = bb::from_monty(e.c[l]); }
     uint32_t cumsum[VGPU_NUM_CHIPS][5];
     {   // permutation traces (339-358)
-        MatGuard perms;
+        std::vector<VgMat> perms;
         {
             Phase ph(ctx, "permutation traces");
             // the cumulative sums of all chips come back with ONE copy: per chip the per-rank sums of its running sum
             // (debug mode: the check results of the 14 chips, first keys then failing-row counts, ride in the same buffer and copy)
             const uint32_t slots = vg_perm_totals_ranks(ctx);
             const size_t tot_words = (size_t)VGPU_NUM_CHIPS * slots * 5, chk_words = debug ? 4 * VGPU_NUM_CHIPS : 0;
-            BufGuard tot(ctx);
-            VG_TRY(vg_alloc(ctx, (void**)&tot.p, (tot_words + chk_words) * 4));
+            VgBuf tot(ctx);
+            VG_TRY(tot.alloc((tot_words + chk_words) * 4));
             uint32_t nt[VGPU_NUM_CHIPS];
             for (int i = 0; i < VGPU_NUM_CHIPS; i++) {
                 vgpu_dmat* pm = nullptr;
-                VG_TRY(vg_perm_trace_enqueue(ctx, chips[i], main[i], prep_for(i), perm_challenges, &pm, (uint32_t*)tot.p + (size_t)i * slots * 5, &nt[i]));
-                perms.v.push_back(pm);
+                VG_TRY(vg_perm_trace_enqueue(ctx, chips[i], main[i], prep_for(i), perm_challenges, &pm, tot.as<uint32_t>() + (size_t)i * slots * 5, &nt[i]));
+                perms.emplace_back(pm);
             }
             if (debug) {   // check_constraints (derive/src/lib.rs:246-253) while the main traces are still held
                 Phase pc(ctx, "check constraints");
-                unsigned long long* d_chk = (unsigned long long*)((uint32_t*)tot.p + tot_words);   // tot_words is even: 8-byte aligned
+                unsigned long long* d_chk = (unsigned long long*)(tot.as<uint32_t>() + tot_words);   // tot_words is even: 8-byte aligned
                 VG_CUDA(ctx, cudaMemsetAsync(d_chk, 0xff, VGPU_NUM_CHIPS * 8, ctx->stream));
                 VG_CUDA(ctx, cudaMemsetAsync(d_chk + VGPU_NUM_CHIPS, 0, VGPU_NUM_CHIPS * 8, ctx->stream));
                 for (int i = 0; i < VGPU_NUM_CHIPS; i++)
-                    VG_TRY(vg_check_enqueue(ctx, chips[i], main[i], prep_for(i), perms.v[i], perm_challenges, d_chk + i, d_chk + VGPU_NUM_CHIPS + i));
+                    VG_TRY(vg_check_enqueue(ctx, chips[i], main[i], prep_for(i), perms[i].get(), perm_challenges, d_chk + i, d_chk + VGPU_NUM_CHIPS + i));
             }
             std::vector<uint32_t> ht(tot_words + chk_words);
             VG_CUDA(ctx, cudaMemcpyAsync(ht.data(), tot.p, ht.size() * 4, cudaMemcpyDeviceToHost, ctx->stream));
@@ -524,34 +513,34 @@ static int32_t prove_device(vgpu_ctx* ctx, const vgpu_dmat* const main[VGPU_NUM_
             }
         }
         Phase ph(ctx, "commit permutation");
-        VG_TRY(vgpu_commit_batches(ctx, perms.v.data(), VGPU_NUM_CHIPS, nullptr, mp.perm_trace.data(), &perm_pd.p));
+        VG_TRY(commit(vg_handles(perms).data(), VGPU_NUM_CHIPS, nullptr, mp.perm_trace.data(), &perm_pd));
         ch.observe_digest_canonical(mp.perm_trace.data());
     }
     E5 alpha = ch.sample_ext();
     uint32_t alpha_c[5];
     for (int l = 0; l < 5; l++) alpha_c[l] = bb::from_monty(alpha.c[l]);
     {   // quotients (246-270, 362-374)
-        MatGuard quots;
+        std::vector<VgMat> quots;
         {
             Phase ph(ctx, "quotient");
             int prep_idx = 0;
             for (int i = 0; i < VGPU_NUM_CHIPS; i++) {
-                const vgpu_dmat* plde = chips[i]->preprocessed_width ? prep_pd.p->ldes[prep_idx++] : nullptr;
+                const vgpu_dmat* plde = chips[i]->preprocessed_width ? prep_pd->ldes[prep_idx++] : nullptr;
                 vgpu_dmat* q = nullptr;
-                VG_TRY(vgpu_quotient(ctx, chips[i], (uint32_t)log_degrees[i], plde, main_pd.p->ldes[i], perm_pd.p->ldes[i], cumsum[i], perm_challenges, alpha_c, &q));
-                quots.v.push_back(q);
+                VG_TRY(vgpu_quotient(ctx, chips[i], (uint32_t)log_degrees[i], plde, main_pd->ldes[i], perm_pd->ldes[i], cumsum[i], perm_challenges, alpha_c, &q));
+                quots.emplace_back(q);
             }
         }
         Phase ph(ctx, "commit quotient");
         uint32_t shifts[VGPU_NUM_CHIPS];
         for (int i = 0; i < VGPU_NUM_CHIPS; i++) shifts[i] = (uint32_t)(((uint64_t)bb::GEN_CANON * bb::GEN_CANON) % bb::P);   // coset_shift^(2^log_quotient_degree)
-        VG_TRY(vgpu_commit_batches(ctx, quots.v.data(), VGPU_NUM_CHIPS, shifts, mp.quotient_chunks.data(), &quot_pd.p));
+        VG_TRY(commit(vg_handles(quots).data(), VGPU_NUM_CHIPS, shifts, mp.quotient_chunks.data(), &quot_pd));
         ch.observe_digest_canonical(mp.quotient_chunks.data());
     }
     E5 zeta = ch.sample_ext();
     // openings (379-392): main & perm at [zeta, zeta*g_i], quotient at [zeta^2]; preprocessed is NOT opened
     std::vector<OpenRound> rounds(3);
-    rounds[0].pd = main_pd.p; rounds[1].pd = perm_pd.p; rounds[2].pd = quot_pd.p;
+    rounds[0].pd = main_pd.get(); rounds[1].pd = perm_pd.get(); rounds[2].pd = quot_pd.get();
     for (int i = 0; i < VGPU_NUM_CHIPS; i++) {
         E5 zg = bb::e5_mul_base(zeta, bb::two_adic_generator_monty(log_degrees[i]));
         rounds[0].points.push_back({zeta, zg});
@@ -588,28 +577,28 @@ int32_t vgpu_prove(vgpu_ctx* ctx, const vgpu_matrix main[VGPU_NUM_CHIPS], const 
     // Split proof: of a trace tall enough to be split a rank uploads ITS run of rows only (1 / comm_size of the bytes).
     VG_TRY(debug_mode_allowed(ctx));
     VG_TRY(vg_enter(ctx));
-    MatGuard dm, dp;
+    std::vector<VgMat> dm(VGPU_NUM_CHIPS), dp(2);
     phases_reset(ctx);
     auto t0 = std::chrono::steady_clock::now();
-    dm.v.assign(VGPU_NUM_CHIPS, nullptr); dp.v.assign(2, nullptr);
-    auto alloc_for = [&](const vgpu_matrix& hm, vgpu_dmat** out) {
+    auto alloc_for = [&](const vgpu_matrix& hm, VgMat* out) {
         return vg_dmat_alloc_run(ctx, hm.height, hm.width, vg_trace_run(ctx, hm.height).split, false, out);
     };
     auto begin_upload = [&](const vgpu_matrix& hm, vgpu_dmat* m) { return vg_upload_begin(ctx, hm.data + m->row0 * hm.width, m->h, m->w, repr, m); };
-    for (int i = 0; i < 2; i++) VG_TRY(alloc_for(prep[i], &dp.v[i]));
-    for (int i = 0; i < VGPU_NUM_CHIPS; i++) VG_TRY(alloc_for(main[i], &dm.v[i]));
-    for (int i = 0; i < 2; i++) VG_TRY(begin_upload(prep[i], dp.v[i]));
+    for (int i = 0; i < 2; i++) VG_TRY(alloc_for(prep[i], &dp[i]));
+    for (int i = 0; i < VGPU_NUM_CHIPS; i++) VG_TRY(alloc_for(main[i], &dm[i]));
+    for (int i = 0; i < 2; i++) VG_TRY(begin_upload(prep[i], dp[i].get()));
     std::vector<int> order(VGPU_NUM_CHIPS);
     for (int i = 0; i < VGPU_NUM_CHIPS; i++) order[i] = i;
     std::stable_sort(order.begin(), order.end(), [&](int a, int b) { return main[a].height > main[b].height; });
-    for (int i : order) VG_TRY(begin_upload(main[i], dm.v[i]));
+    for (int i : order) VG_TRY(begin_upload(main[i], dm[i].get()));
     float up = std::chrono::duration<float, std::milli>(std::chrono::steady_clock::now() - t0).count();
     ctx->phases.push_back({"upload traces (H2D enqueue; copies overlap the commits)", up});
     // traces in pageable memory are copied by the context's staging threads from here on (staging.cu)
     struct StagerGuard { vgpu_ctx* c; ~StagerGuard() { vg_stager_finish(c); } } sg{ctx};
     VG_TRY(vg_stager_start(ctx));
     ctx->in_host_prove = true;
-    int32_t rc = prove_device(ctx, dm.v.data(), dp.v.data(), dm.v.data(), proof_out, proof_len);
+    const std::vector<vgpu_dmat*> mains = vg_handles(dm), preps = vg_handles(dp);
+    int32_t rc = prove_device(ctx, mains.data(), preps.data(), mains.data(), proof_out, proof_len);
     ctx->in_host_prove = false;
     if (rc == 0) rc = vg_stager_finish(ctx);
     return rc;

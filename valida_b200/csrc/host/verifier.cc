@@ -242,9 +242,9 @@ extern "C" int32_t vgpu_verify(vgpu_ctx* ctx, const uint8_t* proof, uint64_t pro
         const bool was_sharding = ctx->sharding;
         ctx->sharding = false;
         const int32_t rc = vgpu_commit_batches_host(ctx, prep, 2, repr, nullptr, digest, &pd);
+        const VgPd commitment(pd);               // only its root is needed
         ctx->sharding = was_sharding;
         if (rc) return rc;
-        vgpu_prover_data_free(pd);
         ch.observe_digest_canonical(digest);
     }
     ch.observe_digest_canonical(pf.main_trace.data());

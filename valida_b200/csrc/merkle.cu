@@ -576,17 +576,18 @@ static std::vector<LayerPlan> plan_tree(const vgpu_ctx* ctx, uint64_t leaves, bo
 // context's cache when the build returns (the kernels writing and reading it are already enqueued on the context's stream), and
 // the tree's pointers into it cleared.
 struct LowerLayers {
-    vgpu_ctx* ctx; VgTree* t; uint32_t* d = nullptr; size_t n = 0;
-    ~LowerLayers() { vg_free(ctx, d); for (size_t i = 0; i < n; i++) t->layer_ptr[i] = nullptr; }
+    VgTree* t; VgBuf d; size_t n = 0;
+    ~LowerLayers() { for (size_t i = 0; i < n; i++) t->layer_ptr[i] = nullptr; }
 };
 static int32_t alloc_tree(vgpu_ctx* ctx, const std::vector<LayerPlan>& plan, VgTree* t, LowerLayers* low) {
     const size_t keep = std::min(plan.size() - 1, VG_TREE_DROP);     // first kept layer
     uint64_t kept = 0, dropped = 0;
     for (size_t i = 0; i < plan.size(); i++) (i < keep ? dropped : kept) += plan[i].scount;
-    VG_TRY(vg_alloc(ctx, (void**)&t->digests, kept * 32));
-    if (dropped) VG_TRY(vg_alloc(ctx, (void**)&low->d, dropped * 32));
+    t->digests = VgBuf(ctx);
+    VG_TRY(t->digests.alloc(kept * 32));
+    if (dropped) VG_TRY(low->d.alloc(dropped * 32));
     t->layer_ptr.clear(); t->layer_len.clear(); t->layer_begin.clear(); t->layer_count.clear();
-    uint32_t* at[2] = {low->d, t->digests};
+    uint32_t* at[2] = {low->d.as<uint32_t>(), t->digests.as<uint32_t>()};
     for (size_t i = 0; i < plan.size(); i++) {
         const LayerPlan& p = plan[i];
         uint32_t*& a = at[i >= keep];
@@ -596,7 +597,6 @@ static int32_t alloc_tree(vgpu_ctx* ctx, const std::vector<LayerPlan>& plan, VgT
     low->n = keep;
     return 0;
 }
-void vg_tree_free(vgpu_ctx* ctx, VgTree* t) { vg_free(ctx, t->digests); t->digests = nullptr; }
 
 // digest of rows [row0, row0 + nrows) of the concatenated matrices, written to digests_v[row * 8] (digests_v is a VIRTUAL
 // base: the stored run starts at its first row).  A row shard contributes its local rows through a base shifted likewise.
@@ -621,17 +621,14 @@ static int32_t hash_rows(vgpu_ctx* ctx, bool p16, const std::vector<const vgpu_d
         VG_LAUNCH_CHECK(ctx);
         return 0;
     }
-    const uint32_t** dcols = nullptr;
-    VG_TRY(vg_alloc(ctx, (void**)&dcols, cols.size() * sizeof(void*)));
-    // cudaMemcpyAsync from pageable memory stages synchronously: `cols` may go once the call returns
-    VG_CUDA(ctx, cudaMemcpyAsync(dcols, cols.data(), cols.size() * sizeof(void*), cudaMemcpyHostToDevice, ctx->stream));
+    VgBuf dcols(ctx);
+    VG_TRY(dcols.upload(cols.data(), cols.size()));
     {
         KScope ks(ctx, p16 ? KC_P16_LEAF : KC_LEAF_HASH, (double)nrows * (4.0 * nwords + 32.0));
-        if (p16) p16_leaf_kernel<<<grid, 128, 0, ctx->stream>>>(dcols, nwords, row0, nrows, digests_v, consts);
-        else leaf_hash_kernel<<<grid, 128, 0, ctx->stream>>>(dcols, nwords, row0, nrows, digests_v);
+        if (p16) p16_leaf_kernel<<<grid, 128, 0, ctx->stream>>>(dcols.as<const uint32_t*>(), nwords, row0, nrows, digests_v, consts);
+        else leaf_hash_kernel<<<grid, 128, 0, ctx->stream>>>(dcols.as<const uint32_t*>(), nwords, row0, nrows, digests_v);
     }
     VG_LAUNCH_CHECK(ctx);
-    vg_free(ctx, dcols);
     return 0;
 }
 
@@ -707,7 +704,7 @@ static int32_t build_upper_layers(vgpu_ctx* ctx, const std::vector<LayerPlan>& p
 // Single-matrix tree over ext5 pairs (p3-fri commit phase).
 int32_t vg_fri_layer_commit(vgpu_ctx* ctx, const uint32_t* v, uint64_t cs, uint64_t npairs, bool v_is_shard, VgTree* tree, uint32_t root_out[8]) {
     const std::vector<LayerPlan> plan = plan_tree(ctx, npairs, v_is_shard);
-    LowerLayers low{ctx, tree};
+    LowerLayers low{tree, VgBuf(ctx)};
     VG_TRY(alloc_tree(ctx, plan, tree, &low));
     tree->hash = ctx->merkle_hash;
     const bool p16 = tree->hash == VGPU_MERKLE_POSEIDON16;
@@ -741,7 +738,7 @@ int32_t vg_merkle_build(vgpu_ctx* ctx, vgpu_prover_data* pd, const std::vector<u
     if (max_h & (max_h - 1)) VG_FAIL(ctx, "commit: heights must be powers of two");
     pd->max_height = max_h;
     const std::vector<LayerPlan> plan = plan_tree(ctx, max_h, vg_row_run(ctx, max_h).split);
-    LowerLayers low{ctx, &pd->tree};
+    LowerLayers low{&pd->tree, VgBuf(ctx)};
     VG_TRY(alloc_tree(ctx, plan, &pd->tree, &low));
     pd->tree.hash = ctx->merkle_hash;
     const bool p16 = pd->tree.hash == VGPU_MERKLE_POSEIDON16;
@@ -761,21 +758,20 @@ int32_t vg_merkle_build(vgpu_ctx* ctx, vgpu_prover_data* pd, const std::vector<u
     };
     VG_TRY(take(max_h));
     VG_TRY(hash_rows(ctx, p16, group, plan[0].cbegin, plan[0].ccount, pd->tree.layer_ptr[0] - plan[0].sbegin * 8));
-    uint32_t* inject_buf = nullptr;
+    VgBuf inject_buf(ctx);
     if (pos < n) {
         // one layer's row digests at a time — except inside a fused run of short layers, where the digests of every injecting
         // layer of the run (at most 2 * TAIL_FUSE in all) must coexist
         const uint64_t c1 = plan.size() > 1 ? plan[1].ccount : 1;
-        VG_TRY(vg_alloc(ctx, (void**)&inject_buf, (c1 <= 2 * TAIL_FUSE ? 2 * c1 : c1) * 32));
+        VG_TRY(inject_buf.alloc((c1 <= 2 * TAIL_FUSE ? 2 * c1 : c1) * 32));
     }
-    int32_t rc = build_upper_layers(ctx, plan, &pd->tree, inject_buf, [&](size_t, const LayerPlan& p, uint32_t* buf_v, bool* have) -> int32_t {
+    VG_TRY(build_upper_layers(ctx, plan, &pd->tree, inject_buf.as<uint32_t>(), [&](size_t, const LayerPlan& p, uint32_t* buf_v, bool* have) -> int32_t {
         VG_TRY(take(p.len));
         *have = !group.empty();
         if (*have) VG_TRY(hash_rows(ctx, p16, group, p.cbegin, p.ccount, buf_v));
         return 0;
-    });
-    if (inject_buf) vg_free(ctx, inject_buf);
-    if (rc) return rc;
+    }));
+    inject_buf.reset();
     if (pos != n) VG_FAIL(ctx, "commit: a matrix height does not match any tree layer");
     VG_CUDA(ctx, cudaMemcpyAsync(pd->root, pd->tree.layer_ptr.back(), 32, cudaMemcpyDeviceToHost, ctx->stream));
     VG_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
@@ -783,8 +779,9 @@ int32_t vg_merkle_build(vgpu_ctx* ctx, vgpu_prover_data* pd, const std::vector<u
 }
 
 // The lower levels of the requested paths (merkle.h): one upload of the tree table, the column pointers and the requests, one launch.
-int32_t vg_tree_paths(vgpu_ctx* ctx, const std::vector<VgPathTree>& trees, const std::vector<VgPathReq>& reqs, size_t slots, uint32_t** out) {
-    VG_TRY(vg_alloc(ctx, (void**)out, slots * VG_TREE_DROP * 32));
+int32_t vg_tree_paths(vgpu_ctx* ctx, const std::vector<VgPathTree>& trees, const std::vector<VgPathReq>& reqs, size_t slots, VgBuf* out) {
+    *out = VgBuf(ctx);
+    VG_TRY(out->alloc(slots * VG_TREE_DROP * 32));
     if (reqs.empty()) return 0;
     const bool p16 = trees[0].tree->hash == VGPU_MERKLE_POSEIDON16;
     for (const VgPathTree& t : trees)
@@ -819,9 +816,9 @@ int32_t vg_tree_paths(vgpu_ctx* ctx, const std::vector<VgPathTree>& trees, const
     }
     // one device block: [trees][requests][column table]
     const size_t tree_b = pt.size() * sizeof(PathTree), req_b = reqs.size() * sizeof(VgPathReq), col_b = cols.size() * sizeof(void*);
-    uint8_t* blk = nullptr;
-    VG_TRY(vg_alloc(ctx, (void**)&blk, tree_b + req_b + col_b));
-    const uint32_t* const* dcols = reinterpret_cast<const uint32_t* const*>(blk + tree_b + req_b);
+    VgBuf blk(ctx);
+    VG_TRY(blk.alloc(tree_b + req_b + col_b));
+    const uint32_t* const* dcols = reinterpret_cast<const uint32_t* const*>(blk.as<uint8_t>() + tree_b + req_b);
     for (size_t k = 0; k < pt.size(); k++)
         if (trees[k].pd) pt[k].cols = dcols + col_first[k];
     std::vector<uint8_t> host(tree_b + req_b + col_b);
@@ -829,17 +826,16 @@ int32_t vg_tree_paths(vgpu_ctx* ctx, const std::vector<VgPathTree>& trees, const
     std::memcpy(host.data() + tree_b, reqs.data(), req_b);
     std::memcpy(host.data() + tree_b + req_b, cols.data(), col_b);
     // cudaMemcpyAsync from pageable memory stages synchronously: `host` may go once the call returns
-    VG_CUDA(ctx, cudaMemcpyAsync(blk, host.data(), host.size(), cudaMemcpyHostToDevice, ctx->stream));
+    VG_CUDA(ctx, cudaMemcpyAsync(blk.p, host.data(), host.size(), cudaMemcpyHostToDevice, ctx->stream));
     double total = 0;
     for (const VgPathReq& r : reqs) total += bytes[r.tree];
     {
         KScope ks(ctx, p16 ? KC_P16_PATH : KC_TREE_PATH, total);
-        const PathTree* dt = reinterpret_cast<const PathTree*>(blk);
-        const VgPathReq* dr = reinterpret_cast<const VgPathReq*>(blk + tree_b);
-        if (p16) p16_path_kernel<<<(unsigned)reqs.size(), PATH_THREADS, 0, ctx->stream>>>(dt, dr, *out, consts);
-        else query_path_kernel<<<(unsigned)reqs.size(), PATH_THREADS, 0, ctx->stream>>>(dt, dr, *out);
+        const PathTree* dt = blk.as<const PathTree>();
+        const VgPathReq* dr = reinterpret_cast<const VgPathReq*>(blk.as<uint8_t>() + tree_b);
+        if (p16) p16_path_kernel<<<(unsigned)reqs.size(), PATH_THREADS, 0, ctx->stream>>>(dt, dr, out->as<uint32_t>(), consts);
+        else query_path_kernel<<<(unsigned)reqs.size(), PATH_THREADS, 0, ctx->stream>>>(dt, dr, out->as<uint32_t>());
     }
-    vg_free(ctx, blk);
     VG_LAUNCH_CHECK(ctx);
     return 0;
 }

@@ -18,7 +18,7 @@ constexpr size_t VG_TREE_DROP = 8;
 
 struct VgTree {
     int32_t hash = VGPU_MERKLE_KECCAK256;  // the hash it was built with (vgpu_ctx_set_merkle_hash)
-    uint32_t* digests = nullptr;           // the stored parts of the kept layers
+    VgBuf digests;                         // the stored parts of the kept layers
     std::vector<uint32_t*> layer_ptr;      // layer_ptr[i] -> node layer_begin[i] of layer i; null for a dropped layer
     std::vector<uint64_t> layer_len;       // nodes of the whole layer
     std::vector<uint64_t> layer_begin, layer_count;   // the run of nodes computed on this rank (and stored, if the layer is kept)
@@ -54,13 +54,12 @@ int32_t vg_merkle_build(vgpu_ctx* ctx, vgpu_prover_data* pd, const std::vector<u
 // [pair0, pair0 + local_pairs) of the npairs of the layer (all of them, or this rank's run).  The root arrives in root_out
 // once the context's stream has been synchronised (the caller needs it for the transcript anyway).
 int32_t vg_fri_layer_commit(vgpu_ctx* ctx, const uint32_t* v, uint64_t cs, uint64_t npairs, bool v_is_shard, VgTree* tree, uint32_t root_out[8]);
-void vg_tree_free(vgpu_ctx* ctx, VgTree* t);
 
 // The leaves of a tree whose lower paths vg_tree_paths rebuilds: the rows of pd->ldes (an input tree, pd->tree), or the ext5
 // pairs of a FRI layer's values (fri_v: limb-major, limb stride fri_cs, addressed by the layer's global element index).
 struct VgPathTree { const VgTree* tree; const vgpu_prover_data* pd; const uint32_t* fri_v; uint64_t fri_cs; };
 struct VgPathReq { uint32_t tree, slot; uint64_t leaf; };
 // Enqueues ONE launch that writes, for every request, the sibling digests of levels 0 .. rebuilt() - 1 of leaf `leaf`'s path to
-// out[(slot * VG_TREE_DROP + lvl) * 8 ..]; out holds `slots` * VG_TREE_DROP digests (the caller frees it with vg_free).  Every
-// requested leaf must be one this rank reports (VgTree::reports at layer 0).
-int32_t vg_tree_paths(vgpu_ctx* ctx, const std::vector<VgPathTree>& trees, const std::vector<VgPathReq>& reqs, size_t slots, uint32_t** out);
+// out[(slot * VG_TREE_DROP + lvl) * 8 ..]; out receives a block of `slots` * VG_TREE_DROP digests.  Every requested leaf must be
+// one this rank reports (VgTree::reports at layer 0).
+int32_t vg_tree_paths(vgpu_ctx* ctx, const std::vector<VgPathTree>& trees, const std::vector<VgPathReq>& reqs, size_t slots, VgBuf* out);

@@ -718,34 +718,29 @@ int32_t vg_coset_lde(vgpu_ctx* ctx, const uint32_t* src, uint64_t src_cs, uint64
     uint64_t batch = (2ull << 30) / (8 * h);   // coefficient + intermediate scratch <= 2 GB; whole matrices per launch
     if (batch < 1) batch = 1;
     if (batch > w) batch = w;
-    uint32_t *coef = nullptr, *tmp = nullptr;
-    VG_TRY(vg_alloc(ctx, (void**)&coef, batch * h * 4));
-    VG_TRY(vg_alloc(ctx, (void**)&tmp, batch * h * 4));
-    int32_t rc = 0;
-    for (uint64_t c0 = 0; c0 < w && rc == 0; c0 += batch) {
+    VgBuf coef_buf(ctx), tmp_buf(ctx);
+    VG_TRY(coef_buf.alloc(batch * h * 4));
+    VG_TRY(tmp_buf.alloc(batch * h * 4));
+    uint32_t *coef = coef_buf.as<uint32_t>(), *tmp = tmp_buf.as<uint32_t>();
+    for (uint64_t c0 = 0; c0 < w; c0 += batch) {
         uint64_t wc = w - c0 < batch ? w - c0 : batch;
         if (bit_reversed) {
-            rc = src_bitrev ? ntt_bitrev2bitrev(ctx, src + c0 * src_cs, src_cs, coef, h, tmp, h, log_n, wc, false, true, tab)
-                            : intt_nat2bitrev_scaled(ctx, src + c0 * src_cs, src_cs, coef, h, log_n, wc, tab);
-            if (rc) break;
-            rc = ntt_bitrev2bitrev(ctx, coef, h, dst + c0 * dst_cs, dst_cs, tmp, h, log_n, wc, false);
-            if (rc) break;
-            rc = ntt_bitrev2bitrev(ctx, coef, h, dst + c0 * dst_cs + h, dst_cs, tmp, h, log_n, wc, true);
+            VG_TRY(src_bitrev ? ntt_bitrev2bitrev(ctx, src + c0 * src_cs, src_cs, coef, h, tmp, h, log_n, wc, false, true, tab)
+                              : intt_nat2bitrev_scaled(ctx, src + c0 * src_cs, src_cs, coef, h, log_n, wc, tab));
+            VG_TRY(ntt_bitrev2bitrev(ctx, coef, h, dst + c0 * dst_cs, dst_cs, tmp, h, log_n, wc, false));
+            VG_TRY(ntt_bitrev2bitrev(ctx, coef, h, dst + c0 * dst_cs + h, dst_cs, tmp, h, log_n, wc, true));
         } else {
             // natural-order output (API completeness, not on the proving path): zero-pad and transform at size h << log_blowup
-            rc = vg_ntt_nat2nat(ctx, src + c0 * src_cs, src_cs, coef, h, log_n, wc, true, tab, tmp, h);
-            if (rc) break;
+            VG_TRY(vg_ntt_nat2nat(ctx, src + c0 * src_cs, src_cs, coef, h, log_n, wc, true, tab, tmp, h));
             const uint64_t H = h << log_blowup;
-            uint32_t* padb = nullptr; uint32_t* tmp2 = nullptr;
-            rc = vg_alloc(ctx, (void**)&padb, wc * H * 4); if (rc) break;
-            rc = vg_alloc(ctx, (void**)&tmp2, wc * H * 4); if (rc) { vg_free(ctx, padb); break; }
+            VgBuf padb(ctx), tmp2(ctx);
+            VG_TRY(padb.alloc(wc * H * 4));
+            VG_TRY(tmp2.alloc(wc * H * 4));
             uint64_t tot = H * wc;
-            zero_pad_kernel<<<(unsigned)((tot + 255) / 256), 256, 0, ctx->stream>>>(coef, h, padb, H, h, H, wc);
+            zero_pad_kernel<<<(unsigned)((tot + 255) / 256), 256, 0, ctx->stream>>>(coef, h, padb.as<uint32_t>(), H, h, H, wc);
             ctx->launches++;
-            rc = vg_ntt_nat2nat(ctx, padb, H, dst + c0 * dst_cs, dst_cs, log_n + (int)log_blowup, wc, false, nullptr, tmp2, H);
-            vg_free(ctx, padb); vg_free(ctx, tmp2);
+            VG_TRY(vg_ntt_nat2nat(ctx, padb.as<uint32_t>(), H, dst + c0 * dst_cs, dst_cs, log_n + (int)log_blowup, wc, false, nullptr, tmp2.as<uint32_t>(), H));
         }
     }
-    vg_free(ctx, coef); vg_free(ctx, tmp);
-    return rc;
+    return 0;
 }

@@ -408,10 +408,10 @@ int32_t vg_eval_columns_enqueue(vgpu_ctx* ctx, const vgpu_dmat* lde, uint32_t np
     p.mat = lde->d + (uint64_t)c_begin * lde->col_stride; p.mcs = lde->col_stride; p.h = rows; p.row_begin = 0; p.w = w;
     p.invden[0] = invden[0]; p.invden[1] = npoints > 1 ? invden[1] : invden[0]; p.ics = ics; p.npoints = npoints;
     uint32_t nblocks = 1;
-    uint32_t* partial = nullptr;
+    VgBuf partial(ctx);
     const uint32_t nout = w * BARY_OUT, nout_all = (uint32_t)lde->gw * BARY_OUT;
     if (rows == 0) {
-        VG_TRY(vg_alloc(ctx, (void**)&partial, 512));
+        VG_TRY(partial.alloc(512));
     } else if (rows >= BARY_TILE && rows % BARY_TILE == 0) {
         const unsigned by = (w + 31) / 32;
         p.cpg = 2 * (((w + by - 1) / by + 1) / 2);               // columns per CTA, even
@@ -419,8 +419,8 @@ int32_t vg_eval_columns_enqueue(vgpu_ctx* ctx, const vgpu_dmat* lde, uint32_t np
         const uint64_t ntiles = rows / BARY_TILE;
         const unsigned bx = (unsigned)std::min<uint64_t>(ntiles, std::max<uint64_t>(1, (uint64_t)ctx->sm_count / by));
         nblocks = bx * p.rs;
-        VG_TRY(vg_alloc(ctx, (void**)&partial, (size_t)nblocks * w * BARY_OUT * 4));
-        p.partial = partial;
+        VG_TRY(partial.alloc((size_t)nblocks * w * BARY_OUT * 4));
+        p.partial = partial.as<uint32_t>();
         if (!ctx->bary_attrs_set) {
             VG_CUDA(ctx, cudaFuncSetAttribute(bary_kernel<1>, cudaFuncAttributeMaxDynamicSharedMemorySize, 2 * 1 * 5 * BARY_TILE * 4));
             VG_CUDA(ctx, cudaFuncSetAttribute(bary_kernel<2>, cudaFuncAttributeMaxDynamicSharedMemorySize, 2 * 2 * 5 * BARY_TILE * 4));
@@ -431,30 +431,28 @@ int32_t vg_eval_columns_enqueue(vgpu_ctx* ctx, const vgpu_dmat* lde, uint32_t np
         else bary_kernel<1><<<dim3(bx, by), BARY_THREADS, 2 * 1 * 5 * BARY_TILE * 4, ctx->stream>>>(p);
         VG_LAUNCH_CHECK(ctx);
     } else {
-        VG_TRY(vg_alloc(ctx, (void**)&partial, (size_t)w * BARY_OUT * 4));
-        p.partial = partial;
+        VG_TRY(partial.alloc((size_t)w * BARY_OUT * 4));
+        p.partial = partial.as<uint32_t>();
         KScope ks(ctx, KC_BARY, 4.0 * (double)rows * w);
         bary_small_kernel<<<w, 128, 0, ctx->stream>>>(p);
         VG_LAUNCH_CHECK(ctx);
     }
     if (!split) {
-        bary_reduce_kernel<<<(nout + 255) / 256, 256, 0, ctx->stream>>>(partial, nblocks, nout, d_out);
+        bary_reduce_kernel<<<(nout + 255) / 256, 256, 0, ctx->stream>>>(partial.as<uint32_t>(), nblocks, nout, d_out);
         VG_LAUNCH_CHECK(ctx);
     } else {
-        uint32_t* gathered = nullptr;                                                      // [rank 0 | rank 1 | ...], all columns each
-        VG_TRY(vg_alloc(ctx, (void**)&gathered, (size_t)nout_all * 4 * ctx->comm_size));
-        uint32_t* mine = gathered + (size_t)nout_all * ctx->comm_rank;
+        VgBuf gathered(ctx);                                                               // [rank 0 | rank 1 | ...], all columns each
+        VG_TRY(gathered.alloc((size_t)nout_all * 4 * ctx->comm_size));
+        uint32_t* mine = gathered.as<uint32_t>() + (size_t)nout_all * ctx->comm_rank;
         VG_CUDA(ctx, cudaMemsetAsync(mine, 0, (size_t)nout_all * 4, ctx->stream));         // the columns the other coset's ranks sum
         if (nout) {
-            bary_reduce_kernel<<<(nout + 255) / 256, 256, 0, ctx->stream>>>(partial, nblocks, nout, mine + (size_t)c_begin * BARY_OUT);
+            bary_reduce_kernel<<<(nout + 255) / 256, 256, 0, ctx->stream>>>(partial.as<uint32_t>(), nblocks, nout, mine + (size_t)c_begin * BARY_OUT);
             VG_LAUNCH_CHECK(ctx);
         }
-        VG_TRY(vg_comm_allgather_inplace(ctx, gathered, nout_all));
-        bary_reduce_kernel<<<(nout_all + 255) / 256, 256, 0, ctx->stream>>>(gathered, (uint32_t)ctx->comm_size, nout_all, d_out);
+        VG_TRY(vg_comm_allgather_inplace(ctx, gathered.as<uint32_t>(), nout_all));
+        bary_reduce_kernel<<<(nout_all + 255) / 256, 256, 0, ctx->stream>>>(gathered.as<uint32_t>(), (uint32_t)ctx->comm_size, nout_all, d_out);
         VG_LAUNCH_CHECK(ctx);
-        vg_free(ctx, gathered);
     }
-    vg_free(ctx, partial);
     return 0;
 }
 
@@ -532,22 +530,21 @@ int32_t vg_gather_words(vgpu_ctx* ctx, const std::vector<const uint32_t*>& ptrs,
     if (!n) return 0;
     const bool all = vg_sharded(ctx);
     const size_t G = all ? (size_t)ctx->comm_size : 1;
-    const uint32_t** dptr = nullptr; uint32_t* dout = nullptr; uint32_t* dsum = nullptr;
-    VG_TRY(vg_alloc(ctx, (void**)&dptr, n * sizeof(void*)));
-    VG_TRY(vg_alloc(ctx, (void**)&dout, n * 4 * G));
-    VG_CUDA(ctx, cudaMemcpyAsync(dptr, ptrs.data(), n * sizeof(void*), cudaMemcpyHostToDevice, ctx->stream));
-    gather_words_kernel<<<(unsigned)((n + 255) / 256), 256, 0, ctx->stream>>>(dptr, n, dout + (all ? n * (size_t)ctx->comm_rank : 0));
+    VgBuf dptr(ctx), dout_buf(ctx), dsum(ctx);
+    VG_TRY(dptr.upload(ptrs.data(), n));
+    VG_TRY(dout_buf.alloc(n * 4 * G));
+    uint32_t* dout = dout_buf.as<uint32_t>();
+    gather_words_kernel<<<(unsigned)((n + 255) / 256), 256, 0, ctx->stream>>>(dptr.as<const uint32_t*>(), n, dout + (all ? n * (size_t)ctx->comm_rank : 0));
     VG_LAUNCH_CHECK(ctx);
     const uint32_t* res = dout;
     if (all) {
         VG_TRY(vg_comm_allgather_inplace(ctx, dout, n));
-        VG_TRY(vg_alloc(ctx, (void**)&dsum, n * 4));
-        sum_ranks_kernel<<<(unsigned)((n + 255) / 256), 256, 0, ctx->stream>>>(dout, (uint32_t)G, n, dsum);
+        VG_TRY(dsum.alloc(n * 4));
+        sum_ranks_kernel<<<(unsigned)((n + 255) / 256), 256, 0, ctx->stream>>>(dout, (uint32_t)G, n, dsum.as<uint32_t>());
         VG_LAUNCH_CHECK(ctx);
-        res = dsum;
+        res = dsum.as<uint32_t>();
     }
     VG_CUDA(ctx, cudaMemcpyAsync(out->data(), res, n * 4, cudaMemcpyDeviceToHost, ctx->stream));
     VG_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
-    vg_free(ctx, dptr); vg_free(ctx, dout); vg_free(ctx, dsum);
     return 0;
 }

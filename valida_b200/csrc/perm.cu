@@ -198,16 +198,15 @@ __global__ void __launch_bounds__(256) scan_add_rank_offset_kernel(uint32_t* __r
 // Inclusive prefix sum (mod p) of `ncols` columns of length n, in place.
 int32_t vg_prefix_sum_columns(vgpu_ctx* ctx, uint32_t* data, uint64_t cs, uint64_t n, uint32_t ncols) {
     uint64_t chunks = (n + SCAN_CHUNK - 1) / SCAN_CHUNK;
-    uint32_t* sums = nullptr;
-    if (chunks > 1) VG_TRY(vg_alloc(ctx, (void**)&sums, chunks * ncols * 4));
-    scan_chunks_kernel<<<dim3((unsigned)chunks, ncols), SCAN_THREADS, 0, ctx->stream>>>(data, cs, n, sums, chunks);
+    VgBuf sums(ctx);
+    if (chunks > 1) VG_TRY(sums.alloc(chunks * ncols * 4));
+    scan_chunks_kernel<<<dim3((unsigned)chunks, ncols), SCAN_THREADS, 0, ctx->stream>>>(data, cs, n, sums.as<uint32_t>(), chunks);
     VG_LAUNCH_CHECK(ctx);
     if (chunks > 1) {
-        scan_small_kernel<<<dim3(1, ncols), 1024, 0, ctx->stream>>>(sums, chunks, chunks);
+        scan_small_kernel<<<dim3(1, ncols), 1024, 0, ctx->stream>>>(sums.as<uint32_t>(), chunks, chunks);
         VG_LAUNCH_CHECK(ctx);
-        scan_add_offsets_kernel<<<dim3((unsigned)((n + 255) / 256), ncols), 256, 0, ctx->stream>>>(data, cs, n, sums, chunks);
+        scan_add_offsets_kernel<<<dim3((unsigned)((n + 255) / 256), ncols), 256, 0, ctx->stream>>>(data, cs, n, sums.as<uint32_t>(), chunks);
         VG_LAUNCH_CHECK(ctx);
-        vg_free(ctx, sums);
     }
     return 0;
 }
@@ -243,28 +242,28 @@ int32_t vg_perm_trace_enqueue(vgpu_ctx* ctx, const vgpu_chip_desc* chip, const v
     if (!split && main->dist != VG_FULL) VG_FAIL(ctx, "perm_trace: the trace is a shard but too short to be split");
     const uint64_t h = run.count, row0 = run.begin;          // rows swept here
     uint32_t k = chip->n_interactions;
-    vgpu_dmat* perm = nullptr;
+    VgMat perm;
     VG_TRY(vg_dmat_alloc_run(ctx, main->gh, 5 * (k + 1), split, false, &perm));
-    struct Undo { vgpu_dmat* m; ~Undo() { vgpu_dmat_free(m); } } undo{perm};       // released on every failing exit below
     // first swept row of a matrix: a shard starts there, a whole trace is entered at row0
     auto rows_of = [&](const vgpu_dmat* m) { return m->d + (m->dist == VG_ROWS ? 0 : row0); };
     const uint32_t* md = rows_of(main);
     const uint32_t* pd = prep_or_null ? rows_of(prep_or_null) : nullptr;
     uint64_t pcs = prep_or_null ? prep_or_null->col_stride : 0;
     unsigned blocks = (unsigned)((h + 255) / 256);
-    auto ks = std::make_unique<KScope>(ctx, KC_PERM, 4.0 * (double)h * (chip->width + 5.0 * (k + 1)));
-    if (k) {
-        perm_denominators_kernel<<<blocks, 256, 0, ctx->stream>>>(dchip, md, main->col_stride, pd, pcs, h, perm->d, perm->col_stride);
-        VG_LAUNCH_CHECK(ctx);
-        VG_TRY(vg_ext_batch_inverse(ctx, perm->d, perm->col_stride, h, k));
-    }
-    perm_terms_kernel<<<blocks, 256, 0, ctx->stream>>>(dchip, md, main->col_stride, pd, pcs, h, perm->d, perm->col_stride);
-    VG_LAUNCH_CHECK(ctx);
     uint32_t* phi = perm->d + (uint64_t)(5 * k) * perm->col_stride;
-    VG_TRY(vg_prefix_sum_columns(ctx, phi, perm->col_stride, h, 5));
-    perm_totals_kernel<<<1, 32, 0, ctx->stream>>>(phi, perm->col_stride, h, d_totals + (split ? 5 * ctx->comm_rank : 0));
-    VG_LAUNCH_CHECK(ctx);
-    ks.reset();
+    {
+        KScope ks(ctx, KC_PERM, 4.0 * (double)h * (chip->width + 5.0 * (k + 1)));
+        if (k) {
+            perm_denominators_kernel<<<blocks, 256, 0, ctx->stream>>>(dchip, md, main->col_stride, pd, pcs, h, perm->d, perm->col_stride);
+            VG_LAUNCH_CHECK(ctx);
+            VG_TRY(vg_ext_batch_inverse(ctx, perm->d, perm->col_stride, h, k));
+        }
+        perm_terms_kernel<<<blocks, 256, 0, ctx->stream>>>(dchip, md, main->col_stride, pd, pcs, h, perm->d, perm->col_stride);
+        VG_LAUNCH_CHECK(ctx);
+        VG_TRY(vg_prefix_sum_columns(ctx, phi, perm->col_stride, h, 5));
+        perm_totals_kernel<<<1, 32, 0, ctx->stream>>>(phi, perm->col_stride, h, d_totals + (split ? 5 * ctx->comm_rank : 0));
+        VG_LAUNCH_CHECK(ctx);
+    }
     if (split) {
         VG_TRY(vg_comm_allgather_inplace(ctx, d_totals, 5));
         KScope ks2(ctx, KC_PERM, 0.0);
@@ -272,8 +271,7 @@ int32_t vg_perm_trace_enqueue(vgpu_ctx* ctx, const vgpu_chip_desc* chip, const v
         VG_LAUNCH_CHECK(ctx);
     }
     *n_totals = split ? (uint32_t)ctx->comm_size : 1;
-    *out_perm = perm;
-    undo.m = nullptr;
+    *out_perm = perm.release();
     return 0;
 }
 uint32_t vg_perm_totals_ranks(const vgpu_ctx* ctx) { return vg_sharded(ctx) ? (uint32_t)ctx->comm_size : 1; }
@@ -281,22 +279,21 @@ uint32_t vg_perm_totals_ranks(const vgpu_ctx* ctx) { return vg_sharded(ctx) ? (u
 extern "C" int32_t vgpu_perm_trace(vgpu_ctx* ctx, const vgpu_chip_desc* chip, const vgpu_dmat* main, const vgpu_dmat* prep_or_null,
                                    const uint32_t challenges[15], vgpu_dmat** out_perm, uint32_t cumulative_sum_out[5]) {
     VG_TRY(vg_enter(ctx));
-    uint32_t* d_tot = nullptr;
+    VgBuf d_tot(ctx);
     const uint32_t slots = vg_perm_totals_ranks(ctx);
-    VG_TRY(vg_alloc(ctx, (void**)&d_tot, slots * 5 * 4));
+    VG_TRY(d_tot.alloc(slots * 5 * 4));
     uint32_t nt = 0;
-    int32_t rc = vg_perm_trace_enqueue(ctx, chip, main, prep_or_null, challenges, out_perm, d_tot, &nt);
-    if (rc == 0 && cumulative_sum_out) {
+    VG_TRY(vg_perm_trace_enqueue(ctx, chip, main, prep_or_null, challenges, out_perm, d_tot.as<uint32_t>(), &nt));
+    if (cumulative_sum_out) {
         uint32_t tot[16 * 5];
-        cudaError_t e = cudaMemcpyAsync(tot, d_tot, nt * 5 * 4, cudaMemcpyDeviceToHost, ctx->stream);
+        cudaError_t e = cudaMemcpyAsync(tot, d_tot.p, nt * 5 * 4, cudaMemcpyDeviceToHost, ctx->stream);
         if (e == cudaSuccess) e = cudaStreamSynchronize(ctx->stream);
-        if (e != cudaSuccess) { vg_free(ctx, d_tot); VG_FAIL(ctx, "perm_trace: reading the cumulative sum failed: %s", cudaGetErrorString(e)); }
+        if (e != cudaSuccess) VG_FAIL(ctx, "perm_trace: reading the cumulative sum failed: %s", cudaGetErrorString(e));
         for (int l = 0; l < 5; l++) {
             uint32_t a = 0;
             for (uint32_t p = 0; p < nt; p++) a = bb::add(a, tot[p * 5 + l]);
             cumulative_sum_out[l] = bb::from_monty(a);
         }
     }
-    vg_free(ctx, d_tot);
-    return rc;
+    return 0;
 }

@@ -220,13 +220,13 @@ extern "C" int32_t vgpu_quotient(vgpu_ctx* ctx, const vgpu_chip_desc* chip, uint
         if (!m->symm) return nullptr;
         return vg_peer_ptr(ctx, m->d, next_rank) - (uint64_t)next_rank * m->h;
     };
-    vgpu_dmat* out = nullptr;
+    VgMat out;
     VG_TRY(vg_dmat_alloc_run(ctx, h, 10, split, false, &out));
     out->bitrev_rows = true;
     p.main = base_of(main_lde); p.main_n = next_of(main_lde); p.mcs = main_lde->col_stride;
     p.prep = prep_lde ? base_of(prep_lde) : nullptr; p.prep_n = prep_lde ? next_of(prep_lde) : nullptr; p.pcs = prep_lde ? prep_lde->col_stride : 0;
     p.perm = base_of(perm_lde); p.perm_n = next_of(perm_lde); p.qcs = perm_lde->col_stride;
-    if (!p.main_n || !p.perm_n || (prep_lde && !p.prep_n)) { vgpu_dmat_free(out); VG_FAIL(ctx, "quotient: a row shard read by a peer must live in the symmetric heap"); }
+    if (!p.main_n || !p.perm_n || (prep_lde && !p.prep_n)) VG_FAIL(ctx, "quotient: a row shard read by a peer must live in the symmetric heap");
     p.out = out->d - p.row_begin / 2; p.ocs = out->col_stride;
     p.log_h = log_degree;
     p.s = bb::to_monty(bb::GEN_CANON);
@@ -242,21 +242,20 @@ extern "C" int32_t vgpu_quotient(vgpu_ctx* ctx, const vgpu_chip_desc* chip, uint
     for (int i = 0; i < 5; i++) p.cumsum.c[i] = bb::to_monty(cumulative_sum[i] % bb::P);
     p.root_lo = ctx->root_table.lo; p.root_hi = ctx->root_table.hi;
     const uint64_t pb = p.row_begin / 2, pc = (p.row_end - p.row_begin) / 2;     // pairs swept here
-    uint32_t* selinv = nullptr;
-    { int32_t rc = vg_alloc(ctx, (void**)&selinv, pc * 4); if (rc) { vgpu_dmat_free(out); return rc; } }
-    p.selinv = selinv - pb;
-    KScope* ks = new KScope(ctx, KC_QUOTIENT, 4.0 * (double)(p.row_end - p.row_begin) * (main_lde->gw + perm_lde->gw + (prep_lde ? prep_lde->gw : 0)) + 20.0 * (double)(p.row_end - p.row_begin));
+    VgBuf selinv(ctx);
+    VG_TRY(selinv.alloc(pc * 4));
+    p.selinv = selinv.as<uint32_t>() - pb;
     {
+        KScope ks(ctx, KC_QUOTIENT, 4.0 * (double)(p.row_end - p.row_begin) * (main_lde->gw + perm_lde->gw + (prep_lde ? prep_lde->gw : 0)) + 20.0 * (double)(p.row_end - p.row_begin));
         const uint64_t stride = (pc + SEL_BATCH - 1) / SEL_BATCH;
-        selector_inverse_kernel<<<(unsigned)((stride + 255) / 256), 256, 0, ctx->stream>>>(selinv - pb, pb, pc, log_degree, p.s, p.glast, p.root_lo, p.root_hi);
+        selector_inverse_kernel<<<(unsigned)((stride + 255) / 256), 256, 0, ctx->stream>>>(selinv.as<uint32_t>() - pb, pb, pc, log_degree, p.s, p.glast, p.root_lo, p.root_hi);
         ctx->launches++;
+        air::with_chip(chip->chip_id, [&](auto c) {
+            quotient_kernel<decltype(c)::value><<<(unsigned)((p.row_end - p.row_begin + 127) / 128), 128, 0, ctx->stream>>>(p);
+        });
     }
-    air::with_chip(chip->chip_id, [&](auto c) {
-        quotient_kernel<decltype(c)::value><<<(unsigned)((p.row_end - p.row_begin + 127) / 128), 128, 0, ctx->stream>>>(p);
-    });
-    delete ks;
-    vg_free(ctx, selinv);
+    selinv.reset();
     VG_LAUNCH_CHECK(ctx);
-    *out_chunks = out;
+    *out_chunks = out.release();
     return 0;
 }

@@ -58,12 +58,9 @@ static int32_t transpose_in(vgpu_ctx* ctx, const uint32_t* stage, uint64_t h, ui
 
 int32_t vg_upload_rowmajor(vgpu_ctx* ctx, const uint32_t* host, uint64_t h, uint64_t w, int32_t repr, vgpu_dmat* dst) {
     if (h == 0 || w == 0) return 0;
-    uint32_t* stage = nullptr;
-    VG_TRY(vg_alloc(ctx, (void**)&stage, h * w * 4));
-    VG_CUDA(ctx, cudaMemcpyAsync(stage, host, h * w * 4, cudaMemcpyHostToDevice, ctx->stream));
-    int32_t rc = transpose_in(ctx, stage, h, w, repr, dst);
-    vg_free(ctx, stage);
-    return rc;
+    VgBuf stage(ctx);
+    VG_TRY(stage.upload(host, h * w));
+    return transpose_in(ctx, stage.as<uint32_t>(), h, w, repr, dst);
 }
 
 // ---- uploads out of PAGEABLE caller memory (a Rust Vec, a numpy array) ------------------------------------------------------
@@ -230,17 +227,16 @@ int32_t vg_dmat_materialize(vgpu_ctx* ctx, const vgpu_dmat* cm) {
 int32_t vg_download_rowmajor(vgpu_ctx* ctx, const vgpu_dmat* src, int32_t repr, uint32_t* host) {
     uint64_t h = src->h, w = src->w;
     if (h == 0 || w == 0) return 0;
-    uint32_t* stage = nullptr;
-    VG_TRY(vg_alloc(ctx, (void**)&stage, h * w * 4));
+    VgBuf stage(ctx);
+    VG_TRY(stage.alloc(h * w * 4));
     for (uint64_t c0 = 0; c0 < w; c0 += TW) {
         uint32_t wc = (uint32_t)(w - c0 < TW ? w - c0 : TW);
         KScope ks(ctx, KC_TRANSPOSE, 8.0 * (double)h * wc);
-        cm_to_rm_kernel<<<(unsigned)((h + TR - 1) / TR), 256, 0, ctx->stream>>>(src->d, src->col_stride, h, w, stage, repr == VGPU_REPR_CANONICAL, c0, wc);
+        cm_to_rm_kernel<<<(unsigned)((h + TR - 1) / TR), 256, 0, ctx->stream>>>(src->d, src->col_stride, h, w, stage.as<uint32_t>(), repr == VGPU_REPR_CANONICAL, c0, wc);
         VG_LAUNCH_CHECK(ctx);
     }
-    VG_CUDA(ctx, cudaMemcpyAsync(host, stage, h * w * 4, cudaMemcpyDeviceToHost, ctx->stream));
+    VG_CUDA(ctx, cudaMemcpyAsync(host, stage.p, h * w * 4, cudaMemcpyDeviceToHost, ctx->stream));
     VG_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
-    vg_free(ctx, stage);
     return 0;
 }
 
@@ -334,9 +330,9 @@ int32_t vg_import_strided(vgpu_ctx* ctx, const uint32_t* src, uint64_t h, uint64
                           unsigned long long* bad_key) {
     *bad_key = ~0ull;
     if (h == 0 || w == 0) return 0;
-    unsigned long long* d_bad = nullptr;
-    VG_TRY(vg_alloc(ctx, (void**)&d_bad, sizeof *d_bad));
-    struct Free { vgpu_ctx* c; void* p; ~Free() { vg_free(c, p); } } fr{ctx, d_bad};
+    VgBuf bad(ctx);
+    VG_TRY(bad.alloc(sizeof(unsigned long long)));
+    unsigned long long* d_bad = bad.as<unsigned long long>();
     VG_CUDA(ctx, cudaMemsetAsync(d_bad, 0xff, sizeof *d_bad, ctx->stream));
     const IoTiles g = io_tiles(h, w);
     const uint64_t tiles = g.row_tiles * ((w + TW - 1) / TW);

@@ -278,21 +278,13 @@ __global__ void __launch_bounds__(SORT_THREADS) sort_scatter_kernel(const uint32
     }
 }
 
-struct DevBuf { vgpu_ctx* ctx; void* p = nullptr; explicit DevBuf(vgpu_ctx* c) : ctx(c) {} ~DevBuf() { vg_free(ctx, p); }
-                template <class T> T* as() const { return (T*)p; } };
-template <class T> int32_t upload(vgpu_ctx* ctx, DevBuf& b, const T* host, size_t count) {
-    VG_TRY(vg_alloc(ctx, &b.p, std::max<size_t>(count, 1) * sizeof(T)));
-    if (count) VG_CUDA(ctx, cudaMemcpyAsync(b.p, host, count * sizeof(T), cudaMemcpyHostToDevice, ctx->stream));
-    return 0;
-}
-
 uint64_t next_pow2(uint64_t n) { uint64_t p = 1; while (p < n) p <<= 1; return p; }
 
 // sorted position -> log index; null result = the log is already in address order (every address identical)
-int32_t sort_log_by_addr(vgpu_ctx* ctx, const VgMemOp* d_mem, uint64_t n, DevBuf& out_idx) {
+int32_t sort_log_by_addr(vgpu_ctx* ctx, const VgMemOp* d_mem, uint64_t n, VgBuf& out_idx) {
     if (n < 2) return 0;
-    DevBuf bits(ctx), k0(ctx), k1(ctx), i0(ctx), i1(ctx), hist(ctx);
-    VG_TRY(vg_alloc(ctx, &bits.p, 8));
+    VgBuf bits(ctx), k0(ctx), k1(ctx), i0(ctx), i1(ctx), hist(ctx);
+    VG_TRY(bits.alloc(8));
     const uint32_t init[2] = {0u, 0xffffffffu};
     VG_CUDA(ctx, cudaMemcpyAsync(bits.p, init, 8, cudaMemcpyHostToDevice, ctx->stream));
     addr_bits_kernel<<<2 * ctx->sm_count, 256, 0, ctx->stream>>>(d_mem, n, bits.as<uint32_t>());
@@ -303,9 +295,9 @@ int32_t sort_log_by_addr(vgpu_ctx* ctx, const VgMemOp* d_mem, uint64_t n, DevBuf
     const uint32_t varying = oa[0] ^ oa[1];
     if (!varying) return 0;
     const uint32_t nblocks = (uint32_t)((n + SORT_TILE - 1) / SORT_TILE);
-    VG_TRY(vg_alloc(ctx, &k0.p, n * 4)); VG_TRY(vg_alloc(ctx, &k1.p, n * 4));
-    VG_TRY(vg_alloc(ctx, &i0.p, n * 4)); VG_TRY(vg_alloc(ctx, &i1.p, n * 4));
-    VG_TRY(vg_alloc(ctx, &hist.p, (size_t)256 * nblocks * 4));
+    VG_TRY(k0.alloc(n * 4)); VG_TRY(k1.alloc(n * 4));
+    VG_TRY(i0.alloc(n * 4)); VG_TRY(i1.alloc(n * 4));
+    VG_TRY(hist.alloc((size_t)256 * nblocks * 4));
     sort_init_kernel<<<(unsigned)((n + 255) / 256), 256, 0, ctx->stream>>>(d_mem, n, k0.as<uint32_t>(), i0.as<uint32_t>());
     VG_LAUNCH_CHECK(ctx);
     uint32_t *ka = k0.as<uint32_t>(), *kb = k1.as<uint32_t>(), *ia = i0.as<uint32_t>(), *ib = i1.as<uint32_t>();
@@ -320,7 +312,7 @@ int32_t sort_log_by_addr(vgpu_ctx* ctx, const VgMemOp* d_mem, uint64_t n, DevBuf
         std::swap(ka, kb); std::swap(ia, ib);
     }
     // hand the buffer holding the final order to the caller
-    if (ia == i0.as<uint32_t>()) { out_idx.p = i0.p; i0.p = nullptr; } else { out_idx.p = i1.p; i1.p = nullptr; }
+    out_idx = std::move(ia == i0.as<uint32_t>() ? i0 : i1);
     return 0;
 }
 
@@ -336,86 +328,89 @@ int32_t vgpu_witness_device(vgpu_ctx* ctx, const vgpu_vmlog* log, vgpu_dmat* mai
     const VgVmLogs& L = *vg_vmlog_view(log);
     for (int i = 0; i < VGPU_NUM_CHIPS; i++) main_out[i] = nullptr;
     prep_out[0] = prep_out[1] = nullptr;
-    struct Undo { vgpu_dmat** m; vgpu_dmat** p; bool armed = true; ~Undo() { if (!armed) return; for (int i = 0; i < VGPU_NUM_CHIPS; i++) { vgpu_dmat_free(m[i]); m[i] = nullptr; } for (int i = 0; i < 2; i++) { vgpu_dmat_free(p[i]); p[i] = nullptr; } } } undo{main_out, prep_out};
     if (!L.n_cpu) VG_FAIL(ctx, "witness: the run has no cycles");
+    VgMat main[VGPU_NUM_CHIPS], prep[2];                   // handed out only once every trace is built
     // a tall chip's trace: whole, or this rank's run of rows (split proof)
-    auto alloc_rows = [&](uint64_t h, uint64_t w, vgpu_dmat** out, RowRange* rr) -> int32_t {
+    auto alloc_rows = [&](uint64_t h, uint64_t w, VgMat* out, RowRange* rr) -> int32_t {
         VG_TRY(vg_dmat_alloc_run(ctx, h, w, vg_trace_run(ctx, h).split, false, out));
         rr->row0 = (*out)->row0; rr->rows = (*out)->h; rr->out = (*out)->d; rr->cs = (*out)->col_stride;
         return 0;
     };
-    auto small = [&](const std::vector<uint32_t>& rows, uint64_t h, uint64_t w, vgpu_dmat** out) -> int32_t {   // host-built short chip
+    auto small = [&](const std::vector<uint32_t>& rows, uint64_t h, uint64_t w, VgMat* out) -> int32_t {   // host-built short chip
         vgpu_matrix hm{rows.data(), h, w};
-        return vgpu_dmat_upload(ctx, &hm, VGPU_REPR_CANONICAL, out);
+        vgpu_dmat* m = nullptr;
+        VG_TRY(vgpu_dmat_upload(ctx, &hm, VGPU_REPR_CANONICAL, &m));
+        out->reset(m);
+        return 0;
     };
-    DevBuf d_prog(ctx), d_cpu(ctx), d_mem(ctx), d_adds(ctx), d_subs(ctx), d_lts(ctx), d_bits(ctx), d_sa(ctx), d_sv(ctx), d_order(ctx);
-    VG_TRY(upload(ctx, d_prog, L.program, 6 * L.n_instr));
-    VG_TRY(upload(ctx, d_cpu, L.cpu, L.n_cpu));
-    VG_TRY(upload(ctx, d_mem, L.mem, L.n_mem));
-    VG_TRY(upload(ctx, d_adds, L.adds, L.n_adds));
-    VG_TRY(upload(ctx, d_subs, L.subs, L.n_subs));
-    VG_TRY(upload(ctx, d_lts, L.lts, L.n_lts));
-    VG_TRY(upload(ctx, d_bits, L.bits, L.n_bits));
-    VG_TRY(upload(ctx, d_sa, L.static_addr, L.n_static));
-    VG_TRY(upload(ctx, d_sv, L.static_value, L.n_static));
+    VgBuf d_prog(ctx), d_cpu(ctx), d_mem(ctx), d_adds(ctx), d_subs(ctx), d_lts(ctx), d_bits(ctx), d_sa(ctx), d_sv(ctx), d_order(ctx);
+    VG_TRY(d_prog.upload(L.program, 6 * L.n_instr));
+    VG_TRY(d_cpu.upload(L.cpu, L.n_cpu));
+    VG_TRY(d_mem.upload(L.mem, L.n_mem));
+    VG_TRY(d_adds.upload(L.adds, L.n_adds));
+    VG_TRY(d_subs.upload(L.subs, L.n_subs));
+    VG_TRY(d_lts.upload(L.lts, L.n_lts));
+    VG_TRY(d_bits.upload(L.bits, L.n_bits));
+    VG_TRY(d_sa.upload(L.static_addr, L.n_static));
+    VG_TRY(d_sv.upload(L.static_value, L.n_static));
     RowRange rr{};
     {   // 0 cpu
         const uint64_t h = next_pow2(L.n_cpu);
-        VG_TRY(alloc_rows(h, 51, &main_out[0], &rr));
+        VG_TRY(alloc_rows(h, 51, &main[0], &rr));
         cpu_rows_kernel<<<(unsigned)((rr.rows + 127) / 128), 128, 0, ctx->stream>>>(d_cpu.as<VgCpuRec>(), d_mem.as<VgMemOp>(), d_prog.as<int32_t>(), L.n_cpu, L.n_mem, rr);
         VG_LAUNCH_CHECK(ctx);
     }
     {   // 2 memory: sort by address (stable), then the rows
         VG_TRY(sort_log_by_addr(ctx, d_mem.as<VgMemOp>(), L.n_mem, d_order));
         const uint64_t h = next_pow2(L.n_static + L.n_mem);
-        VG_TRY(alloc_rows(h, 14, &main_out[2], &rr));
+        VG_TRY(alloc_rows(h, 14, &main[2], &rr));
         mem_rows_kernel<<<(unsigned)((rr.rows + 255) / 256), 256, 0, ctx->stream>>>(d_mem.as<VgMemOp>(), d_order.as<uint32_t>(), L.n_mem, d_sa.as<uint32_t>(), d_sv.as<uint32_t>(), L.n_static, rr);
         VG_LAUNCH_CHECK(ctx);
     }
     for (int which = 0; which < 2; which++) {   // 3 add, 4 sub
         const uint64_t n = which ? L.n_subs : L.n_adds, h = next_pow2(n);
-        VG_TRY(alloc_rows(h, 16, &main_out[3 + which], &rr));
+        VG_TRY(alloc_rows(h, 16, &main[3 + which], &rr));
         addsub_rows_kernel<<<(unsigned)((rr.rows + 255) / 256), 256, 0, ctx->stream>>>(which ? d_subs.as<VgAluRec>() : d_adds.as<VgAluRec>(), n, which == 0, rr);
         VG_LAUNCH_CHECK(ctx);
     }
     {   // 8 lt
         const uint64_t h = next_pow2(L.n_lts);
-        VG_TRY(alloc_rows(h, 45, &main_out[8], &rr));
+        VG_TRY(alloc_rows(h, 45, &main[8], &rr));
         lt_rows_kernel<<<(unsigned)((rr.rows + 127) / 128), 128, 0, ctx->stream>>>(d_lts.as<VgAluOpRec>(), L.n_lts, rr);
         VG_LAUNCH_CHECK(ctx);
     }
     {   // 10 bitwise
         const uint64_t h = next_pow2(L.n_bits);
-        VG_TRY(alloc_rows(h, 79, &main_out[10], &rr));
+        VG_TRY(alloc_rows(h, 79, &main[10], &rr));
         bitwise_rows_kernel<<<(unsigned)((rr.rows + 127) / 128), 128, 0, ctx->stream>>>(d_bits.as<VgAluOpRec>(), L.n_bits, rr);
         VG_LAUNCH_CHECK(ctx);
     }
     // ---- the short chips, on the host ----
     {   // 1 program: 1 main column (execution counts) + 7 preprocessed (program/src/lib.rs:38-81, program/src/stark.rs:22-40)
         const uint64_t h = next_pow2(L.n_instr);
-        std::vector<uint32_t> counts(h, 0), prep(h * 7, 0);
+        std::vector<uint32_t> counts(h, 0), prep_rows(h * 7, 0);
         for (size_t i = 0; i < L.n_instr; i++) counts[i] = L.prog_counts[i];
         for (uint64_t i = 0; i < h; i++) {
-            prep[i * 7] = (uint32_t)i;
+            prep_rows[i * 7] = (uint32_t)i;
             if (i < L.n_instr) {
-                prep[i * 7 + 1] = (uint32_t)L.program[6 * i];
-                for (int k = 0; k < 5; k++) { const int32_t x = L.program[6 * i + 1 + k]; prep[i * 7 + 2 + k] = x < 0 ? (bb::P - (uint32_t)(-(int64_t)x) % bb::P) % bb::P : (uint32_t)x % bb::P; }
+                prep_rows[i * 7 + 1] = (uint32_t)L.program[6 * i];
+                for (int k = 0; k < 5; k++) { const int32_t x = L.program[6 * i + 1 + k]; prep_rows[i * 7 + 2 + k] = x < 0 ? (bb::P - (uint32_t)(-(int64_t)x) % bb::P) % bb::P : (uint32_t)x % bb::P; }
             }
         }
-        VG_TRY(small(counts, h, 1, &main_out[1]));
-        VG_TRY(small(prep, h, 7, &prep_out[0]));
+        VG_TRY(small(counts, h, 1, &main[1]));
+        VG_TRY(small(prep_rows, h, 7, &prep[0]));
     }
     {   // 5 mul: 2^10 counter rows (alu_u32/src/mul/mod.rs:38-64)
         std::vector<uint32_t> m(1024 * 18, 0);
         for (uint32_t i = 0; i < 1024; i++) m[i * 18 + 17] = i + 1;
-        VG_TRY(small(m, 1024, 18, &main_out[5]));
+        VG_TRY(small(m, 1024, 18, &main[5]));
     }
     {   // the chips without rows in the provable instruction subset: one zero row each
         const int ids[5] = {6, 7, 9, 11, 13}; const uint64_t ws[5] = {14, 28, 14, 7, 6};
         for (int k = 0; k < 5; k++) {
             if (ids[k] == 13 && L.n_static) continue;
             std::vector<uint32_t> z(ws[k], 0);
-            VG_TRY(small(z, 1, ws[k], &main_out[ids[k]]));
+            VG_TRY(small(z, 1, ws[k], &main[ids[k]]));
         }
     }
     if (L.n_static) {   // 13 static data: (addr, value[4], is_real), ascending address (static_data/src/lib.rs:60-96)
@@ -426,16 +421,17 @@ int32_t vgpu_witness_device(vgpu_ctx* ctx, const vgpu_vmlog* log, vgpu_dmat* mai
             const uint32_t v = L.static_value[i];
             row[0] = L.static_addr[i]; row[1] = v >> 24; row[2] = (v >> 16) & 0xff; row[3] = (v >> 8) & 0xff; row[4] = v & 0xff; row[5] = 1;
         }
-        VG_TRY(small(s, h, 6, &main_out[13]));
+        VG_TRY(small(s, h, 6, &main[13]));
     }
     {   // 12 range: (multiplicity, counter) + preprocessed counter (range/src/lib.rs:32-72)
         std::vector<uint32_t> r(512), p(256);
         for (uint32_t i = 0; i < 256; i++) { r[2 * i] = L.range_count[i]; r[2 * i + 1] = i; p[i] = i; }
-        VG_TRY(small(r, 256, 2, &main_out[12]));
-        VG_TRY(small(p, 256, 1, &prep_out[1]));
+        VG_TRY(small(r, 256, 2, &main[12]));
+        VG_TRY(small(p, 256, 1, &prep[1]));
     }
     VG_CUDA(ctx, cudaStreamSynchronize(ctx->stream));      // the logs are the caller's (pageable) memory: they may go once this returns
-    undo.armed = false;
+    for (int i = 0; i < VGPU_NUM_CHIPS; i++) main_out[i] = main[i].release();
+    for (int i = 0; i < 2; i++) prep_out[i] = prep[i].release();
     return 0;
 }
 
