@@ -5,13 +5,13 @@
 // host, input to the GPU path"); it follows
 //   run loop + STOP padding        basic/src/lib.rs:127-145, 1063-1188
 //   instruction semantics          cpu/src/lib.rs:437-923, alu_u32/src/add/mod.rs:138-169, sub/mod.rs:126-166
-//   CPU rows                       cpu/src/lib.rs:79-97, 163-373
-//   memory rows                    memory/src/lib.rs:85-136, 143-194, 237-263
-//   add/sub rows                   alu_u32/src/add/mod.rs:38-129, alu_u32/src/sub/mod.rs
 //   mul floor (2^10 counter rows)  alu_u32/src/mul/mod.rs:38-64
 //   range / program rows           range/src/lib.rs:32-72, program/src/lib.rs:38-81, program/src/stark.rs:22-40
 //   static data                    static_data/src/lib.rs:26-79 (chip rows), memory/src/lib.rs:132-135, 163-169, 265-283
 //                                  (write_static, the static rows that open the memory trace); basic/src/lib.rs:131
+// The builders read the interpreter's logs through VgVmLogs (vmlog.h), the view the device builder (witness.cu) reads too.  The
+// rows of the tall chips (cpu, memory, add, sub, lt, bitwise) come from the row functions of chip_rows.cuh, which the device
+// builder calls as well; the short chips come from vg_short_chip_traces, whose matrices the device builder uploads.
 // Output: 14 row-major matrices of canonical BabyBear words in chip order
 // (cpu, program, mem, add, sub, mul, div, shift, lt, com, bitwise, output, range, static_data)
 // plus the two preprocessed traces.
@@ -27,18 +27,14 @@
 #include <cstdio>
 #include <omp.h>
 #include "../../../include/valida_b200.h"
-#include "vmlog.h"
+#include "../chip_rows.cuh"
 
 namespace {
 
-constexpr uint32_t P = 2013265921u;
+using bb::P;
 inline uint32_t fmul(uint32_t a, uint32_t b) { return (uint32_t)(((uint64_t)a * b) % P); }
 inline uint32_t fpow(uint32_t a, uint32_t e) { uint32_t r = 1; while (e) { if (e & 1) r = fmul(r, a); a = fmul(a, a); e >>= 1; } return r; }
-inline uint32_t from_i32(int32_t x) { return x < 0 ? (P - (uint32_t)(-(int64_t)x) % P) % P : (uint32_t)x % P; }
-inline size_t next_pow2(size_t n) { size_t p = 1; while (p < n) p <<= 1; return p; }
 
-enum : uint32_t { OP_LOAD32 = 1, OP_STORE32 = 2, OP_JAL = 3, OP_JALV = 4, OP_BEQ = 5, OP_BNE = 6, OP_IMM32 = 7, OP_STOP = 8, OP_LOADFP = 10,
-                  OP_ADD32 = 100, OP_SUB32 = 101, OP_LT32 = 104, OP_AND32 = 107, OP_OR32 = 108, OP_XOR32 = 109, OP_LTE32 = 115, OP_SLT32 = 117, OP_SLE32 = 118 };
 using CpuOp = uint8_t;
 enum : uint8_t { K_STORE32 = VG_K_STORE32, K_LOAD32 = VG_K_LOAD32, K_JAL = VG_K_JAL, K_JALV = VG_K_JALV, K_BEQ = VG_K_BEQ, K_BNE = VG_K_BNE, K_IMM32 = VG_K_IMM32,
                  K_BUS = VG_K_BUS, K_STOP = VG_K_STOP, K_LOADFP = VG_K_LOADFP, K_BUS_LEFT_IMM = VG_K_BUS_LEFT_IMM };
@@ -136,7 +132,7 @@ struct Vm {
     const int32_t* prog; size_t n_instr;
     uint32_t pc = 0, fp = 0, clock = 0;
     CellMap cells;
-    std::vector<std::pair<uint32_t, uint32_t>> static_cells;   // (addr, value), ascending addr (the reference keeps a BTreeMap)
+    std::vector<uint32_t> static_addr, static_value;           // ascending addr (the reference keeps a BTreeMap)
     PodVec<MemOp> mem_ops;
     PodVec<CpuRec> cpu;
     PodVec<AluRec> adds, subs;
@@ -236,6 +232,20 @@ struct Vm {
         prog_counts[pc0]++;
         return opcode == OP_STOP ? 1 : 0;
     }
+    // the logs of the run as the view both witness builders read
+    VgVmLogs logs() const {
+        VgVmLogs v;
+        v.program = prog; v.n_instr = n_instr;
+        v.cpu = cpu.data(); v.n_cpu = cpu.size();
+        v.mem = mem_ops.data(); v.n_mem = mem_ops.size();
+        v.adds = adds.data(); v.n_adds = adds.size();
+        v.subs = subs.data(); v.n_subs = subs.size();
+        v.lts = lts.data(); v.n_lts = lts.size();
+        v.bits = bits.data(); v.n_bits = bits.size();
+        v.prog_counts = prog_counts.data(); v.range_count = range_count;
+        v.static_addr = static_addr.data(); v.static_value = static_value.data(); v.n_static = static_addr.size();
+        return v;
+    }
 };
 
 struct Traces {
@@ -246,60 +256,18 @@ struct Traces {
     CellMap cells;
 };
 
-inline void word_be(uint32_t v, uint32_t* out) { out[0] = v >> 24; out[1] = (v >> 16) & 0xff; out[2] = (v >> 8) & 0xff; out[3] = v & 0xff; }
-
-void build_cpu(const Vm& vm, Traces& t) {
-    constexpr size_t W = 51;
-    size_t n = vm.cpu.size(), h = next_pow2(n);
+void build_cpu(const VgVmLogs& L, Traces& t) {
+    constexpr size_t W = CPU_COLS;
+    const size_t n = L.n_cpu, h = next_pow2(n);       // n >= 1: a run ends with STOP
     Buf& v = t.store[0];
-    v.zeros(h * W);
-    // the memory operations of a cycle are contiguous in vm.mem_ops: [cpu[i].mem0, cpu[i + 1].mem0)
-    auto first_of = [&](size_t i) { return i < n ? (size_t)vm.cpu[i].mem0 : vm.mem_ops.size(); };
-    std::vector<uint32_t> diff(n, 0);
+    v.alloc(h * W);                                   // every row is written below: the n cycles, then the STOP padding
+    std::vector<uint32_t> diff(n);
 #pragma omp parallel for schedule(static)
     for (long i = 0; i < (long)n; i++) {
-        const CpuRec& r = vm.cpu[i];
-        uint32_t* row = &v[(size_t)i * W];
-        const int32_t* w = vm.prog + 6 * (size_t)r.instr;
-        row[0] = (uint32_t)i; row[1] = r.pc; row[2] = r.fp % P;      // from_canonical_u32 (cpu/src/lib.rs:171-172) reduces mod p
-        row[3] = (uint32_t)w[0];
-        for (int k = 0; k < 5; k++) row[4 + k] = from_i32(w[1 + k]);
-        bool left_imm = false;
-        switch (r.kind) {
-            case K_STORE32: row[16] = 1; break;
-            case K_LOAD32: row[13] = 1; break;
-            case K_JAL: row[20] = 1; break;
-            case K_JALV: row[21] = 1; break;
-            case K_BEQ: row[18] = 1; break;
-            case K_BNE: row[19] = 1; break;
-            case K_IMM32: row[22] = 1; break;
-            case K_BUS: row[9] = 1; break;
-            case K_STOP: row[24] = 1; break;
-            case K_LOADFP: row[25] = 1; break;
-            case K_BUS_LEFT_IMM: row[9] = 1; break;
-        }
-        if (r.has_imm && r.kind == K_BUS_LEFT_IMM) {  // set_left_imm_value (cpu/src/lib.rs:364-371)
-            row[12] = 1; left_imm = true;
-            word_be(r.imm, &row[29 + 3]);
-            row[5] = r.imm % P;
-        } else if (r.has_imm) {  // set_imm_value (cpu/src/lib.rs:355-362)
-            row[11] = 1;
-            word_be(r.imm, &row[36 + 3]);
-            row[6] = r.imm % P;
-        }
-        row[29 + 1] = 1; row[36 + 1] = 1; row[43 + 1] = 0;
-        bool first_read = true;
-        for (size_t k = first_of(i), ke = first_of(i + 1); k < ke; k++) {
-            const MemOp& m = vm.mem_ops[k];
-            uint32_t ch;
-            if (m.is_write) ch = 43;
-            else if (first_read && !left_imm) { ch = 29; first_read = false; }
-            else ch = 36;
-            row[ch] = 1; row[ch + 2] = m.addr % P; word_be(m.value, &row[ch + 3]);     // cpu/src/lib.rs:263-276
-        }
-        uint64_t dsum = 0;
-        for (int k = 0; k < 4; k++) { int64_t dd = (int64_t)row[32 + k] - (int64_t)row[39 + k]; dsum += (uint64_t)(dd * dd); }
-        diff[i] = (uint32_t)(dsum % P);
+        const CpuRec& r = L.cpu[i];
+        // the memory operations of a cycle are contiguous in the log: [cpu[i].mem0, cpu[i + 1].mem0)
+        const size_t k1 = (size_t)i + 1 < n ? L.cpu[i + 1].mem0 : L.n_mem;
+        diff[i] = cpu_row(&v[(size_t)i * W], i, r, L.program + 6 * (size_t)r.instr, L.mem + r.mem0, k1 - r.mem0);
     }
     // diff_inv through a table over the possible values (diff <= 4*255^2): mark, invert the marked entries, fill
     {
@@ -311,24 +279,10 @@ void build_cpu(const Vm& vm, Traces& t) {
 #pragma omp parallel for schedule(dynamic, 1024)
         for (long d = 1; d <= (long)DMAX; d++) if (seen[d]) invs[d] = fpow((uint32_t)d, P - 2);
 #pragma omp parallel for schedule(static)
-        for (long i = 0; i < (long)n; i++) {
-            uint32_t* row = &v[(size_t)i * W];
-            row[26] = diff[i];
-            if (diff[i]) { row[27] = invs[diff[i]]; row[28] = 1; }
-        }
+        for (long i = 0; i < (long)n; i++) if (diff[i]) v[(size_t)i * W + 27] = invs[diff[i]];
     }
-    // pad_to_power_of_two (cpu/src/lib.rs:318-353)
-    if (n) {
-        const uint32_t* last = &v[(n - 1) * W];
-        uint32_t pc = last[1], fp = last[2], clk = last[0];        // fp already reduced
 #pragma omp parallel for schedule(static)
-        for (long i = (long)n; i < (long)h; i++) {
-            uint32_t* row = &v[(size_t)i * W];
-            row[1] = pc; row[2] = fp; row[0] = clk + (uint32_t)(i - n) + 1;
-            row[24] = 1; row[3] = OP_STOP;
-            row[29 + 1] = 1; row[36 + 1] = 1;
-        }
-    }
+    for (long i = (long)n; i < (long)h; i++) cpu_pad_row(&v[(size_t)i * W], i, L.cpu[n - 1]);
     t.main[0] = {v.data(), h, W};
 }
 
@@ -336,9 +290,8 @@ void build_cpu(const Vm& vm, Traces& t) {
 // STABLE sort on the address alone gives the same order).  LSD radix, 11 bits per pass, passes whose digit is the same for
 // every key are skipped; per-thread histograms over contiguous chunks keep each pass stable.
 // Returns the sorted log (a fresh array, or `in` itself when no pass was needed); `hold` owns whatever was allocated.
-const MemOp* sort_by_addr(const PodVec<MemOp>& in, std::unique_ptr<MemOp[]> hold[2]) {
-    const size_t n = in.size();
-    if (n < 2) return in.data();
+const MemOp* sort_by_addr(const MemOp* in, size_t n, std::unique_ptr<MemOp[]> hold[2]) {
+    if (n < 2) return in;
     uint32_t all_or = 0, all_and = 0xffffffffu;
 #pragma omp parallel for schedule(static) reduction(|: all_or) reduction(&: all_and)
     for (long i = 0; i < (long)n; i++) { all_or |= in[i].addr; all_and &= in[i].addr; }
@@ -346,7 +299,7 @@ const MemOp* sort_by_addr(const PodVec<MemOp>& in, std::unique_ptr<MemOp[]> hold
     constexpr int BITS = 11, BUCKETS = 1 << BITS;
     const int T = std::max(1, omp_get_max_threads());
     std::vector<size_t> hist((size_t)T * BUCKETS);
-    const MemOp* src = in.data();
+    const MemOp* src = in;
     int next = 0;
     for (int shift = 0; shift < 32; shift += BITS) {
         if (((varying >> shift) & (BUCKETS - 1)) == 0) continue;
@@ -374,114 +327,80 @@ const MemOp* sort_by_addr(const PodVec<MemOp>& in, std::unique_ptr<MemOp[]> hold
     return src;
 }
 
-void build_mem(const Vm& vm, Traces& t) {
-    constexpr size_t W = 14;
-    std::unique_ptr<MemOp[]> hold[2];
-    const MemOp* ops = sort_by_addr(vm.mem_ops, hold);
-    // the static cells open the trace (memory/src/lib.rs:163-169): is_static_initial = 1, clk = 0, is_write = 1, counter = n
-    const size_t n0 = vm.static_cells.size();
-    size_t n = vm.mem_ops.size(), h = next_pow2(n0 + n);
-    Buf& v = t.store[2];
+// The n x W rows fill(row, i) writes, zero rows up to a power of two: every word of the n rows is written by the row function and
+// only the padding is cleared (no zero fill of a 0.9 GB matrix first)
+template <class Fill> void build_rows(size_t n, size_t W, Buf& v, vgpu_matrix& out, Fill fill) {
+    const size_t h = next_pow2(n);
     v.alloc(h * W);
-    for (size_t i = 0; i < n0; i++) {
-        uint32_t* row = &v[i * W];
-        std::memset(row, 0, W * sizeof(uint32_t));
-        row[0] = vm.static_cells[i].first % P; word_be(vm.static_cells[i].second, &row[1]);     // memory/src/lib.rs:276
-        row[6] = 1; row[8] = 1; row[12] = (uint32_t)i;
-    }
-    // every word of the n operation rows is written here and the padding rows are cleared below: no zero fill of the
-    // whole 0.9 GB matrix first
 #pragma omp parallel for schedule(static)
-    for (long i = 0; i < (long)n; i++) {
-        uint32_t* row = &v[(n0 + (size_t)i) * W];
-        row[0] = ops[i].addr % P; word_be(ops[i].value, &row[1]);      // sorted by the u32 address, stored reduced (memory/src/lib.rs:247-262)
-        row[5] = ops[i].clk; row[6] = 0;
-        row[7] = ops[i].is_write ? 0 : 1; row[8] = ops[i].is_write ? 1 : 0;
-        row[9] = 0; row[10] = 0; row[11] = 0;
-        row[12] = (uint32_t)(n0 + (size_t)i); row[13] = 0;
-    }
-    v.clear_range((n0 + n) * W, h * W);
-    t.main[2] = {v.data(), h, W};
-}
-
-void build_addsub(const PodVec<AluRec>& ops, bool is_add, Buf& v, vgpu_matrix& out) {
-    constexpr size_t W = 16;
-    size_t n = ops.size(), h = next_pow2(n);
-    v.zeros(h * W);
-#pragma omp parallel for schedule(static)
-    for (long i = 0; i < (long)n; i++) {
-        uint32_t* row = &v[(size_t)i * W];
-        uint32_t a[4], b[4], c[4];
-        word_be(ops[i].a, a); word_be(ops[i].b, b); word_be(ops[i].c, c);
-        std::memcpy(row + 0, b, 16); std::memcpy(row + 4, c, 16); std::memcpy(row + 11, a, 16);
-        if (is_add) {
-            uint32_t c1 = (b[3] + c[3] > 255), c2 = (b[2] + c[2] + c1 > 255), c3 = (b[1] + c[1] + c2 > 255);
-            row[8] = c1; row[9] = c2; row[10] = c3;
-        } else {  // alu_u32/src/sub/mod.rs op_to_row
-            // exactly as the reference (no borrow propagation into the comparison): sub/mod.rs:103-111
-            uint32_t b1 = (b[3] < c[3]), b2 = (b[2] < c[2]), b3 = (b[1] < c[1]);
-            row[8] = b1; row[9] = b2; row[10] = b3;
-        }
-        row[15] = 1;
-    }
+    for (long i = 0; i < (long)n; i++) fill(&v[(size_t)i * W], (size_t)i);
+    v.clear_range(n * W, h * W);
     out = {v.data(), h, W};
 }
 
-// Lt32Chip::op_to_row / set_cols (alu_u32/src/lt/mod.rs:86-160)
-void build_lt(const PodVec<LtRec>& ops, Buf& v, vgpu_matrix& out) {
-    constexpr size_t W = 45;
-    size_t n = ops.size(), h = next_pow2(n);
-    v.zeros(h * W);
-#pragma omp parallel for schedule(static)
-    for (long i = 0; i < (long)n; i++) {
-        uint32_t* row = &v[(size_t)i * W];
-        uint32_t a[4], b[4], c[4];
-        word_be(ops[i].a, a); word_be(ops[i].b, b); word_be(ops[i].c, c);
-        std::memcpy(row + 0, b, 16); std::memcpy(row + 4, c, 16);
-        row[21] = a[3];
-        bool is_signed = ops[i].opcode == OP_SLT32 || ops[i].opcode == OP_SLE32;
-        row[ops[i].opcode == OP_LT32 ? 23 : ops[i].opcode == OP_LTE32 ? 24 : ops[i].opcode == OP_SLT32 ? 25 : 26] = 1;
-        for (int k = 0; k < 4; k++) {
-            if (b[k] != c[k]) {
-                uint32_t z = 256u + b[k] - c[k];
-                for (int bit = 0; bit < 9; bit++) row[12 + bit] = (z >> bit) & 1;
-                row[8 + k] = 1;
-                uint32_t diff = (b[k] + P - c[k]) % P;
-                row[27] = fpow(diff, P - 2);
-                break;
-            }
-        }
-        for (int bit = 0; bit < 8; bit++) { row[28 + bit] = (b[0] >> bit) & 1; row[36 + bit] = (c[0] >> bit) & 1; }
-        row[44] = (is_signed && row[28 + 7] != row[36 + 7]) ? 1 : 0;
-        row[22] = 1;
-    }
-    out = {v.data(), h, W};
+void build_mem(const VgVmLogs& L, Traces& t) {
+    std::unique_ptr<MemOp[]> hold[2];
+    const MemOp* ops = sort_by_addr(L.mem, L.n_mem, hold);
+    const size_t n0 = L.n_static;                     // the static cells open the trace
+    build_rows(n0 + L.n_mem, MEM_COLS, t.store[2], t.main[2], [&](uint32_t* row, size_t i) {
+        if (i < n0) mem_row(row, i, {0u, L.static_addr[i], L.static_value[i], 1u}, true);
+        else mem_row(row, i, ops[i - n0], false);
+    });
 }
-
-// Bitwise32Chip::op_to_row / set_cols (alu_u32/src/bitwise/mod.rs:84-131): input_1 0..3, input_2 4..7,
-// bits_1[byte][bit] 8 + 8*byte + bit, bits_2 40 + ..., output 72..75, is_and 76, is_or 77, is_xor 78
-void build_bitwise(const PodVec<BitRec>& ops, Buf& v, vgpu_matrix& out) {
-    constexpr size_t W = 79;
-    size_t n = ops.size(), h = next_pow2(n);
-    v.zeros(h * W);
-#pragma omp parallel for schedule(static)
-    for (long i = 0; i < (long)n; i++) {
-        uint32_t* row = &v[(size_t)i * W];
-        uint32_t a[4], b[4], c[4];
-        word_be(ops[i].a, a); word_be(ops[i].b, b); word_be(ops[i].c, c);
-        std::memcpy(row + 0, b, 16); std::memcpy(row + 4, c, 16); std::memcpy(row + 72, a, 16);
-        for (int k = 0; k < 4; k++)
-            for (int bit = 0; bit < 8; bit++) { row[8 + 8 * k + bit] = (b[k] >> bit) & 1; row[40 + 8 * k + bit] = (c[k] >> bit) & 1; }
-        row[ops[i].opcode == OP_AND32 ? 76 : ops[i].opcode == OP_OR32 ? 77 : 78] = 1;
-    }
-    out = {v.data(), h, W};
-}
-
-void zero_chip(Buf& v, vgpu_matrix& out, size_t w) { v.zeros(w); out = {v.data(), 1, w}; }
 
 }  // namespace
 
 struct vgpu_traces { Traces t; };
+
+// The short chips: a zero-filled h-row trace of chip `id` in store[id], preprocessed trace `which` in store[14 + which]; widths
+// from the machine's chip table
+vgpu_traces* vg_short_chip_traces(const VgVmLogs& L) {
+    std::unique_ptr<vgpu_traces> tr(new vgpu_traces());      // freed if an allocation below throws
+    Traces& t = tr->t;
+    const auto chip = [&](uint32_t id, size_t h) {
+        const size_t w = vgpu_basic_machine_chip(id)->width;
+        t.main[id] = {t.store[id].zeros(h * w), h, w};
+        return t.store[id].data();
+    };
+    const auto prep = [&](int which, uint32_t id, size_t h) {
+        const size_t w = vgpu_basic_machine_chip(id)->preprocessed_width;
+        t.prep[which] = {t.store[14 + which].zeros(h * w), h, w};
+        return t.store[14 + which].data();
+    };
+    {   // program: 1 main column (execution counts) + 7 preprocessed
+        const size_t h = next_pow2(L.n_instr);
+        uint32_t* counts = chip(1, h);
+        uint32_t* pre = prep(0, 1, h);
+        for (size_t i = 0; i < h; i++) {
+            uint32_t* row = &pre[i * 7];
+            row[0] = (uint32_t)i;
+            // every row of the program, executed or not: InstructionWord::flatten takes the opcode from_canonical_u32 (machine/src/program.rs:44)
+            if (i < L.n_instr) {
+                counts[i] = L.prog_counts[i];
+                row[1] = (uint32_t)L.program[6 * i] % P;
+                for (int k = 0; k < 5; k++) row[2 + k] = from_i32(L.program[6 * i + 1 + k]);
+            }
+        }
+    }
+    {   // mul: 2^10 counter rows
+        uint32_t* m = chip(5, 1024);
+        for (uint32_t i = 0; i < 1024; i++) m[i * 18 + 17] = i + 1;
+    }
+    for (uint32_t id : {6u, 7u, 9u, 11u}) chip(id, 1);      // div, shift, com, output: no rows in the provable instruction subset
+    {   // range: (multiplicity, counter) + preprocessed counter
+        uint32_t* r = chip(12, 256);
+        uint32_t* c = prep(1, 12, 256);
+        for (uint32_t i = 0; i < 256; i++) { r[2 * i] = L.range_count[i]; r[2 * i + 1] = i; c[i] = i; }
+    }
+    {   // static_data: (addr, value[4], is_real) per cell in address order, padded to a power of two (one zero row when empty)
+        uint32_t* s = chip(13, next_pow2(L.n_static ? L.n_static : 1));
+        for (size_t i = 0; i < L.n_static; i++) {
+            uint32_t* row = &s[i * 6];
+            row[0] = L.static_addr[i] % P; word_be(L.static_value[i], &row[1]); row[5] = 1;    // static_data/src/lib.rs:67
+        }
+    }
+    return tr.release();
+}
 
 extern "C" {
 
@@ -495,10 +414,10 @@ static int vm_run_impl(const int32_t* program_words, uint64_t n_instr, uint32_t 
         for (uint64_t i = 0; i < n_static; i++) sc.push_back({static_addrs[i], static_values[i]});
         std::stable_sort(sc.begin(), sc.end(), [](const std::pair<uint32_t, uint32_t>& x, const std::pair<uint32_t, uint32_t>& y) { return x.first < y.first; });
         for (auto& c : sc) {            // a repeated address keeps the LAST value, as BTreeMap::insert does
-            if (!vm.static_cells.empty() && vm.static_cells.back().first == c.first) vm.static_cells.back().second = c.second;
-            else vm.static_cells.push_back(c);
+            if (!vm.static_addr.empty() && vm.static_addr.back() == c.first) vm.static_value.back() = c.second;
+            else { vm.static_addr.push_back(c.first); vm.static_value.push_back(c.second); }
         }
-        for (auto& c : vm.static_cells) vm.cells.set(c.first, c.second);
+        for (size_t i = 0; i < vm.static_addr.size(); i++) vm.cells.set(vm.static_addr[i], vm.static_value[i]);
     }
     int rc = 0;
     while ((rc = vm.step()) == 0) {
@@ -511,58 +430,20 @@ static int vm_run_impl(const int32_t* program_words, uint64_t n_instr, uint32_t 
     return 0;
 }
 
-// Chip::generate_trace x14 on the host
-static vgpu_traces* build_traces_host(Vm& vm) {
-    const int32_t* program_words = vm.prog;
-    const uint64_t n_instr = vm.n_instr;
-    std::unique_ptr<vgpu_traces> tr(new vgpu_traces());      // released to the caller at the end; freed if an allocation below throws
+// Chip::generate_trace x14 on the host from the interpreter's logs; `cells` is the memory the run left (vgpu_traces_mem_cell)
+static vgpu_traces* build_traces_host(const VgVmLogs& L, const CellMap& cells) {
+    std::unique_ptr<vgpu_traces> tr(vg_short_chip_traces(L));      // released to the caller at the end; freed if an allocation below throws
     Traces& t = tr->t;
-    t.clock = vm.clock; t.n_mem_ops = (uint32_t)vm.mem_ops.size(); t.n_add_ops = (uint32_t)vm.adds.size(); t.n_sub_ops = (uint32_t)vm.subs.size();
-    build_cpu(vm, t);
-    build_mem(vm, t);
-    {  // program: 1 main column (counts) + 7 preprocessed
-        size_t h = next_pow2(n_instr);
-        t.store[1].zeros(h);
-        for (size_t i = 0; i < n_instr; i++) t.store[1][i] = vm.prog_counts[i];
-        t.main[1] = {t.store[1].data(), h, 1};
-        t.store[14].zeros(h * 7);
-        for (size_t i = 0; i < h; i++) {
-            uint32_t* row = &t.store[14][i * 7];
-            row[0] = (uint32_t)i;
-            // every row of the program, executed or not: InstructionWord::flatten takes the opcode from_canonical_u32 (machine/src/program.rs:44)
-            if (i < n_instr) { row[1] = (uint32_t)program_words[6 * i] % P; for (int k = 0; k < 5; k++) row[2 + k] = from_i32(program_words[6 * i + 1 + k]); }
-        }
-        t.prep[0] = {t.store[14].data(), h, 7};
-    }
-    build_addsub(vm.adds, true, t.store[3], t.main[3]);
-    build_addsub(vm.subs, false, t.store[4], t.main[4]);
-    {  // mul: 2^10 counter rows
-        t.store[5].zeros(1024 * 18);
-        for (size_t i = 0; i < 1024; i++) t.store[5][i * 18 + 17] = (uint32_t)i + 1;
-        t.main[5] = {t.store[5].data(), 1024, 18};
-    }
-    zero_chip(t.store[6], t.main[6], 14);   // div
-    zero_chip(t.store[7], t.main[7], 28);   // shift
-    build_lt(vm.lts, t.store[8], t.main[8]);   // lt
-    zero_chip(t.store[9], t.main[9], 14);   // com
-    build_bitwise(vm.bits, t.store[10], t.main[10]);   // bitwise
-    zero_chip(t.store[11], t.main[11], 7);  // output
-    {  // range: (mult, counter) + preprocessed counter
-        t.store[12].zeros(256 * 2); t.store[15].zeros(256);
-        for (uint32_t i = 0; i < 256; i++) { t.store[12][i * 2] = vm.range_count[i]; t.store[12][i * 2 + 1] = i; t.store[15][i] = i; }
-        t.main[12] = {t.store[12].data(), 256, 2};
-        t.prep[1] = {t.store[15].data(), 256, 1};
-    }
-    {   // static_data: (addr, value[4], is_real) per cell in address order, padded to a power of two (one zero row when empty)
-        const size_t n0 = vm.static_cells.size(), h = next_pow2(n0 ? n0 : 1);
-        t.store[13].zeros(h * 6);
-        for (size_t i = 0; i < n0; i++) {
-            uint32_t* row = &t.store[13][i * 6];
-            row[0] = vm.static_cells[i].first % P; word_be(vm.static_cells[i].second, &row[1]); row[5] = 1;    // static_data/src/lib.rs:67
-        }
-        t.main[13] = {t.store[13].data(), h, 6};
-    }
-    t.cells = vm.cells;
+    t.clock = (uint32_t)L.n_cpu; t.n_mem_ops = (uint32_t)L.n_mem; t.n_add_ops = (uint32_t)L.n_adds; t.n_sub_ops = (uint32_t)L.n_subs;
+    build_cpu(L, t);
+    build_mem(L, t);
+    build_rows(L.n_adds, ADDSUB_COLS, t.store[3], t.main[3], [&](uint32_t* row, size_t i) { addsub_row(row, L.adds[i], true); });
+    build_rows(L.n_subs, ADDSUB_COLS, t.store[4], t.main[4], [&](uint32_t* row, size_t i) { addsub_row(row, L.subs[i], false); });
+    build_rows(L.n_lts, LT_COLS, t.store[8], t.main[8], [&](uint32_t* row, size_t i) {
+        if (const uint32_t d = lt_row(row, L.lts[i])) row[27] = fpow(d, P - 2);
+    });
+    build_rows(L.n_bits, BITWISE_COLS, t.store[10], t.main[10], [&](uint32_t* row, size_t i) { bitwise_row(row, L.bits[i]); });
+    t.cells = cells;
     return tr.release();
 }
 
@@ -571,13 +452,13 @@ static int machine_run_impl(const int32_t* program_words, uint64_t n_instr, uint
                             vgpu_traces** out, char* err, uint64_t err_len) {
     Vm vm;
     if (vm_run_impl(program_words, n_instr, initial_pc, initial_fp, max_cycles, static_addrs, static_values, n_static, vm, err, err_len) != 0) return -1;
-    *out = build_traces_host(vm);
+    *out = build_traces_host(vm.logs(), vm.cells);
     return 0;
 }
 
 // ---- the interpreter's logs as an object: Machine::run without the row fill (the device builds the rows, witness.cu) ----
 }  // extern "C"
-struct vgpu_vmlog { Vm vm; std::vector<int32_t> program; std::vector<uint32_t> st_addr, st_val; VgVmLogs view; };
+struct vgpu_vmlog { Vm vm; std::vector<int32_t> program; VgVmLogs view; };
 extern "C" {
 
 int32_t vgpu_vm_run(const int32_t* program_words, uint64_t n_instr, uint32_t initial_pc, uint32_t initial_fp, uint64_t max_cycles,
@@ -586,18 +467,7 @@ int32_t vgpu_vm_run(const int32_t* program_words, uint64_t n_instr, uint32_t ini
         std::unique_ptr<vgpu_vmlog> L(new vgpu_vmlog());
         L->program.assign(program_words, program_words + 6 * n_instr);
         if (vm_run_impl(L->program.data(), n_instr, initial_pc, initial_fp, max_cycles, static_addrs, static_values, n_static, L->vm, err, err_len) != 0) return -1;
-        Vm& vm = L->vm;
-        for (auto& c : vm.static_cells) { L->st_addr.push_back(c.first); L->st_val.push_back(c.second); }
-        VgVmLogs& v = L->view;
-        v.program = L->program.data(); v.n_instr = n_instr;
-        v.cpu = vm.cpu.data(); v.n_cpu = vm.cpu.size();
-        v.mem = vm.mem_ops.data(); v.n_mem = vm.mem_ops.size();
-        v.adds = vm.adds.data(); v.n_adds = vm.adds.size();
-        v.subs = vm.subs.data(); v.n_subs = vm.subs.size();
-        v.lts = vm.lts.data(); v.n_lts = vm.lts.size();
-        v.bits = vm.bits.data(); v.n_bits = vm.bits.size();
-        v.prog_counts = vm.prog_counts.data(); v.range_count = vm.range_count;
-        v.static_addr = L->st_addr.data(); v.static_value = L->st_val.data(); v.n_static = L->st_addr.size();
+        L->view = L->vm.logs();
         *out = L.release();
         return 0;
     } catch (const std::exception& e) {
@@ -611,7 +481,7 @@ void vgpu_vmlog_stats(const vgpu_vmlog* l, uint32_t* clock, uint32_t* mem_ops, u
 }
 // Chip::generate_trace x14 on the host from the same logs (the reference witness the device builder is compared with)
 int32_t vgpu_vmlog_traces(vgpu_vmlog* l, vgpu_traces** out, char* err, uint64_t err_len) {
-    try { *out = build_traces_host(l->vm); return 0; }
+    try { *out = build_traces_host(l->view, l->vm.cells); return 0; }
     catch (const std::exception& e) { if (err && err_len) std::snprintf(err, err_len, "host witness generation failed: %s", e.what()); return -1; }
 }
 void vgpu_vmlog_free(vgpu_vmlog* l) { delete l; }
