@@ -229,6 +229,35 @@ int32_t vgpu_quotient(vgpu_ctx* ctx, const vgpu_chip_desc* chip, uint32_t log_de
 int32_t vgpu_check_constraints(vgpu_ctx* ctx, const vgpu_chip_desc* chip, const vgpu_dmat* main, const vgpu_dmat* prep_or_null,
                                const vgpu_dmat* perm, const uint32_t challenges[15],
                                int64_t* first_row, uint32_t* first_constraint, uint64_t* failing_rows);
+/* Collective: every rank of a split proof makes the call with its own matrices (this rank's row shards of the tall traces, or whole
+ * matrices).  Writes on every rank what vgpu_check_constraints writes for the whole traces on one GPU.  On a context that does not
+ * split proofs it IS vgpu_check_constraints.  Synchronises.
+ * A trace tall enough to be split is swept over this rank's run of rows (of a whole matrix too, so its failing rows count once); the
+ * next row of the run's last row is the next rank's first row, and the cumulative sum the last rank's, which one all-gather of a
+ * small block per rank brings over (no peer pointers: a borrowed shard may be any caller memory).  One more all-gather combines the
+ * verdicts.  A shorter trace is checked whole by every rank.  Refused alike on every rank, before anything is enqueued: what
+ * vgpu_check_constraints refuses except row shards, a matrix stored with bit-reversed rows (quotient chunks), and a row shard that
+ * is not this context's run for its height (vgpu_ctx_local_rows; e.g. after vgpu_comm_set_sharding(ctx, 0)). */
+int32_t vgpu_check_constraints_local(vgpu_ctx* ctx, const vgpu_chip_desc* chip, const vgpu_dmat* main, const vgpu_dmat* prep_or_null,
+                                     const vgpu_dmat* perm, const uint32_t challenges[15],
+                                     int64_t* first_row, uint32_t* first_constraint, uint64_t* failing_rows);
+
+typedef struct vgpu_check_report {
+    int64_t first_row;          /* -1: every constraint vanishes on every row */
+    uint32_t first_constraint;
+    uint64_t failing_rows;
+    uint32_t cumulative_sum[5]; /* canonical */
+} vgpu_check_report;
+/* check_constraints of the 14 BasicMachine chips + check_cumulative_sums over a machine witness (the reference's debug-build check,
+ * derive/src/lib.rs:246-253,376-377) without a proof: LogUp traces built here with the caller's 15 challenge words, every chip checked,
+ * *sums_cancel = 1 when the cumulative sums add to zero.  Whole matrices or row shards (vgpu_witness_device on a split context,
+ * *_local imports and borrows); collective on a split context, identical reports on every rank.  Each chip's permutation trace is
+ * released once its sweep is enqueued, so the call needs the traces, the largest permutation trace and small scratch.  Besides the
+ * LogUp traces' own all-gathers, one all-gather exchanges the boundary rows of every split chip and one the verdicts.  Synchronises
+ * once.  A witness that passes for random challenges passes for the transcript's with overwhelming probability; the cancellation
+ * check holds for any challenges. */
+int32_t vgpu_check_witness(vgpu_ctx* ctx, const vgpu_dmat* const main[VGPU_NUM_CHIPS], const vgpu_dmat* const prep[2],
+                           const uint32_t challenges[15], vgpu_check_report report[VGPU_NUM_CHIPS], int32_t* sums_cancel);
 
 /* ---- Fiat-Shamir transcript owned by the context (DuplexChallenger; config.challenger() clone) ------
  * reset() restores the initial sponge of vgpu_set_challenger; values are canonical words. */

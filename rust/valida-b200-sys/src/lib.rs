@@ -96,6 +96,18 @@ pub struct vgpu_chip_desc {
     pub interactions: [vgpu_interaction; VGPU_MAX_INTERACTIONS],
 }
 
+/// One chip's verdict of [`vgpu_check_witness`].
+#[repr(C)]
+#[derive(Clone, Copy, Debug, Default)]
+pub struct vgpu_check_report {
+    /// `-1`: every constraint vanishes on every row.
+    pub first_row: i64,
+    pub first_constraint: u32,
+    pub failing_rows: u64,
+    /// Canonical words.
+    pub cumulative_sum: [u32; 5],
+}
+
 extern "C" {
     // ---- context ----
     pub fn vgpu_ctx_create(device: i32, cuda_stream: *mut c_void, out: *mut *mut vgpu_ctx) -> i32;
@@ -148,6 +160,8 @@ extern "C" {
     pub fn vgpu_perm_trace(ctx: *mut vgpu_ctx, chip: *const vgpu_chip_desc, main: *const vgpu_dmat, prep_or_null: *const vgpu_dmat, challenges: *const u32, out_perm: *mut *mut vgpu_dmat, cumulative_sum_out: *mut u32) -> i32;
     pub fn vgpu_quotient(ctx: *mut vgpu_ctx, chip: *const vgpu_chip_desc, log_degree: u32, prep_lde_or_null: *const vgpu_dmat, main_lde: *const vgpu_dmat, perm_lde: *const vgpu_dmat, cumulative_sum: *const u32, perm_challenges: *const u32, alpha: *const u32, out_chunks: *mut *mut vgpu_dmat) -> i32;
     pub fn vgpu_check_constraints(ctx: *mut vgpu_ctx, chip: *const vgpu_chip_desc, main: *const vgpu_dmat, prep_or_null: *const vgpu_dmat, perm: *const vgpu_dmat, challenges: *const u32, first_row: *mut i64, first_constraint: *mut u32, failing_rows: *mut u64) -> i32;
+    pub fn vgpu_check_constraints_local(ctx: *mut vgpu_ctx, chip: *const vgpu_chip_desc, main: *const vgpu_dmat, prep_or_null: *const vgpu_dmat, perm: *const vgpu_dmat, challenges: *const u32, first_row: *mut i64, first_constraint: *mut u32, failing_rows: *mut u64) -> i32;
+    pub fn vgpu_check_witness(ctx: *mut vgpu_ctx, main: *const *const vgpu_dmat, prep: *const *const vgpu_dmat, challenges: *const u32, report: *mut vgpu_check_report, sums_cancel: *mut i32) -> i32;
 
     // ---- transcript ----
     pub fn vgpu_challenger_reset(ctx: *mut vgpu_ctx) -> i32;

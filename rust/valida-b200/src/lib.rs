@@ -370,6 +370,33 @@ impl Context {
         Ok(proof)
     }
 
+    /// `check_constraints` (`machine/src/check_constraints.rs:14-84`) of BasicMachine chip `chip_id` on a rank of a split proof:
+    /// every rank passes its own matrices (its row shards of the tall traces, or whole matrices) and gets what the check of the
+    /// whole traces on one GPU gives: `(first failing row or -1, its first failing constraint, number of failing rows)`.  On a
+    /// context that does not split proofs it is the single-GPU check.  Collective; synchronises.
+    pub fn check_constraints_local(&self, chip_id: u32, main: &DMat<'_>, prep: Option<&DMat<'_>>, perm: &DMat<'_>, challenges: &[u32; 15]) -> Result<(i64, u32, u64)> {
+        let chip = unsafe { sys::vgpu_basic_machine_chip(chip_id) };
+        let prep_ptr = prep.map_or(ptr::null(), |m| m.as_ptr());
+        let (mut row, mut constraint, mut failing) = (0i64, 0u32, 0u64);
+        self.check(unsafe {
+            sys::vgpu_check_constraints_local(self.raw, chip, main.as_ptr(), prep_ptr, perm.as_ptr(), challenges.as_ptr(), &mut row, &mut constraint, &mut failing)
+        })?;
+        Ok((row, constraint, failing))
+    }
+
+    /// The witness check of the reference's debug builds (`check_constraints` of every chip + `check_cumulative_sums`,
+    /// `derive/src/lib.rs:246-253,376-377`) without a proof, with the caller's 15 challenge words: one report per chip and whether
+    /// the cumulative sums cancel.  `main` / `prep` are whole traces or, on a [`LocalGroup`] rank, its row shards; every rank of a
+    /// split proof makes the call and gets the same reports.  A host that splits proofs runs this in debug builds.
+    pub fn check_witness(&self, main: &[&DMat<'_>; sys::VGPU_NUM_CHIPS], prep: &[&DMat<'_>; 2], challenges: &[u32; 15]) -> Result<([sys::vgpu_check_report; sys::VGPU_NUM_CHIPS], bool)> {
+        let main_raw: Vec<*const vgpu_dmat> = main.iter().map(|m| m.as_ptr()).collect();
+        let prep_raw: Vec<*const vgpu_dmat> = prep.iter().map(|m| m.as_ptr()).collect();
+        let mut reports = [sys::vgpu_check_report::default(); sys::VGPU_NUM_CHIPS];
+        let mut cancel = 0i32;
+        self.check(unsafe { sys::vgpu_check_witness(self.raw, main_raw.as_ptr(), prep_raw.as_ptr(), challenges.as_ptr(), reports.as_mut_ptr(), &mut cancel) })?;
+        Ok((reports, cancel != 0))
+    }
+
     /// Kernels launched by this context so far.
     pub fn launch_count(&self) -> u64 {
         unsafe { sys::vgpu_ctx_launch_count(self.raw) }

@@ -26,6 +26,8 @@ from .api import (  # noqa: F401
     generate_permutation_trace,
     quotient,
     check_constraints,
+    check_constraints_local,
+    check_witness,
     lib,
     lib_path,
     run_program,

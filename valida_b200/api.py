@@ -36,6 +36,11 @@ class _DevMatrix(C.Structure):
     _fields_ = [("data", C.c_void_p), ("height", C.c_uint64), ("width", C.c_uint64), ("row_stride", C.c_uint64), ("col_stride", C.c_uint64)]
 
 
+class _CheckReport(C.Structure):
+    """vgpu_check_report: one chip's verdict of vgpu_check_witness."""
+    _fields_ = [("first_row", C.c_int64), ("first_constraint", C.c_uint32), ("failing_rows", C.c_uint64), ("cumulative_sum", C.c_uint32 * 5)]
+
+
 def _load():
     if not os.path.exists(lib_path):
         raise VgpuError(
@@ -82,6 +87,8 @@ def _load():
         "vgpu_perm_trace": (C.c_int32, [vp, vp, vp, vp, u32p, C.POINTER(vp), u32p]),
         "vgpu_quotient": (C.c_int32, [vp, vp, C.c_uint32, vp, vp, vp, u32p, u32p, u32p, C.POINTER(vp)]),
         "vgpu_check_constraints": (C.c_int32, [vp, vp, vp, vp, vp, u32p, C.POINTER(C.c_int64), u32p, C.POINTER(u64)]),
+        "vgpu_check_constraints_local": (C.c_int32, [vp, vp, vp, vp, vp, u32p, C.POINTER(C.c_int64), u32p, C.POINTER(u64)]),
+        "vgpu_check_witness": (C.c_int32, [vp, C.POINTER(vp), C.POINTER(vp), u32p, C.POINTER(_CheckReport), C.POINTER(C.c_int32)]),
         "vgpu_ctx_set_debug_checks": (C.c_int32, [vp, C.c_int32]),
         "vgpu_set_challenger": (C.c_int32, [vp, u32p, u32p]),
         "vgpu_ctx_set_merkle_hash": (C.c_int32, [vp, C.c_int32]),
@@ -580,6 +587,30 @@ def check_constraints(ctx, chip_id, main, prep, perm, perm_challenges):
     ctx.check(lib().vgpu_check_constraints(ctx._h, chip, main._h, prep._h if prep is not None else None, perm._h,
                                            _u32arr(perm_challenges, 15), C.byref(row), C.byref(con), C.byref(n)))
     return int(row.value), int(con.value), int(n.value)
+
+
+def check_constraints_local(ctx, chip_id, main, prep, perm, perm_challenges):
+    """check_constraints on a split context: every rank calls it with its own matrices (its row shards of the tall traces, or whole
+    matrices) and gets what check_constraints returns for the whole traces on one GPU.  On a context that does not split proofs it is
+    check_constraints."""
+    chip = lib().vgpu_basic_machine_chip(chip_id)
+    row, con, n = C.c_int64(), C.c_uint32(), C.c_uint64()
+    ctx.check(lib().vgpu_check_constraints_local(ctx._h, chip, main._h, prep._h if prep is not None else None, perm._h,
+                                                 _u32arr(perm_challenges, 15), C.byref(row), C.byref(con), C.byref(n)))
+    return int(row.value), int(con.value), int(n.value)
+
+
+def check_witness(ctx, main, prep, challenges):
+    """check_constraints of the 14 chips and check_cumulative_sums over a machine witness (the reference's debug-build check), without
+    a proof: main / prep are the 14 + 2 DeviceMatrix traces (whole, or this rank's row shards on a split context, where every rank
+    calls it).  Returns ([(first row or -1, constraint, failing rows, cumulative sum [5]) per chip], sums_cancel)."""
+    a = (C.c_void_p * NUM_CHIPS)(*[m._h for m in main])
+    b = (C.c_void_p * 2)(*[m._h for m in prep])
+    rep = (_CheckReport * NUM_CHIPS)()
+    cancel = C.c_int32()
+    ctx.check(lib().vgpu_check_witness(ctx._h, a, b, _u32arr(challenges, 15), rep, C.byref(cancel)))
+    return ([(int(r.first_row), int(r.first_constraint), int(r.failing_rows), np.array(list(r.cumulative_sum), dtype=np.uint32)) for r in rep],
+            bool(cancel.value))
 
 
 class StarkConfig:

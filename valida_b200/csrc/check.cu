@@ -1,12 +1,18 @@
 // check_constraints (machine/src/check_constraints.rs:14-84; debug builds of the reference's prove, derive/src/lib.rs:246-253) on the
-// device: every constraint of a chip's Air::eval and of eval_permutation_constraints on every row i of the TRACE, with row (i+1) mod h
-// as "next" and the debug selectors is_first_row = [i == 0], is_last_row = [i == h-1], is_transition = 1 - is_last_row.
+// device: every constraint of a chip's Air::eval and of eval_permutation_constraints on every row g of the TRACE, with row (g+1) mod h
+// as "next" and the debug selectors is_first_row = [g == 0], is_last_row = [g == h-1], is_transition = 1 - is_last_row.
 // One thread per natural trace row reads the column-major traces (coalesced) through the same AIR text as the quotient sweep
 // (airs.cuh, logup.cuh), so constraint i here is constraint i there: the chip's assertions in eval order, one per interaction,
 // then the LogUp transition, first-row and last-row constraints.  The cumulative sum is read on the device from the permutation
 // trace's last row and last column (check_constraints.rs:33).
-// Result per chip: the first failing (row, constraint) as ONE 64-bit key (row << 8 | constraint, atomicMin) and the number of rows
-// with at least one failure; both are aggregated per warp, so a clean trace costs no atomic at all.
+// One launch sweeps a RUN of rows: local rows [0, n) of matrices entered at global row g0, the next row of local row n-1 being local
+// row `wrap`.  A whole trace is one run (g0 = 0, n = h, wrap = 0).  A split proof's rank r holds the run vg_trace_run(ctx, h): it
+// sweeps all its rows but the last, whose next row is rank (r+1) mod N's first row; every rank packs its first row (and its last
+// row's running sum) into a small block, one all-gather exchanges the blocks, and the last row is swept from a 2-row window (own
+// last row, next rank's first row; column-major, stride 2) as a run of one row whose next row is window row 1.  No peer pointers:
+// a borrowed shard is caller memory, outside the symmetric heap.
+// Result per chip: the first failing (row, constraint) as ONE 64-bit key (global row << 8 | constraint, atomicMin) and the number of
+// rows with at least one failure; both are aggregated per warp, so a clean trace costs no atomic at all.
 #include "ctx.h"
 #include "devchip.h"
 #include "airs.cuh"
@@ -23,10 +29,11 @@ constexpr uint32_t CHECK_NONE = 0xffffffffu;
 constexpr uint32_t CHECK_MAX_CONSTRAINTS = 256;   // the constraint index takes the low 8 bits of the key
 
 struct CParams {
-    const uint32_t* main; uint64_t mcs;
+    const uint32_t* main; uint64_t mcs;             // every matrix pointer is at local row 0 of the run
     const uint32_t* prep; uint64_t pcs;             // null without a preprocessed trace
-    const uint32_t* perm; uint64_t qcs;             // flattened permutation trace, h x 5(k+1)
-    uint64_t h;
+    const uint32_t* perm; uint64_t qcs;             // flattened permutation trace, 5(k+1) columns
+    const uint32_t* cumsum; uint64_t ccs;           // the cumulative sum's 5 words, ccs apart (read only by the row g = h-1)
+    uint64_t g0, n, h, wrap;                        // global row of local row 0; rows swept; global height; next row of local row n-1
     unsigned long long* first;                      // min over failing rows of (row << 8 | first failing constraint); ~0: none
     unsigned long long* count;                      // rows with at least one failing constraint
     DevChip chip;
@@ -46,66 +53,109 @@ struct CheckBuilder {
 template <int CHIP>
 __global__ void __launch_bounds__(128) check_kernel(const __grid_constant__ CParams p) {
     const uint64_t i_raw = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
-    const bool active = i_raw < p.h;
-    const uint64_t i = active ? i_raw : p.h - 1;          // idle lanes shadow the last row (the warp vote needs every lane)
-    const bool is_last = i + 1 == p.h;
-    const uint64_t n = is_last ? 0 : i + 1;                // a one-row chip is its own next row
+    const bool active = i_raw < p.n;
+    const uint64_t i = active ? i_raw : p.n - 1;          // idle lanes shadow the last row (the warp vote needs every lane)
+    // the global row is p.g0 + i, recomputed where it is used: a register kept for it makes two chips spill
+    const bool is_last = p.g0 + i + 1 == p.h;
+    const uint64_t n = i + 1 < p.n ? i + 1 : p.wrap;       // a one-row chip is its own next row
     CheckBuilder b;
     b.lrow = p.main + i; b.nrow = p.main + n; b.cs = p.mcs;
-    b.first = F{i == 0 ? bb::R1 : 0u};
+    b.first = F{p.g0 + i == 0 ? bb::R1 : 0u};
     b.last = F{is_last ? bb::R1 : 0u};
     b.trans = F{is_last ? 0u : bb::R1};
     b.idx = 0; b.bad = CHECK_NONE;
     air::eval_chip<CHIP>(b);
-    const uint32_t k = p.chip.n_interactions;
     E5 cumsum;
 #pragma unroll
-    for (int l = 0; l < 5; l++) cumsum.c[l] = __ldg(p.perm + (uint64_t)(5 * k + l) * p.qcs + p.h - 1);
+    for (int l = 0; l < 5; l++) cumsum.c[l] = __ldg(p.cumsum + (uint64_t)l * p.ccs);
     logup::eval_constraints(b, p.chip, b.lrow, b.nrow, p.mcs, p.prep ? p.prep + i : nullptr, p.prep ? p.prep + n : nullptr, p.pcs,
                             p.perm + i, p.perm + n, p.qcs, cumsum);
     const bool fail = active && b.bad != CHECK_NONE;
     const unsigned vote = __ballot_sync(0xffffffffu, fail);
     // the lowest failing lane holds the warp's lowest row, hence its smallest key
     if (vote && (threadIdx.x & 31) == (unsigned)(__ffs(vote) - 1)) {
-        atomicMin(p.first, ((unsigned long long)i << 8) | b.bad);
+        atomicMin(p.first, ((unsigned long long)(p.g0 + i) << 8) | b.bad);
         atomicAdd(p.count, (unsigned long long)__popc(vote));
     }
 }
 
-}  // namespace
+// n words of a strided source into a strided destination, per segment (one CTA each): the boundary rows of a split chip in and
+// out of the exchanged block and the windows.
+struct CopySeg { const uint32_t* src; uint64_t scs; uint32_t* dst; uint64_t dcs; uint32_t n; };
+constexpr int COPY_SEGS = 7;
+struct CopyList { CopySeg s[COPY_SEGS]; };
+__global__ void __launch_bounds__(64) check_copy_kernel(const __grid_constant__ CopyList l) {
+    const CopySeg& s = l.s[blockIdx.x];
+    for (uint32_t c = threadIdx.x; c < s.n; c += blockDim.x) s.dst[(uint64_t)c * s.dcs] = __ldg(s.src + (uint64_t)c * s.scs);
+}
 
-// Validates the arguments (before anything is enqueued) and enqueues the sweep of one chip.  d_first / d_count must hold ~0 / 0.
-int32_t vg_check_enqueue(vgpu_ctx* ctx, const vgpu_chip_desc* chip, const vgpu_dmat* main, const vgpu_dmat* prep, const vgpu_dmat* perm,
-                         const uint32_t challenges[15], unsigned long long* d_first, unsigned long long* d_count) {
-    if (!chip || !main || !perm || !challenges) VG_FAIL(ctx, "check_constraints: null argument");
+int32_t copy_segments(vgpu_ctx* ctx, const CopyList& l, int nseg) {
+    KScope ks(ctx, KC_CHECK, 0.0);
+    check_copy_kernel<<<nseg, 64, 0, ctx->stream>>>(l);
+    VG_LAUNCH_CHECK(ctx);
+    return 0;
+}
+
+// Refuses, before anything is enqueued and alike on every rank (global shapes and this context's run rule only), what the sweep
+// cannot check.  perm may be null (vgpu_check_witness builds it).  shards: row shards of this rank's run are accepted.
+int32_t check_shapes(vgpu_ctx* ctx, const vgpu_chip_desc* chip, const vgpu_dmat* main, const vgpu_dmat* prep, const vgpu_dmat* perm, bool shards) {
     if (chip->chip_id >= VGPU_NUM_CHIPS) VG_FAIL(ctx, "check_constraints: unknown chip id %u", chip->chip_id);
-    for (const vgpu_dmat* m : {main, prep, perm})
-        if (m && (m->dist != VG_FULL || m->bitrev_rows)) VG_FAIL(ctx, "check_constraints: whole matrices in natural row order only (not row shards)");
+    for (const vgpu_dmat* m : {main, prep, perm}) {
+        if (!m) continue;
+        if (!shards && (m->dist != VG_FULL || m->bitrev_rows)) VG_FAIL(ctx, "check_constraints: whole matrices in natural row order only (not row shards)");
+        if (m->bitrev_rows) VG_FAIL(ctx, "check_constraints: a matrix stores its rows bit-reversed (quotient chunks); the check reads traces in natural row order");
+    }
     if (main->gw != chip->width) VG_FAIL(ctx, "check_constraints: main width %llu != chip width %u", (unsigned long long)main->gw, chip->width);
     const uint64_t pw = 5ull * (chip->n_interactions + 1);
-    if (perm->gw != pw) VG_FAIL(ctx, "check_constraints: permutation trace width %llu != 5 (k + 1) = %llu", (unsigned long long)perm->gw, (unsigned long long)pw);
+    if (perm && perm->gw != pw) VG_FAIL(ctx, "check_constraints: permutation trace width %llu != 5 (k + 1) = %llu", (unsigned long long)perm->gw, (unsigned long long)pw);
     if (chip->preprocessed_width && !prep) VG_FAIL(ctx, "check_constraints: chip %u needs its preprocessed trace (%u columns)", chip->chip_id, chip->preprocessed_width);
     if (!chip->preprocessed_width && prep) VG_FAIL(ctx, "check_constraints: chip %u has no preprocessed trace", chip->chip_id);
     if (prep && prep->gw != chip->preprocessed_width) VG_FAIL(ctx, "check_constraints: preprocessed width %llu != %u", (unsigned long long)prep->gw, chip->preprocessed_width);
     const uint64_t h = main->gh;
     if (h == 0 || (h & (h - 1))) VG_FAIL(ctx, "check_constraints: trace height %llu is not a power of two", (unsigned long long)h);
-    if (perm->gh != h || (prep && prep->gh != h)) VG_FAIL(ctx, "check_constraints: the main, preprocessed and permutation traces differ in height");
+    if ((perm && perm->gh != h) || (prep && prep->gh != h)) VG_FAIL(ctx, "check_constraints: the main, preprocessed and permutation traces differ in height");
+    const VgRun run = vg_trace_run(ctx, h);
+    for (const vgpu_dmat* m : {main, prep, perm})
+        if (m && m->dist == VG_ROWS && !(run.split && m->row0 == run.begin && m->h == run.count))
+            VG_FAIL(ctx, "check_constraints: a row shard holding rows [%llu, %llu) of a trace of height %llu is not this context's run of that "
+                    "height, rows [%llu, %llu)%s", (unsigned long long)m->row0, (unsigned long long)(m->row0 + m->h), (unsigned long long)h,
+                    (unsigned long long)run.begin, (unsigned long long)(run.begin + run.count), run.split ? "" : " (the trace is not split here)");
     const uint32_t N = vg_chip_base_constraints(chip->chip_id) + chip->n_interactions + 3;
     if (N > CHECK_MAX_CONSTRAINTS) VG_FAIL(ctx, "check_constraints: %u constraints exceed the 8-bit index (%u)", N, CHECK_MAX_CONSTRAINTS);
+    return 0;
+}
+
+// Enqueues one run's sweep; p holds everything but the chip, which is built here from the challenges.
+int32_t enqueue_sweep(vgpu_ctx* ctx, const vgpu_chip_desc* chip, const uint32_t challenges[15], CParams& p) {
+    if (!p.n) return 0;
+    VG_TRY(vg_build_devchip(ctx, chip, challenges, &p.chip));
+    KScope ks(ctx, KC_CHECK, 4.0 * (double)p.n * (double)(chip->width + chip->preprocessed_width + 5.0 * (chip->n_interactions + 1)));
+    air::with_chip(chip->chip_id, [&](auto c) { check_kernel<decltype(c)::value><<<(unsigned)((p.n + 127) / 128), 128, 0, ctx->stream>>>(p); });
+    VG_LAUNCH_CHECK(ctx);
+    return 0;
+}
+
+}  // namespace
+
+// Validates the arguments (before anything is enqueued) and enqueues the sweep of one chip's whole traces.  d_first / d_count must
+// hold ~0 / 0.
+int32_t vg_check_enqueue(vgpu_ctx* ctx, const vgpu_chip_desc* chip, const vgpu_dmat* main, const vgpu_dmat* prep, const vgpu_dmat* perm,
+                         const uint32_t challenges[15], unsigned long long* d_first, unsigned long long* d_count) {
+    if (!chip || !main || !perm || !challenges) VG_FAIL(ctx, "check_constraints: null argument");
+    VG_TRY(check_shapes(ctx, chip, main, prep, perm, false));
     VG_TRY(vg_dmat_materialize(ctx, main));
     VG_TRY(vg_dmat_materialize(ctx, prep));
     VG_TRY(vg_dmat_materialize(ctx, perm));
     auto pp = std::make_unique<CParams>();
     CParams& p = *pp;
-    VG_TRY(vg_build_devchip(ctx, chip, challenges, &p.chip));
+    const uint64_t h = main->gh, k = chip->n_interactions;
     p.main = main->d; p.mcs = main->col_stride;
     p.prep = prep ? prep->d : nullptr; p.pcs = prep ? prep->col_stride : 0;
     p.perm = perm->d; p.qcs = perm->col_stride;
-    p.h = h; p.first = d_first; p.count = d_count;
-    KScope ks(ctx, KC_CHECK, 4.0 * (double)h * (double)(main->gw + perm->gw + (prep ? prep->gw : 0)));
-    air::with_chip(chip->chip_id, [&](auto c) { check_kernel<decltype(c)::value><<<(unsigned)((h + 127) / 128), 128, 0, ctx->stream>>>(p); });
-    VG_LAUNCH_CHECK(ctx);
-    return 0;
+    p.cumsum = perm->d + 5 * k * perm->col_stride + h - 1; p.ccs = perm->col_stride;
+    p.g0 = 0; p.n = h; p.h = h; p.wrap = 0;
+    p.first = d_first; p.count = d_count;
+    return enqueue_sweep(ctx, chip, challenges, p);
 }
 
 void vg_check_decode(const unsigned long long first_count[2], int64_t* row, uint32_t* constraint, uint64_t* failing_rows) {
@@ -114,6 +164,147 @@ void vg_check_decode(const unsigned long long first_count[2], int64_t* row, uint
     *constraint = key == ~0ull ? 0 : (uint32_t)(key & 0xff);
     *failing_rows = first_count[1];
 }
+
+void vg_check_reports(const unsigned long long* chk, const uint32_t cumsum[VGPU_NUM_CHIPS][5], vgpu_check_report out[VGPU_NUM_CHIPS]) {
+    for (int i = 0; i < VGPU_NUM_CHIPS; i++) {
+        const unsigned long long fc[2] = {chk[i], chk[VGPU_NUM_CHIPS + i]};
+        vg_check_decode(fc, &out[i].first_row, &out[i].first_constraint, &out[i].failing_rows);
+        for (int l = 0; l < 5; l++) out[i].cumulative_sum[l] = cumsum[i][l];
+    }
+}
+
+bool vg_sums_cancel(const uint32_t cumsum[VGPU_NUM_CHIPS][5]) {
+    for (int l = 0; l < 5; l++) {
+        uint64_t s = 0;
+        for (int i = 0; i < VGPU_NUM_CHIPS; i++) s += cumsum[i][l];
+        if (s % bb::P) return false;
+    }
+    return true;
+}
+
+// The check of n chips on this rank of a split context (or of a lone one, where every chip is whole and nothing crosses ranks).
+// Per chip, sweep() enqueues the run's rows (all but the last when the chip is split) and packs the split chip's boundary words;
+// finish() then makes ONE all-gather of every split chip's block, sweeps the windows, and makes ONE all-gather of the verdicts.
+// Every rank plans from global heights alone, so all ranks make the same collectives.
+namespace {
+class CheckSet {
+  public:
+    CheckSet(vgpu_ctx* ctx, uint32_t n) : ctx_(ctx), n_(n), chips_(n), block_(ctx), win_(ctx), verdicts_(ctx) {}
+
+    // the layout, from the chips and their global heights (before any sweep)
+    void plan(uint32_t i, const vgpu_chip_desc* chip, uint64_t h) {
+        Chip& c = chips_[i];
+        c.desc = chip; c.run = vg_trace_run(ctx_, h); c.h = h;
+        c.wm = chip->width; c.wp = chip->preprocessed_width; c.wq = 5 * (chip->n_interactions + 1);
+        if (c.run.split) {
+            c.at = words_; words_ += c.wm + c.wp + c.wq + 5;
+            c.win_at = win_words_; win_words_ += 2 * (c.wm + c.wp + c.wq);
+            any_split_ = true;
+        }
+    }
+    int32_t alloc() {
+        const uint32_t N = any_split_ ? (uint32_t)ctx_->comm_size : 1;
+        if (words_) VG_TRY(block_.alloc((size_t)N * words_ * 4));
+        if (win_words_) VG_TRY(win_.alloc(win_words_ * 4));
+        VG_TRY(verdicts_.alloc((size_t)N * 2 * n_ * sizeof(unsigned long long)));
+        unsigned long long* mine = own_verdicts();
+        VG_CUDA(ctx_, cudaMemsetAsync(mine, 0xff, n_ * sizeof(unsigned long long), ctx_->stream));
+        VG_CUDA(ctx_, cudaMemsetAsync(mine + n_, 0, n_ * sizeof(unsigned long long), ctx_->stream));
+        return 0;
+    }
+    // Enqueues chip i's sweep of this rank's run (arguments validated); what it reads of perm is read before later work on the stream.
+    int32_t sweep(uint32_t i, const vgpu_dmat* main, const vgpu_dmat* prep, const vgpu_dmat* perm, const uint32_t challenges[15]) {
+        Chip& c = chips_[i];
+        VG_TRY(vg_dmat_materialize(ctx_, main));
+        VG_TRY(vg_dmat_materialize(ctx_, prep));
+        VG_TRY(vg_dmat_materialize(ctx_, perm));
+        const uint64_t row0 = c.run.begin, cnt = c.run.count, k = c.desc->n_interactions;
+        // first row of the run: a shard starts there, a whole trace is entered at row0 (perm.cu's rule)
+        auto rows_of = [&](const vgpu_dmat* m) -> const uint32_t* { return m ? m->d + (m->dist == VG_ROWS ? 0 : row0) : nullptr; };
+        const uint32_t *md = rows_of(main), *pd = rows_of(prep), *qd = rows_of(perm);
+        const uint64_t mcs = main->col_stride, pcs = prep ? prep->col_stride : 0, qcs = perm->col_stride;
+        auto pp = std::make_unique<CParams>();
+        CParams& p = *pp;
+        p.main = md; p.mcs = mcs; p.prep = pd; p.pcs = pcs; p.perm = qd; p.qcs = qcs;
+        // the running sum of the run's last row: the cumulative sum when the run ends the trace; otherwise read by no swept row
+        p.cumsum = qd + 5 * k * qcs + cnt - 1; p.ccs = qcs;
+        p.g0 = row0; p.h = c.h;
+        p.n = c.run.split ? cnt - 1 : cnt;
+        p.wrap = c.run.split ? p.n : 0;
+        p.first = own_verdicts() + i; p.count = own_verdicts() + n_ + i;
+        VG_TRY(enqueue_sweep(ctx_, c.desc, challenges, p));
+        if (!c.run.split) return 0;
+        // the block this rank sends (first rows, last running sum) and the window's row 0 (this rank's last row)
+        uint32_t* blk = block_.as<uint32_t>() + (uint64_t)ctx_->comm_rank * words_ + c.at;
+        uint32_t* win = win_.as<uint32_t>() + c.win_at;
+        CopyList l{};
+        l.s[0] = {md, mcs, blk, 1, c.wm};
+        l.s[1] = {pd, pcs, blk + c.wm, 1, pd ? c.wp : 0};
+        l.s[2] = {qd, qcs, blk + c.wm + c.wp, 1, c.wq};
+        l.s[3] = {qd + 5 * k * qcs + cnt - 1, qcs, blk + c.wm + c.wp + c.wq, 1, 5};
+        l.s[4] = {md + cnt - 1, mcs, win, 2, c.wm};
+        l.s[5] = {pd ? pd + cnt - 1 : nullptr, pcs, win + 2 * c.wm, 2, pd ? c.wp : 0};
+        l.s[6] = {qd + cnt - 1, qcs, win + 2 * (c.wm + c.wp), 2, c.wq};
+        return copy_segments(ctx_, l, 7);
+    }
+    // The exchange of the boundary blocks, the window sweeps and the exchange of the verdicts.
+    int32_t finish(const uint32_t challenges[15]) {
+        if (!any_split_) return 0;
+        const uint32_t N = (uint32_t)ctx_->comm_size, next = ((uint32_t)ctx_->comm_rank + 1) % N;
+        VG_TRY(vg_comm_allgather_inplace(ctx_, block_.as<uint32_t>(), words_));
+        for (uint32_t i = 0; i < n_; i++) {
+            Chip& c = chips_[i];
+            if (!c.run.split) continue;
+            const uint32_t* nb = block_.as<uint32_t>() + (uint64_t)next * words_ + c.at;
+            uint32_t* win = win_.as<uint32_t>() + c.win_at;
+            CopyList l{};
+            l.s[0] = {nb, 1, win + 1, 2, c.wm};
+            l.s[1] = {nb + c.wm, 1, win + 2 * c.wm + 1, 2, c.wp};
+            l.s[2] = {nb + c.wm + c.wp, 1, win + 2 * (c.wm + c.wp) + 1, 2, c.wq};
+            VG_TRY(copy_segments(ctx_, l, 3));
+            auto pp = std::make_unique<CParams>();
+            CParams& p = *pp;
+            p.main = win; p.mcs = 2;
+            p.prep = c.wp ? win + 2 * c.wm : nullptr; p.pcs = 2;
+            p.perm = win + 2 * (c.wm + c.wp); p.qcs = 2;
+            p.cumsum = block_.as<uint32_t>() + (uint64_t)(N - 1) * words_ + c.at + c.wm + c.wp + c.wq; p.ccs = 1;   // the last rank's
+            p.g0 = c.run.begin + c.run.count - 1; p.n = 1; p.h = c.h; p.wrap = 1;
+            p.first = own_verdicts() + i; p.count = own_verdicts() + n_ + i;
+            VG_TRY(enqueue_sweep(ctx_, c.desc, challenges, p));
+        }
+        return vg_comm_allgather_inplace(ctx_, (uint32_t*)verdicts_.p, 4 * (uint64_t)n_);
+    }
+    // every rank's verdicts, as finish() left them on the device
+    const void* verdicts() const { return verdicts_.p; }
+    size_t verdict_bytes() const { return (any_split_ ? (size_t)ctx_->comm_size : 1) * 2 * n_ * sizeof(unsigned long long); }
+    // all: verdict_bytes() copied to the host -> out: [first keys n | failing-row counts n].  A split chip's rows are spread over the
+    // ranks (min of the keys, sum of the counts); any other chip was swept whole by every rank and counts once, as rank 0 reports it.
+    void reduce(const unsigned long long* all, unsigned long long* out) const {
+        const uint32_t N = any_split_ ? (uint32_t)ctx_->comm_size : 1;
+        for (uint32_t i = 0; i < n_; i++) {
+            unsigned long long key = all[i], cnt = all[n_ + i];
+            for (uint32_t r = 1; chips_[i].run.split && r < N; r++) {
+                key = std::min(key, all[(size_t)r * 2 * n_ + i]);
+                cnt += all[(size_t)r * 2 * n_ + n_ + i];
+            }
+            out[i] = key; out[n_ + i] = cnt;
+        }
+    }
+
+  private:
+    struct Chip { const vgpu_chip_desc* desc = nullptr; VgRun run{}; uint64_t h = 0, at = 0, win_at = 0; uint32_t wm = 0, wp = 0, wq = 0; };
+    unsigned long long* own_verdicts() const {
+        return (unsigned long long*)verdicts_.p + (any_split_ ? (size_t)ctx_->comm_rank : 0) * 2 * n_;
+    }
+
+    vgpu_ctx* ctx_;
+    uint32_t n_;
+    std::vector<Chip> chips_;
+    uint64_t words_ = 0, win_words_ = 0;     // per-rank block words; window words of this rank
+    bool any_split_ = false;
+    VgBuf block_, win_, verdicts_;
+};
+}  // namespace
 
 extern "C" int32_t vgpu_check_constraints(vgpu_ctx* ctx, const vgpu_chip_desc* chip, const vgpu_dmat* main, const vgpu_dmat* prep_or_null,
                                           const vgpu_dmat* perm, const uint32_t challenges[15],
@@ -130,5 +321,72 @@ extern "C" int32_t vgpu_check_constraints(vgpu_ctx* ctx, const vgpu_chip_desc* c
     VG_CUDA(ctx, cudaMemcpyAsync(h, d, sizeof h, cudaMemcpyDeviceToHost, ctx->stream));
     VG_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
     vg_check_decode(h, first_row, first_constraint, failing_rows);
+    return 0;
+}
+
+extern "C" int32_t vgpu_check_constraints_local(vgpu_ctx* ctx, const vgpu_chip_desc* chip, const vgpu_dmat* main, const vgpu_dmat* prep_or_null,
+                                                const vgpu_dmat* perm, const uint32_t challenges[15],
+                                                int64_t* first_row, uint32_t* first_constraint, uint64_t* failing_rows) {
+    if (!first_row || !first_constraint || !failing_rows) VG_FAIL(ctx, "check_constraints_local: null output");
+    if (!chip || !main || !perm || !challenges) VG_FAIL(ctx, "check_constraints_local: null argument");
+    VG_TRY(check_shapes(ctx, chip, main, prep_or_null, perm, true));
+    if (!vg_sharded(ctx)) return vgpu_check_constraints(ctx, chip, main, prep_or_null, perm, challenges, first_row, first_constraint, failing_rows);
+    VG_TRY(vg_enter(ctx));
+    CheckSet set(ctx, 1);
+    set.plan(0, chip, main->gh);
+    VG_TRY(set.alloc());
+    VG_TRY(set.sweep(0, main, prep_or_null, perm, challenges));
+    VG_TRY(set.finish(challenges));
+    std::vector<unsigned long long> all(set.verdict_bytes() / sizeof(unsigned long long));
+    VG_CUDA(ctx, cudaMemcpyAsync(all.data(), set.verdicts(), set.verdict_bytes(), cudaMemcpyDeviceToHost, ctx->stream));
+    VG_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
+    unsigned long long fc[2];
+    set.reduce(all.data(), fc);
+    vg_check_decode(fc, first_row, first_constraint, failing_rows);
+    return 0;
+}
+
+extern "C" int32_t vgpu_check_witness(vgpu_ctx* ctx, const vgpu_dmat* const main[VGPU_NUM_CHIPS], const vgpu_dmat* const prep[2],
+                                      const uint32_t challenges[15], vgpu_check_report report[VGPU_NUM_CHIPS], int32_t* sums_cancel) {
+    if (!main || !prep || !challenges || !report || !sums_cancel) VG_FAIL(ctx, "check_witness: null argument");
+    const vgpu_chip_desc* chips[VGPU_NUM_CHIPS];
+    auto prep_for = [&](int i) -> const vgpu_dmat* { return i == 1 ? prep[0] : i == 12 ? prep[1] : nullptr; };
+    for (int i = 0; i < VGPU_NUM_CHIPS; i++) {
+        chips[i] = vgpu_basic_machine_chip(i);
+        if (!main[i]) VG_FAIL(ctx, "check_witness: chip %d has no trace", i);
+        VG_TRY(check_shapes(ctx, chips[i], main[i], prep_for(i), nullptr, true));
+    }
+    VG_TRY(vg_enter(ctx));
+    CheckSet set(ctx, VGPU_NUM_CHIPS);
+    for (int i = 0; i < VGPU_NUM_CHIPS; i++) set.plan(i, chips[i], main[i]->gh);
+    VG_TRY(set.alloc());
+    const uint32_t slots = vg_perm_totals_ranks(ctx);
+    const size_t tot_words = (size_t)VGPU_NUM_CHIPS * slots * 5, tot_at = (set.verdict_bytes() + 3) / 4;
+    VgBuf res(ctx);                                   // the verdicts, then the LogUp totals: one copy back
+    VG_TRY(res.alloc((tot_at + tot_words) * 4));
+    uint32_t* d_tot = res.as<uint32_t>() + tot_at;
+    uint32_t nt[VGPU_NUM_CHIPS];
+    for (int i = 0; i < VGPU_NUM_CHIPS; i++) {
+        vgpu_dmat* pm = nullptr;
+        VG_TRY(vg_perm_trace_enqueue(ctx, chips[i], main[i], prep_for(i), challenges, &pm, d_tot + (size_t)i * slots * 5, &nt[i]));
+        VgMat perm(pm);                               // back to the cache once the sweep that reads it is enqueued
+        VG_TRY(set.sweep(i, main[i], prep_for(i), perm.get(), challenges));
+    }
+    VG_TRY(set.finish(challenges));
+    VG_CUDA(ctx, cudaMemcpyAsync(res.p, set.verdicts(), set.verdict_bytes(), cudaMemcpyDeviceToDevice, ctx->stream));
+    std::vector<uint32_t> host(tot_at + tot_words);
+    VG_CUDA(ctx, cudaMemcpyAsync(host.data(), res.p, host.size() * 4, cudaMemcpyDeviceToHost, ctx->stream));
+    VG_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
+    unsigned long long chk[2 * VGPU_NUM_CHIPS];
+    set.reduce((const unsigned long long*)host.data(), chk);
+    uint32_t cumsum[VGPU_NUM_CHIPS][5];
+    for (int i = 0; i < VGPU_NUM_CHIPS; i++)
+        for (int l = 0; l < 5; l++) {
+            uint32_t a = 0;
+            for (uint32_t r = 0; r < nt[i]; r++) a = bb::add(a, host[tot_at + ((size_t)i * slots + r) * 5 + l]);
+            cumsum[i][l] = bb::from_monty(a);
+        }
+    vg_check_reports(chk, cumsum, report);
+    *sums_cancel = vg_sums_cancel(cumsum) ? 1 : 0;
     return 0;
 }

@@ -32,3 +32,7 @@ uint32_t vg_perm_totals_ranks(const vgpu_ctx* ctx);
 int32_t vg_check_enqueue(vgpu_ctx* ctx, const vgpu_chip_desc* chip, const vgpu_dmat* main, const vgpu_dmat* prep_or_null, const vgpu_dmat* perm,
                          const uint32_t challenges[15], unsigned long long* d_first, unsigned long long* d_count);
 void vg_check_decode(const unsigned long long first_count[2], int64_t* row, uint32_t* constraint, uint64_t* failing_rows);
+// the 14 chips' verdicts (first keys [14], then failing-row counts [14]) and canonical cumulative sums -> reports
+void vg_check_reports(const unsigned long long* chk, const uint32_t cumsum[VGPU_NUM_CHIPS][5], vgpu_check_report out[VGPU_NUM_CHIPS]);
+// check_cumulative_sums (machine/src/check_constraints.rs:87-93): the canonical sums of the 14 chips add to zero
+bool vg_sums_cancel(const uint32_t cumsum[VGPU_NUM_CHIPS][5]);

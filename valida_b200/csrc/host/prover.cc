@@ -332,23 +332,17 @@ int32_t debug_mode_allowed(vgpu_ctx* ctx) {
 // (machine/src/check_constraints.rs:87-93): an error naming every failure, or 0.
 int32_t debug_verdict(vgpu_ctx* ctx, const unsigned long long* chk, const uint32_t cumsum[VGPU_NUM_CHIPS][5]) {
     static const char* NAMES[VGPU_NUM_CHIPS] = {"cpu", "program", "mem", "add", "sub", "mul", "div", "shift", "lt", "com", "bitwise", "output", "range", "static_data"};
+    vgpu_check_report rep[VGPU_NUM_CHIPS];
+    vg_check_reports(chk, cumsum, rep);
     std::string msg;
     for (int i = 0; i < VGPU_NUM_CHIPS; i++) {
-        const unsigned long long fc[2] = {chk[i], chk[VGPU_NUM_CHIPS + i]};
-        int64_t row; uint32_t c; uint64_t n;
-        vg_check_decode(fc, &row, &c, &n);
-        if (row < 0) continue;
+        if (rep[i].first_row < 0) continue;
         char b[160];
-        snprintf(b, sizeof b, "chip %d (%s): constraint %u does not vanish on row %lld (%llu rows fail)", i, NAMES[i], c, (long long)row, (unsigned long long)n);
+        snprintf(b, sizeof b, "chip %d (%s): constraint %u does not vanish on row %lld (%llu rows fail)", i, NAMES[i], rep[i].first_constraint,
+                 (long long)rep[i].first_row, (unsigned long long)rep[i].failing_rows);
         msg += (msg.empty() ? "" : "; ") + std::string(b);
     }
-    bool cancel = true;
-    for (int l = 0; l < 5; l++) {
-        uint64_t s = 0;
-        for (int i = 0; i < VGPU_NUM_CHIPS; i++) s += cumsum[i][l];
-        cancel = cancel && s % bb::P == 0;
-    }
-    if (!cancel) msg += (msg.empty() ? "" : "; ") + std::string("cumulative sums do not cancel");
+    if (!vg_sums_cancel(cumsum)) msg += (msg.empty() ? "" : "; ") + std::string("cumulative sums do not cancel");
     if (msg.empty()) return 0;
     ctx->err = "prove: debug checks failed: " + msg;
     return -1;
