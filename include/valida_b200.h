@@ -297,16 +297,19 @@ uint32_t vgpu_last_prove_phases(const vgpu_ctx* ctx, const char** names, float* 
  * pointers; what a torchrun launch uses) or a thread per rank inside one process (vgpu_comm_init_local; what a Rust host
  * with a worker thread per GPU uses; several ranks may share a device).  After either, every rank must make the SAME
  * sequence of library calls with the same arguments, each rank from its own thread / process.
- * Data path with sharding on (the default after init): a trace tall enough (LDE height >= 4096 * nranks) is held as
+ * Which rows a rank holds (vgpu_row_share): nranks is 1..16; with P the next power of two >= nranks, a matrix of n rows is split
+ * when n >= 4096 * P, cut into 8 * P units of n / (8 P) rows, and rank r holds units [floor(8 P r / nranks), floor(8 P (r + 1) / nranks))
+ * — rows [r n / nranks, (r + 1) n / nranks) at a power-of-two nranks, runs that differ by at most one unit otherwise.
+ * Data path with sharding on (the default after init): a trace tall enough (LDE height >= 4096 * P) is held as
  * contiguous ROW shards (vgpu_dmat_upload_rows, vgpu_prove); a commit (1) hands every column to the rank that extends it,
  * (2) extends the column shares (coset LDE) and stores each rank's contiguous run of the committed (bit-reversed) rows into
  * that rank's shard — kernels storing through peer pointers over NVLink, the ONE bulk exchange of a commit — and (3) hashes
- * leaves and builds the sub-tree of its own rows; the nranks x 32-byte sub-roots are all-gathered and the top log2(nranks)
- * layers computed by every rank.  LogUp traces, the quotient sweep (its "next" rows are one peer's shard, read over
- * NVLink), inverse denominators, reduced openings and the FRI folds / layer trees work on a rank's own rows; what crosses
- * ranks afterwards are per-rank partial sums, sub-roots and the 40 opened rows.  Shorter matrices are computed whole by
- * every rank.  Roots and proof bytes are identical on all ranks and identical to the single-GPU ones.
- * nranks must be a power of two (<= 16). */
+ * leaves and builds the sub-tree of its own rows; the last tree layer in which every run is whole nodes (the nranks sub-roots
+ * at a power-of-two nranks, the 8 * P-node layer otherwise) is all-gathered and the layers above it computed by every rank.
+ * LogUp traces, the quotient sweep (the "next" rows of each unit are one rank's, read over NVLink), inverse denominators,
+ * reduced openings and the FRI folds / layer trees work on a rank's own rows; what crosses ranks afterwards are per-rank
+ * partial sums, the gathered tree layer and the 40 opened rows.  Shorter matrices are computed whole by every rank.  Roots and
+ * proof bytes are identical on all ranks and identical to the single-GPU ones. */
 #define VGPU_COMM_ID_BYTES 128
 int32_t vgpu_comm_unique_id(uint8_t out[VGPU_COMM_ID_BYTES]);                 /* rank 0 creates, the caller distributes */
 int32_t vgpu_comm_init(vgpu_ctx* ctx, int32_t nranks, int32_t rank, const uint8_t unique_id[VGPU_COMM_ID_BYTES]);
@@ -319,6 +322,8 @@ void vgpu_shard_range(uint64_t total, int32_t nranks, int32_t rank, uint64_t* be
  * water-filling over the whole commit (tallest first, a column of height h weighs h).  begin_out: n rows of nranks + 1 first-column indices. */
 void vgpu_split_column_plan(int32_t nranks, uint32_t n, const uint64_t* heights, const uint64_t* widths, uint32_t* begin_out);
 void vgpu_tree_share(uint64_t len, int32_t nranks, int32_t rank, uint64_t* begin, uint64_t* count, int32_t* split); /* ... for tree layers */
+/* The run of a matrix / vector of n stored rows that rank `rank` holds (the rule above); *split = 0: every rank holds all of it. */
+void vgpu_row_share(uint64_t n, int32_t nranks, int32_t rank, uint64_t* begin, uint64_t* count, int32_t* split);
 
 /* ---- Machine::verify (machine/src/machine.rs:26-31; body derive/src/lib.rs:492-650) ------------------
  * Checks a CBOR MachineProof (this library's or the reference's) against the preprocessed traces: the

@@ -187,6 +187,7 @@ extern "C" {
     pub fn vgpu_shard_range(total: u64, nranks: i32, rank: i32, begin: *mut u64, end: *mut u64);
     pub fn vgpu_split_column_plan(nranks: i32, n: u32, heights: *const u64, widths: *const u64, begin_out: *mut u32);
     pub fn vgpu_tree_share(len: u64, nranks: i32, rank: i32, begin: *mut u64, count: *mut u64, split: *mut i32);
+    pub fn vgpu_row_share(n: u64, nranks: i32, rank: i32, begin: *mut u64, count: *mut u64, split: *mut i32);
 
     // ---- Machine::verify ----
     pub fn vgpu_verify(ctx: *mut vgpu_ctx, proof: *const u8, proof_len: u64, prep: *const vgpu_matrix, repr: i32, verdict: *mut i32) -> i32;

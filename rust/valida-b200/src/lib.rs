@@ -431,7 +431,8 @@ impl Drop for Context {
 
 /// ONE proof split across the GPUs of a box: a context per device, a worker thread per context.  Every rank makes the same
 /// call with the same traces and copies only its rows of the tall ones; the proof bytes are identical on all ranks and
-/// identical to the single-GPU proof.  The number of ranks must be a power of two (<= 16).
+/// identical to the single-GPU proof.  The number of ranks is 1..=16; at a count that is not a power
+/// of two the ranks' row runs differ by at most one of 8 P units (P: the next power of two).
 pub struct LocalGroup {
     ranks: Vec<Context>,
 }

@@ -39,4 +39,5 @@ from .api import (  # noqa: F401
     shard_range,
     split_column_plan,
     tree_share,
+    row_share,
 )

@@ -103,6 +103,7 @@ def _load():
         "vgpu_shard_range": (None, [u64, C.c_int32, C.c_int32, C.POINTER(u64), C.POINTER(u64)]),
         "vgpu_split_column_plan": (None, [C.c_int32, C.c_uint32, C.POINTER(u64), C.POINTER(u64), u32p]),
         "vgpu_tree_share": (None, [u64, C.c_int32, C.c_int32, C.POINTER(u64), C.POINTER(u64), C.POINTER(C.c_int32)]),
+        "vgpu_row_share": (None, [u64, C.c_int32, C.c_int32, C.POINTER(u64), C.POINTER(u64), C.POINTER(C.c_int32)]),
         "vgpu_open": (C.c_int32, [vp, C.POINTER(vp), C.c_uint32, u32p, u32p, C.POINTER(C.POINTER(C.c_uint8)), C.POINTER(u64)]),
         "vgpu_verify": (C.c_int32, [vp, C.c_char_p, u64, C.POINTER(_Matrix), C.c_int32, C.POINTER(C.c_int32)]),
         "vgpu_prove": (C.c_int32, [vp, C.POINTER(_Matrix), C.POINTER(_Matrix), C.c_int32, C.POINTER(C.POINTER(C.c_uint8)), C.POINTER(u64)]),
@@ -718,9 +719,18 @@ def split_column_plan(world_size, shapes):
 
 
 def tree_share(length, world_size, rank):
-    """(begin, count, split) — the part of a tree layer a rank derives itself when commits are split."""
+    """(begin, count, split) — the part of a tree layer a rank derives itself when commits are split (any world_size 1..16)."""
     b, c, sp = C.c_uint64(), C.c_uint64(), C.c_int32()
     lib().vgpu_tree_share(length, world_size, rank, C.byref(b), C.byref(c), C.byref(sp))
+    return int(b.value), int(c.value), bool(sp.value)
+
+
+def row_share(length, world_size, rank):
+    """(begin, count, split) — the run of a matrix / vector of `length` stored rows a rank holds in a split proof of world_size
+    (1..16) ranks: with P the next power of two >= world_size, a length >= 4096 P is cut into 8 P units and rank r holds units
+    [r * 8P // world_size, (r + 1) * 8P // world_size); a shorter one is held whole by every rank (split False)."""
+    b, c, sp = C.c_uint64(), C.c_uint64(), C.c_int32()
+    lib().vgpu_row_share(length, world_size, rank, C.byref(b), C.byref(c), C.byref(sp))
     return int(b.value), int(c.value), bool(sp.value)
 
 

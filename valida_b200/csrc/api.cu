@@ -47,8 +47,9 @@ int32_t vg_dmat_alloc_run(vgpu_ctx* ctx, uint64_t gh, uint64_t gw, bool split, b
     if (!m) VG_FAIL(ctx, "out of host memory");
     const VgRun run = vg_run(gh, ctx->comm_size, ctx->comm_rank, split);
     m->ctx = ctx; m->gh = gh; m->gw = gw; m->dist = split ? VG_ROWS : VG_FULL; m->owns = true; m->symm = symm;
-    m->h = m->col_stride = run.count; m->w = gw; m->row0 = run.begin;
-    const size_t bytes = m->h * m->w * 4;
+    m->h = run.count; m->w = gw; m->row0 = run.begin;
+    m->col_stride = symm && split ? vg_run_max(gh, ctx->comm_size) : run.count;
+    const size_t bytes = m->col_stride * m->w * 4;
     int32_t rc = symm ? vg_symm_alloc(ctx, (void**)&m->d, bytes) : vg_alloc(ctx, (void**)&m->d, bytes);
     if (rc) { delete m; return rc; }
     out->reset(m);
@@ -462,7 +463,7 @@ static std::vector<ColPlan> plan_columns(const int G, const std::vector<std::pai
 static size_t commit_symm_bytes(int G, const std::vector<std::pair<uint64_t, uint64_t>>& dims, const std::vector<ColPlan>& plan, const std::vector<bool>& as_rows) {
     size_t need = 0;
     for (size_t k = 0; k < dims.size(); k++) {
-        need += vg_symm_round((2 * dims[k].first / (uint64_t)G) * dims[k].second * 4);
+        need += vg_symm_round(vg_run_max(2 * dims[k].first, (uint64_t)G) * dims[k].second * 4);
         if (as_rows[k]) need += vg_symm_round(dims[k].first * plan[k].widest * 4);
     }
     return need;
@@ -486,7 +487,7 @@ void vgpu_split_column_plan(int32_t nranks, uint32_t n, const uint64_t* heights,
 
 // Split proof: the tall matrices of a commit.  (1) a matrix that arrives as row shards is handed to the ranks that extend
 // its columns; (2) every rank extends its column share and stores, through peer pointers, each rank's run of the committed
-// rows into that rank's shard.  After the closing barrier pd->ldes[i] holds rows [rank * H/G, (rank+1) * H/G) of all columns.
+// rows into that rank's shard.  After the closing barrier pd->ldes[i] holds this rank's run of the H committed rows of all columns.
 static int32_t extend_split(vgpu_ctx* ctx, vgpu_prover_data* pd, const vgpu_dmat* const* mats, const std::vector<size_t>& tall, const uint32_t* coset_shifts_or_null) {
     std::vector<std::pair<uint64_t, uint64_t>> dims;
     std::vector<bool> as_rows;

@@ -183,29 +183,63 @@ int32_t vg_get_shift_table(vgpu_ctx* ctx, uint32_t shift_canonical, uint32_t sca
 inline bool vg_sharded(const vgpu_ctx* ctx) { return ctx->sharding && ctx->comm_size > 1; }
 // Which rows each rank of a split proof holds.  Every rank must reach the same answer at every allocation, upload, sweep and query
 // answer (or the proof hangs at a barrier or comes out wrong), so this is the one place that decides it.
-// A run of stored rows: this rank holds [begin, begin + count) of them; split = they are cut into one equal run per rank.
+// The rule, for N = nranks ranks (1..16): with P = 2^ceil(log2 N), a split vector of n stored rows is cut into V = 8 P units of
+// n / V rows, and rank r holds the contiguous units [floor(r V / N), floor((r + 1) V / N)).  At a power of two N that is rows
+// [r n / N, (r + 1) n / N); otherwise the runs differ by at most one unit (N = 3: 10 / 11 / 11 of 32 units).
+constexpr int VG_MAX_RANKS = 16;
+inline uint64_t vg_units(uint64_t nranks) { uint64_t p = 1; while (p < nranks) p <<= 1; return 8 * p; }
+// first unit of `rank` (rank == nranks: V)
+inline uint64_t vg_unit_begin(uint64_t nranks, uint64_t rank) { return rank * vg_units(nranks) / nranks; }
+// A run of stored rows: this rank holds [begin, begin + count) of them; split = they are cut into one run of units per rank.
 struct VgRun { uint64_t begin, count; bool split; };
-inline VgRun vg_run(uint64_t n, uint64_t nranks, uint64_t rank, bool split) {
+// rank d's run of a split vector of n rows begins at row vg_run_bound(n, N, d) (d = N: n); exact whenever the split rules below
+// split n (V divides n, or n is a layer whose run boundaries fall on whole nodes)
+inline uint64_t vg_run_bound(uint64_t n, uint64_t nranks, uint64_t rank) { return vg_unit_begin(nranks, rank) * n / vg_units(nranks); }
+// At a power-of-two nranks the units of a rank are rows [rank n / nranks, (rank + 1) n / nranks): the even split, computed as such.
+inline VgRun vg_run_even(uint64_t n, uint64_t nranks, uint64_t rank, bool split) {
     return split ? VgRun{rank * (n / nranks), n / nranks, true} : VgRun{0, n, false};
 }
-// A matrix / vector of `n` stored rows is cut into comm_size contiguous row shards when every shard keeps >= 4096 rows;
-// shorter ones are replicated (every rank computes and holds all of them).
+inline VgRun vg_run(uint64_t n, uint64_t nranks, uint64_t rank, bool split) {
+    if (!split || !(nranks & (nranks - 1))) return vg_run_even(n, nranks, rank, split);
+    const uint64_t b = vg_run_bound(n, nranks, rank);
+    return VgRun{b, vg_run_bound(n, nranks, rank + 1) - b, true};
+}
+// the longest run of any rank: what a symmetric-heap shard is sized for on every rank (the heap's offsets must match)
+inline uint64_t vg_run_max(uint64_t n, uint64_t nranks) {
+    uint64_t m = 0;
+    for (uint64_t d = 0; d < nranks; d++) m = std::max(m, vg_run_bound(n, nranks, d + 1) - vg_run_bound(n, nranks, d));
+    return m;
+}
+// A matrix / vector of `n` stored rows is cut into runs when n >= 4096 P (a unit keeps >= 512 rows, so a rank's run is whole
+// 256-leaf sub-trees and whole FRI leaf pairs); shorter ones are replicated (every rank computes and holds all of them).  Stored
+// heights are powers of two, and for those n >= 4096 N is the same test (4096 P is the least power of two >= 4096 N).
+inline bool vg_split_rows_n(uint64_t n, int nranks) { return nranks > 1 && n >= (uint64_t)nranks * 4096; }
 inline bool vg_split_rows(const vgpu_ctx* ctx, uint64_t n) { return vg_sharded(ctx) && n >= (uint64_t)ctx->comm_size * 4096; }
 inline VgRun vg_row_run(const vgpu_ctx* ctx, uint64_t n) { return vg_run(n, ctx->comm_size, ctx->comm_rank, vg_split_rows(ctx, n)); }
-// A trace of h rows is split when its LDE of 2h rows is: its rank r holds natural rows [r h / comm_size, (r + 1) h / comm_size).
+// A trace of h rows is split when its LDE of 2h rows is: its rank r holds the natural rows of its units of h.
 inline VgRun vg_trace_run(const vgpu_ctx* ctx, uint64_t h) { return vg_run(h, ctx->comm_size, ctx->comm_rank, vg_split_rows(ctx, 2 * h)); }
-// A Merkle tree layer of `len` nodes is cut into runs when every one of the nranks > 1 ranks gets a node (merkle.h).
-inline VgRun vg_layer_run(uint64_t len, int nranks, int rank) { return vg_run(len, nranks, rank, nranks > 1 && len >= (uint64_t)nranks); }
+// A Merkle tree layer of `len` nodes is cut into runs while every rank's run is a whole number of nodes (merkle.h): down to the layer
+// of N nodes (the sub-roots) at a power of two N, down to the layer of V nodes otherwise.
+inline bool vg_layer_split(uint64_t len, int nranks) {
+    if (nranks <= 1) return false;
+    for (int d = 1; d < nranks; d++) if (vg_unit_begin(nranks, d) * len % vg_units(nranks)) return false;
+    return true;
+}
+inline VgRun vg_layer_run(uint64_t len, int nranks, int rank) { return vg_run(len, nranks, rank, vg_layer_split(len, nranks)); }
 // A query answer is summed over the ranks, so of data every rank holds only rank 0 reports its words.
 inline bool vg_reports_replicated(const vgpu_ctx* ctx) { return ctx->comm_rank == 0 || !vg_sharded(ctx); }
-// The part of a gh x gw matrix this rank holds: its run of gh / comm_size stored rows when `split` (VG_ROWS), else all of it
-// (VG_FULL).  symm: taken from the symmetric heap (peers store into it).
+// The part of a gh x gw matrix this rank holds: its run of stored rows when `split` (VG_ROWS), else all of it (VG_FULL).
+// symm: taken from the symmetric heap (peers store into it and read it); such a shard has the column stride vg_run_max on every rank,
+// so that every rank's allocation, and a column's place in it, is the same.
 int32_t vg_dmat_alloc_run(vgpu_ctx* ctx, uint64_t gh, uint64_t gw, bool split, bool symm, VgMat* out);
 inline int32_t vg_dmat_alloc(vgpu_ctx* ctx, uint64_t h, uint64_t w, VgMat* out) { return vg_dmat_alloc_run(ctx, h, w, false, false, out); }
 
 // host/comm.cc — every rank calls these in the same order with the same sizes
 // buf holds comm_size consecutive blocks of `words_per_rank` u32; this rank's block is already filled
 int32_t vg_comm_allgather_inplace(vgpu_ctx* ctx, uint32_t* buf, uint64_t words_per_rank);
+// buf holds all n rows (`words` u32 each, row i at buf + i * words) of a vector split by the rule above (vg_run over n); this rank's
+// run is already filled.  Afterwards every row is.  Equal runs (a power of two N) are one vg_comm_allgather_inplace.
+int32_t vg_comm_allgather_runs(vgpu_ctx* ctx, uint32_t* buf, uint64_t n, uint64_t words);
 // stream-ordered barrier: everything enqueued before it on ANY rank's stream completes before anything enqueued after it
 // on any rank's stream starts (peer stores become visible, peer buffers may be reused)
 int32_t vg_comm_barrier(vgpu_ctx* ctx);

@@ -2,7 +2,7 @@
 // THROUGH PEER POINTERS: the data moves over NVLink while the kernel runs, no staging buffer and no collective call.
 //   rows -> columns : a rank holds a contiguous run of rows of a trace (what it uploaded, or what its LogUp / quotient
 //                     sweep produced); every column goes to the rank that extends that column (coset LDE);
-//   columns -> rows : the extended columns are cut into comm_size contiguous runs of the committed (bit-reversed) row
+//   columns -> rows : the extended columns are cut into the ranks' runs (ctx.h) of the committed (bit-reversed) row
 //                     order and every run goes to the rank that owns those rows from then on (leaf hashing, sub-tree,
 //                     quotient sweep, openings, FRI) — the ONE bulk exchange of a commit.
 // Both are followed by vg_comm_barrier() (stream-ordered) before anybody reads what it received.
@@ -45,16 +45,17 @@ __global__ void __launch_bounds__(256) rows_to_cols_scalar_kernel(const __grid_c
 }
 
 struct C2RParams {
-    const uint32_t* src; uint64_t H, hs;        // local columns [c0, c1) at stride H; shard height hs = H / nranks
-    uint32_t* dst[MAX_RANKS];                   // peer d's shard matrix (hs x w, stride hs)
+    const uint32_t* src; uint64_t H, cs;        // local columns [c0, c1) at stride H; cs: the shards' column stride (the same on every rank)
+    uint32_t* dst[MAX_RANKS];                   // peer d's shard matrix (rows [rb[d], rb[d + 1]) x w, stride cs)
+    uint64_t rb[MAX_RANKS + 1];                 // the run table: rank d holds committed rows [rb[d], rb[d + 1])
     uint32_t c0, nranks;
 };
 // grid: x = 16-byte chunks of a shard column, y = local column, z = destination rank
 __global__ void __launch_bounds__(256) cols_to_rows_kernel(const __grid_constant__ C2RParams p) {
     const uint32_t lc = blockIdx.y, d = blockIdx.z;
-    const uint64_t n4 = p.hs >> 2;
-    const uint4* s = reinterpret_cast<const uint4*>(p.src + (uint64_t)lc * p.H + (uint64_t)d * p.hs);
-    uint4* o = reinterpret_cast<uint4*>(p.dst[d] + (uint64_t)(p.c0 + lc) * p.hs);
+    const uint64_t n4 = (p.rb[d + 1] - p.rb[d]) >> 2;
+    const uint4* s = reinterpret_cast<const uint4*>(p.src + (uint64_t)lc * p.H + p.rb[d]);
+    uint4* o = reinterpret_cast<uint4*>(p.dst[d] + (uint64_t)(p.c0 + lc) * p.cs);
     for (uint64_t i = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x; i < n4; i += (uint64_t)gridDim.x * blockDim.x) o[i] = __ldg(s + i);
 }
 
@@ -84,21 +85,23 @@ int32_t vg_exchange_rows_to_cols(vgpu_ctx* ctx, const vgpu_dmat* rows, uint32_t*
 }
 
 // lde_cols: this rank's extended columns [c0, c1) of a matrix of H rows (stride H, committed row order).  shard: the VG_ROWS
-// matrix (H / G rows x gw, symmetric heap) that receives, on every rank, that rank's run of rows of ALL columns.
+// matrix (this rank's run of the H rows x gw, symmetric heap) that receives, on every rank, that rank's run of rows of ALL columns.
 int32_t vg_exchange_cols_to_rows(vgpu_ctx* ctx, const uint32_t* lde_cols, uint64_t H, uint64_t c0, uint64_t c1, vgpu_dmat* shard, cudaStream_t on) {
     const cudaStream_t st = on ? on : ctx->stream;
     const int G = ctx->comm_size;
     if (c1 <= c0) return 0;
-    if (shard->dist != VG_ROWS || !shard->symm || shard->h * (uint64_t)G != H || (shard->h & 3)) VG_FAIL(ctx, "exchange: shard matrix does not match the extended columns");
+    if (shard->dist != VG_ROWS || !shard->symm || shard->gh != H || shard->col_stride != vg_run_max(H, G) || (shard->h & 3))
+        VG_FAIL(ctx, "exchange: shard matrix does not match the extended columns");
     C2RParams p{};
-    p.src = lde_cols; p.H = H; p.hs = shard->h; p.c0 = (uint32_t)c0; p.nranks = (uint32_t)G;
+    p.src = lde_cols; p.H = H; p.cs = shard->col_stride; p.c0 = (uint32_t)c0; p.nranks = (uint32_t)G;
+    for (int d = 0; d <= G; d++) p.rb[d] = vg_run_bound(H, G, d);
     for (int d = 0; d < G; d++) p.dst[d] = vg_peer_ptr(ctx, shard->d, d);
-    const uint64_t n4 = shard->h >> 2;
+    const uint64_t n4 = shard->col_stride >> 2;
     unsigned gx = (unsigned)((n4 + 255) / 256);
     if (gx > 64) gx = 64;
     KScope ks(ctx, KC_EXCHANGE, 8.0 * (double)H * (double)(c1 - c0));
     cols_to_rows_kernel<<<dim3(gx, (unsigned)(c1 - c0), (unsigned)G), 256, 0, st>>>(p);
     VG_LAUNCH_CHECK(ctx);
-    ctx->stat_exchange.calls++; ctx->stat_exchange.bytes += 4.0 * (double)H * (double)(c1 - c0) * (G - 1) / G;
+    ctx->stat_exchange.calls++; ctx->stat_exchange.bytes += 4.0 * (double)(H - shard->h) * (double)(c1 - c0);
     return 0;
 }

@@ -28,6 +28,7 @@ struct Nccl {
     ncclResult_t (*CommDestroy)(ncclComm_t) = nullptr;
     const char* (*GetErrorString)(ncclResult_t) = nullptr;
     ncclResult_t (*AllGather)(const void*, void*, size_t, ncclDataType_t, ncclComm_t, cudaStream_t) = nullptr;
+    ncclResult_t (*Broadcast)(const void*, void*, size_t, ncclDataType_t, int, ncclComm_t, cudaStream_t) = nullptr;
     ncclResult_t (*GroupStart)() = nullptr;
     ncclResult_t (*GroupEnd)() = nullptr;
     std::string why;
@@ -46,6 +47,7 @@ Nccl& nccl() {
         n.CommDestroy = (decltype(n.CommDestroy))sym("ncclCommDestroy");
         n.GetErrorString = (decltype(n.GetErrorString))sym("ncclGetErrorString");
         n.AllGather = (decltype(n.AllGather))sym("ncclAllGather");
+        n.Broadcast = (decltype(n.Broadcast))sym("ncclBroadcast");
         n.GroupStart = (decltype(n.GroupStart))sym("ncclGroupStart");
         n.GroupEnd = (decltype(n.GroupEnd))sym("ncclGroupEnd");
         if (!n.why.empty()) n.lib = nullptr;
@@ -140,6 +142,36 @@ int32_t vg_comm_allgather_inplace(vgpu_ctx* ctx, uint32_t* buf, uint64_t words_p
         VG_CUDA(ctx, cudaMemcpyAsync(buf + (uint64_t)p * words_per_rank, src, words_per_rank * 4, cudaMemcpyDefault, ctx->stream));
     }
     return local_barrier(ctx);                        // nobody reuses its block (or the slot table) before all have read it
+}
+
+// Uneven runs are gathered at their own offsets (no padding): processes broadcast each rank's run in place, in one NCCL group;
+// in-process ranks copy each peer's run from its published buffer.
+int32_t vg_comm_allgather_runs(vgpu_ctx* ctx, uint32_t* buf, uint64_t n, uint64_t words) {
+    const int G = ctx->comm_size;
+    if (G <= 1 || !n || !words) return 0;
+    if (vg_run_max(n, G) * (uint64_t)G == n) return vg_comm_allgather_inplace(ctx, buf, n / G * words);    // equal runs, in rank order
+    const VgRun mine = vg_run(n, G, ctx->comm_rank, true);
+    ctx->stat_allgather.calls++; ctx->stat_allgather.bytes += 4.0 * (double)words * (double)(n - mine.count);
+    KScope ks(ctx, KC_COLLECTIVE, 4.0 * (double)words * (double)(n - mine.count));
+    if (ctx->nccl) {
+        VG_NCCL(ctx, nccl().GroupStart());
+        for (int d = 0; d < G; d++) {
+            const VgRun run = vg_run(n, G, d, true);
+            uint32_t* at = buf + run.begin * words;
+            VG_NCCL(ctx, nccl().Broadcast(at, at, run.count * words, ncclUint32, d, (ncclComm_t)ctx->nccl, ctx->stream));
+        }
+        VG_NCCL(ctx, nccl().GroupEnd());
+        return 0;
+    }
+    VgLocalGroup* g = (VgLocalGroup*)ctx->local_group;
+    g->slot[ctx->comm_rank] = buf;
+    VG_TRY(local_barrier(ctx));                       // every run is written, every pointer published
+    for (int d = 0; d < G; d++) {
+        if (d == ctx->comm_rank) continue;
+        const VgRun run = vg_run(n, G, d, true);
+        VG_CUDA(ctx, cudaMemcpyAsync(buf + run.begin * words, (const uint32_t*)g->slot[d] + run.begin * words, run.count * words * 4, cudaMemcpyDefault, ctx->stream));
+    }
+    return local_barrier(ctx);
 }
 
 // ---- symmetric heap ----------------------------------------------------------------------------------------
@@ -283,7 +315,7 @@ int32_t vgpu_comm_unique_id(uint8_t out[VGPU_COMM_ID_BYTES]) {
 int32_t vgpu_comm_init(vgpu_ctx* ctx, int32_t nranks, int32_t rank, const uint8_t unique_id[VGPU_COMM_ID_BYTES]) {
     if (!ctx) return -1;
     if (nranks < 1 || rank < 0 || rank >= nranks || !unique_id) VG_FAIL(ctx, "comm_init: bad rank %d of %d", rank, nranks);
-    if ((nranks & (nranks - 1)) || nranks > 16) VG_FAIL(ctx, "comm_init: the number of ranks must be a power of two <= 16 (row shards and tree layers are split evenly), got %d", nranks);
+    if (nranks > VG_MAX_RANKS) VG_FAIL(ctx, "comm_init: the number of ranks must be 1..%d, got %d", VG_MAX_RANKS, nranks);
     if (!nccl().lib) VG_FAIL(ctx, "comm_init: %s", nccl().why.c_str());
     vg_comm_free(ctx);
     VG_CUDA(ctx, cudaSetDevice(ctx->device));
@@ -302,7 +334,7 @@ int32_t vgpu_comm_init(vgpu_ctx* ctx, int32_t nranks, int32_t rank, const uint8_
 int32_t vgpu_comm_init_local(vgpu_ctx* const* ctxs, int32_t nranks) {
     if (!ctxs || nranks < 1) return -1;
     vgpu_ctx* c0 = ctxs[0];
-    if ((nranks & (nranks - 1)) || nranks > 16) VG_FAIL(c0, "comm_init_local: the number of ranks must be a power of two <= 16, got %d", nranks);
+    if (nranks > VG_MAX_RANKS) VG_FAIL(c0, "comm_init_local: the number of ranks must be 1..%d, got %d", VG_MAX_RANKS, nranks);
     VgLocalGroup* g = new VgLocalGroup();
     g->n = nranks; g->ctx.assign(ctxs, ctxs + nranks); g->slot.assign(nranks, nullptr); g->refs.store(nranks);
     if (const char* e = getenv("VGPU_COMM_TIMEOUT_S")) g->timeout_s = atoi(e) > 0 ? atoi(e) : g->timeout_s;
@@ -341,9 +373,15 @@ void vgpu_comm_stats(vgpu_ctx* ctx, uint32_t calls[3], double bytes[3], int32_t 
 }
 
 // the share of a tree layer of `len` nodes that rank `rank` derives itself (merkle.cu); *split = 0 when the
-// layer is shorter than the communicator and every rank computes all of it
+// layer is above the last split one and every rank computes all of it
 void vgpu_tree_share(uint64_t len, int32_t nranks, int32_t rank, uint64_t* begin, uint64_t* count, int32_t* split) {
     const VgRun run = vg_layer_run(len, nranks, rank);
+    *begin = run.begin; *count = run.count; *split = run.split;
+}
+// the run of a matrix / vector of `n` stored rows that rank `rank` holds in a split proof of nranks ranks (ctx.h); *split = 0 when
+// it is too short to be split and every rank holds all of it
+void vgpu_row_share(uint64_t n, int32_t nranks, int32_t rank, uint64_t* begin, uint64_t* count, int32_t* split) {
+    const VgRun run = vg_run(n, nranks, rank, vg_split_rows_n(n, nranks));
     *begin = run.begin; *count = run.count; *split = run.split;
 }
 

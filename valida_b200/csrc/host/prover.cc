@@ -188,7 +188,7 @@ int32_t open_multi_batches(vgpu_ctx* ctx, const std::vector<OpenRound>& rounds, 
         VG_TRY(vg_fri_fold(ctx, cur.data(), cur.count, cur.n, i0, cnt, beta, add.d ? add.data() - add.begin : nullptr, add.count, next.data() - next.begin, next.count));
         if (cur.shard() && !next.shard()) {   // every rank folded its run into the whole-length buffer: complete it
             VG_TRY(vg_comm_group_begin(ctx));
-            for (int l = 0; l < 5; l++) VG_TRY(vg_comm_allgather_inplace(ctx, next.data() + (uint64_t)l * next.count, cnt));
+            for (int l = 0; l < 5; l++) VG_TRY(vg_comm_allgather_runs(ctx, next.data() + (uint64_t)l * next.count, next.n, 1));
             VG_TRY(vg_comm_group_end(ctx));
         }
         current = std::move(next);

@@ -13,7 +13,7 @@
 // With VGPU_MERKLE_POSEIDON16 the p16_* kernels take the place of each of these, with the same plan, layout and launches.
 // Digests are stored canonical, 8 words (32 B) per node.  Every layer is computed, but only layers VG_TREE_DROP and up are kept for
 // the opening phase; the lower ones live in a transient block freed when the build returns.  Split proof (merkle.h): a rank
-// computes and keeps its run of every layer — the sub-tree over its rows — and only the layer of comm_size sub-roots is all-gathered.
+// computes and keeps its run of every layer — the sub-tree over its rows — and only the last split layer (merkle.h) is all-gathered.
 #include "ctx.h"
 #include "keccak.cuh"
 #include "merkle.h"
@@ -565,7 +565,8 @@ static std::vector<LayerPlan> plan_tree(const vgpu_ctx* ctx, uint64_t leaves, bo
         const VgRun run = vg_layer_run(len, G, r);
         LayerPlan p{};
         p.len = len; p.cbegin = run.begin; p.ccount = run.count;
-        p.gather = run.split && len == (uint64_t)G;     // the sub-roots: one node per rank, completed by the all-gather
+        // the last split layer (the sub-roots at a power of two G, the V-node layer otherwise), completed by the all-gather
+        p.gather = run.split && (len == 1 || !vg_layer_split(len / 2, G));
         if (run.split && !p.gather) { p.sbegin = p.cbegin; p.scount = p.ccount; } else { p.sbegin = 0; p.scount = len; }
         plan.push_back(p);
         if (len == 1) break;
@@ -642,7 +643,7 @@ static int32_t build_upper_layers(vgpu_ctx* ctx, const std::vector<LayerPlan>& p
     const bool p16 = t->hash == VGPU_MERKLE_POSEIDON16;
     uint32_t* consts = nullptr;
     if (p16) VG_TRY(vg_poseidon_consts(ctx, &consts));
-    if (plan[0].gather) VG_TRY(vg_comm_allgather_inplace(ctx, t->layer_ptr[0], 8));
+    if (plan[0].gather) VG_TRY(vg_comm_allgather_runs(ctx, t->layer_ptr[0], plan[0].len, 8));
     size_t lvl = 1;
     while (lvl < plan.size()) {
         const LayerPlan& p = plan[lvl];
@@ -651,7 +652,9 @@ static int32_t build_upper_layers(vgpu_ctx* ctx, const std::vector<LayerPlan>& p
             // one launch: levels lvl .. lvl + n - 1, each half the one below; stop after a gather layer and at the root
             TailParams tp{};
             tp.prev_v = prev_v; tp.first_begin = p.cbegin;
-            tp.sub = (uint32_t)std::min<uint64_t>(TAIL_SUB, p.ccount);
+            // a CTA's sub-tree starts on a multiple of `sub` nodes: a power of two dividing both ends of the run (an uneven run of
+            // units need not start on a multiple of its length)
+            tp.sub = (uint32_t)std::min<uint64_t>(TAIL_SUB, (p.cbegin | p.ccount) & (~(p.cbegin | p.ccount) + 1));
             uint32_t n = 0;
             uint32_t* inj_at = inject_buf;
             double bytes = 0;
@@ -678,7 +681,7 @@ static int32_t build_upper_layers(vgpu_ctx* ctx, const std::vector<LayerPlan>& p
             }
             VG_LAUNCH_CHECK(ctx);
             lvl += n;
-            if (plan[lvl - 1].gather) VG_TRY(vg_comm_allgather_inplace(ctx, t->layer_ptr[lvl - 1], 8));
+            if (plan[lvl - 1].gather) VG_TRY(vg_comm_allgather_runs(ctx, t->layer_ptr[lvl - 1], plan[lvl - 1].len, 8));
             continue;
         }
         uint32_t* next_v = t->layer_ptr[lvl] - p.sbegin * 8;
@@ -695,7 +698,7 @@ static int32_t build_upper_layers(vgpu_ctx* ctx, const std::vector<LayerPlan>& p
             else compress_layer_kernel<<<(unsigned)((p.ccount + 127) / 128), 128, 0, ctx->stream>>>(prev_v, inj_v, p.cbegin, p.ccount, next_v);
         }
         VG_LAUNCH_CHECK(ctx);
-        if (p.gather) VG_TRY(vg_comm_allgather_inplace(ctx, t->layer_ptr[lvl], 8));
+        if (p.gather) VG_TRY(vg_comm_allgather_runs(ctx, t->layer_ptr[lvl], p.len, 8));
         lvl++;
     }
     return 0;

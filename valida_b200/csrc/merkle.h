@@ -1,8 +1,9 @@
 // <ValMmcs as Mmcs>::ProverData, device resident: committed (bit-reversed) LDE matrices in the
 // caller's order + the digest layers (canonical words, 8 per node).
-// Split proof: a layer of more than comm_size nodes is cut into comm_size contiguous runs and a rank computes and KEEPS
-// only its run (its sub-tree); the layer of exactly comm_size nodes — the sub-roots — is all-gathered (comm_size x 32 bytes,
-// the only collective of a tree) and the layers above it are computed by every rank.
+// Split proof: a layer is cut into the ranks' runs of the row rule (ctx.h) while every run is a whole number of nodes, and a rank
+// computes and KEEPS only its run (its sub-tree); the last such layer is all-gathered (the only collective of a tree) and the layers
+// above it are computed by every rank.  That is the layer of comm_size sub-roots at a power-of-two comm_size, and the layer of
+// V = 8 P nodes, a run of whole units per rank, otherwise.
 // A tree keeps only its layers VG_TREE_DROP and up (only the root for a tree of depth VG_TREE_DROP or less): a query's path below
 // them is rebuilt from the leaves by vg_tree_paths.  The lower layers are the bulk of a tree (2^-VG_TREE_DROP of it is kept), and
 // a proof reads 40 paths from them.
@@ -12,8 +13,8 @@
 #include <functional>
 
 // 8: the kept layers are 1/256 of a tree, and a rebuilt path recomputes a 256-leaf sub-tree, one CTA of 256 threads with a thread per
-// leaf.  It must not exceed 11: a split tree's run has at least 2048 leaves per rank (a FRI layer of 4096 values per rank, in pairs),
-// so every dropped node lies inside one rank's run, and the sub-root layer that is all-gathered is never dropped.
+// leaf.  It must not exceed 8: a unit of a split tree's leaves has at least 256 leaves (a FRI layer of 512 values per unit, in pairs),
+// so every dropped node lies inside one rank's run, and the layer that is all-gathered is never dropped.
 constexpr size_t VG_TREE_DROP = 8;
 
 struct VgTree {

@@ -392,67 +392,62 @@ int32_t vg_inverse_denominators(vgpu_ctx* ctx, uint32_t log_H, const E5& z, uint
 // d_out receives w * BARY_OUT words ([c][q*5 + l] = sum_i p_c(x_i) / (x_i - z_q), [c][10] = sum_i p_c(x_i)), stream-ordered, no
 // host synchronisation — open_multi_batches reads the sums of every matrix back with ONE copy.
 int32_t vg_eval_columns_enqueue(vgpu_ctx* ctx, const vgpu_dmat* lde, uint32_t npoints, const uint32_t* const* invden, uint64_t ics, uint32_t* d_out) {
-    uint64_t H = lde->gh, h = H / 2;
-    uint32_t w = (uint32_t)lde->gw;
-    // split proof: the first h committed rows are the coset g*H and lie in the shards of the first half of the ranks, the other
-    // h rows are the coset g*w_2h*H in the shards of the second half — and EITHER coset determines p(z).  So the first-half ranks
-    // evaluate the first ceil(w/2) columns from their rows, the second-half ranks the remaining columns from theirs (all ranks
-    // work, each on half the columns); the per-rank sums meet in one small all-gather and vg_eval_columns_finish normalises a
-    // column by the coset it was summed over.  invden: the caller's vector over the same rows as the matrix part held here.
-    const bool split = lde->dist == VG_ROWS;
-    const uint32_t w_first = split ? vg_eval_columns_first_coset(w) : w;
-    const uint32_t c_begin = split && lde->row0 >= h ? w_first : 0;
-    w = split ? (lde->row0 < h ? w_first : w - w_first) : w;                // columns summed here
-    const uint64_t rows = split ? (w ? lde->h : 0) : h;
-    BaryParams p{};
-    p.mat = lde->d + (uint64_t)c_begin * lde->col_stride; p.mcs = lde->col_stride; p.h = rows; p.row_begin = 0; p.w = w;
-    p.invden[0] = invden[0]; p.invden[1] = npoints > 1 ? invden[1] : invden[0]; p.ics = ics; p.npoints = npoints;
-    uint32_t nblocks = 1;
-    VgBuf partial(ctx);
-    const uint32_t nout = w * BARY_OUT, nout_all = (uint32_t)lde->gw * BARY_OUT;
-    if (rows == 0) {
-        VG_TRY(partial.alloc(512));
-    } else if (rows >= BARY_TILE && rows % BARY_TILE == 0) {
-        const unsigned by = (w + 31) / 32;
-        p.cpg = 2 * (((w + by - 1) / by + 1) / 2);               // columns per CTA, even
-        p.rs = std::min<uint32_t>(BARY_CHUNKS, BARY_WARPS / (p.cpg / BARY_COLS));
-        const uint64_t ntiles = rows / BARY_TILE;
-        const unsigned bx = (unsigned)std::min<uint64_t>(ntiles, std::max<uint64_t>(1, (uint64_t)ctx->sm_count / by));
-        nblocks = bx * p.rs;
-        VG_TRY(partial.alloc((size_t)nblocks * w * BARY_OUT * 4));
-        p.partial = partial.as<uint32_t>();
-        if (!ctx->bary_attrs_set) {
-            VG_CUDA(ctx, cudaFuncSetAttribute(bary_kernel<1>, cudaFuncAttributeMaxDynamicSharedMemorySize, 2 * 1 * 5 * BARY_TILE * 4));
-            VG_CUDA(ctx, cudaFuncSetAttribute(bary_kernel<2>, cudaFuncAttributeMaxDynamicSharedMemorySize, 2 * 2 * 5 * BARY_TILE * 4));
-            ctx->bary_attrs_set = true;
-        }
-        KScope ks(ctx, KC_BARY, 4.0 * (double)rows * w);
-        if (npoints > 1) bary_kernel<2><<<dim3(bx, by), BARY_THREADS, 2 * 2 * 5 * BARY_TILE * 4, ctx->stream>>>(p);
-        else bary_kernel<1><<<dim3(bx, by), BARY_THREADS, 2 * 1 * 5 * BARY_TILE * 4, ctx->stream>>>(p);
-        VG_LAUNCH_CHECK(ctx);
-    } else {
-        VG_TRY(partial.alloc((size_t)w * BARY_OUT * 4));
-        p.partial = partial.as<uint32_t>();
-        KScope ks(ctx, KC_BARY, 4.0 * (double)rows * w);
-        bary_small_kernel<<<w, 128, 0, ctx->stream>>>(p);
-        VG_LAUNCH_CHECK(ctx);
-    }
-    if (!split) {
-        bary_reduce_kernel<<<(nout + 255) / 256, 256, 0, ctx->stream>>>(partial.as<uint32_t>(), nblocks, nout, d_out);
-        VG_LAUNCH_CHECK(ctx);
-    } else {
-        VgBuf gathered(ctx);                                                               // [rank 0 | rank 1 | ...], all columns each
-        VG_TRY(gathered.alloc((size_t)nout_all * 4 * ctx->comm_size));
-        uint32_t* mine = gathered.as<uint32_t>() + (size_t)nout_all * ctx->comm_rank;
-        VG_CUDA(ctx, cudaMemsetAsync(mine, 0, (size_t)nout_all * 4, ctx->stream));         // the columns the other coset's ranks sum
-        if (nout) {
-            bary_reduce_kernel<<<(nout + 255) / 256, 256, 0, ctx->stream>>>(partial.as<uint32_t>(), nblocks, nout, mine + (size_t)c_begin * BARY_OUT);
+    const uint64_t H = lde->gh, h = H / 2;
+    const uint32_t gw = (uint32_t)lde->gw, nout_all = gw * BARY_OUT;
+    // split proof: the first h committed rows are the coset g*H, the other h rows the coset g*w_2h*H — and EITHER coset determines
+    // p(z).  So the first ceil(w/2) columns are summed over the rows of the first coset, the remaining columns over the rows of the
+    // second: a rank sums its rows of each coset for that coset's columns (one part, or two when its run straddles row h), the
+    // per-rank sums meet in one small all-gather and vg_eval_columns_finish normalises a column by the coset it was summed over.
+    // invden: the caller's vector over the same rows as the matrix part held here.
+    // sum_part: columns [c_begin, c_begin + w) over local rows [r0, r0 + rows) -> out (w * BARY_OUT words)
+    auto sum_part = [&](uint64_t r0, uint64_t rows, uint32_t c_begin, uint32_t w, uint32_t* out) -> int32_t {
+        BaryParams p{};
+        p.mat = lde->d + (uint64_t)c_begin * lde->col_stride; p.mcs = lde->col_stride; p.h = rows; p.row_begin = r0; p.w = w;
+        p.invden[0] = invden[0]; p.invden[1] = npoints > 1 ? invden[1] : invden[0]; p.ics = ics; p.npoints = npoints;
+        uint32_t nblocks = 1;
+        VgBuf partial(ctx);
+        const uint32_t nout = w * BARY_OUT;
+        if (rows >= BARY_TILE && rows % BARY_TILE == 0) {
+            const unsigned by = (w + 31) / 32;
+            p.cpg = 2 * (((w + by - 1) / by + 1) / 2);               // columns per CTA, even
+            p.rs = std::min<uint32_t>(BARY_CHUNKS, BARY_WARPS / (p.cpg / BARY_COLS));
+            const uint64_t ntiles = rows / BARY_TILE;
+            const unsigned bx = (unsigned)std::min<uint64_t>(ntiles, std::max<uint64_t>(1, (uint64_t)ctx->sm_count / by));
+            nblocks = bx * p.rs;
+            VG_TRY(partial.alloc((size_t)nblocks * w * BARY_OUT * 4));
+            p.partial = partial.as<uint32_t>();
+            if (!ctx->bary_attrs_set) {
+                VG_CUDA(ctx, cudaFuncSetAttribute(bary_kernel<1>, cudaFuncAttributeMaxDynamicSharedMemorySize, 2 * 1 * 5 * BARY_TILE * 4));
+                VG_CUDA(ctx, cudaFuncSetAttribute(bary_kernel<2>, cudaFuncAttributeMaxDynamicSharedMemorySize, 2 * 2 * 5 * BARY_TILE * 4));
+                ctx->bary_attrs_set = true;
+            }
+            KScope ks(ctx, KC_BARY, 4.0 * (double)rows * w);
+            if (npoints > 1) bary_kernel<2><<<dim3(bx, by), BARY_THREADS, 2 * 2 * 5 * BARY_TILE * 4, ctx->stream>>>(p);
+            else bary_kernel<1><<<dim3(bx, by), BARY_THREADS, 2 * 1 * 5 * BARY_TILE * 4, ctx->stream>>>(p);
+            VG_LAUNCH_CHECK(ctx);
+        } else {
+            VG_TRY(partial.alloc((size_t)w * BARY_OUT * 4));
+            p.partial = partial.as<uint32_t>();
+            KScope ks(ctx, KC_BARY, 4.0 * (double)rows * w);
+            bary_small_kernel<<<w, 128, 0, ctx->stream>>>(p);
             VG_LAUNCH_CHECK(ctx);
         }
-        VG_TRY(vg_comm_allgather_inplace(ctx, gathered.as<uint32_t>(), nout_all));
-        bary_reduce_kernel<<<(nout_all + 255) / 256, 256, 0, ctx->stream>>>(gathered.as<uint32_t>(), (uint32_t)ctx->comm_size, nout_all, d_out);
+        bary_reduce_kernel<<<(nout + 255) / 256, 256, 0, ctx->stream>>>(partial.as<uint32_t>(), nblocks, nout, out);
         VG_LAUNCH_CHECK(ctx);
-    }
+        return 0;
+    };
+    if (lde->dist != VG_ROWS) return sum_part(0, h, 0, gw, d_out);
+    const uint32_t w_first = vg_eval_columns_first_coset(gw);
+    VgBuf gathered(ctx);                                                               // [rank 0 | rank 1 | ...], all columns each
+    VG_TRY(gathered.alloc((size_t)nout_all * 4 * ctx->comm_size));
+    uint32_t* mine = gathered.as<uint32_t>() + (size_t)nout_all * ctx->comm_rank;
+    VG_CUDA(ctx, cudaMemsetAsync(mine, 0, (size_t)nout_all * 4, ctx->stream));         // the columns the other coset's rows sum
+    const uint64_t g0 = lde->row0, g1 = lde->row0 + lde->h, mid = std::min(std::max(h, g0), g1);   // global rows; [g0, mid) in the first coset
+    if (mid > g0 && w_first) VG_TRY(sum_part(0, mid - g0, 0, w_first, mine));
+    if (g1 > mid && gw > w_first) VG_TRY(sum_part(mid - g0, g1 - mid, w_first, gw - w_first, mine + (size_t)w_first * BARY_OUT));
+    VG_TRY(vg_comm_allgather_inplace(ctx, gathered.as<uint32_t>(), nout_all));
+    bary_reduce_kernel<<<(nout_all + 255) / 256, 256, 0, ctx->stream>>>(gathered.as<uint32_t>(), (uint32_t)ctx->comm_size, nout_all, d_out);
+    VG_LAUNCH_CHECK(ctx);
     return 0;
 }
 

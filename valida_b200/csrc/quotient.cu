@@ -35,8 +35,8 @@ constexpr uint32_t Q_MAX_CONSTRAINTS = 128;   // bitwise: 88 base + interactions
 
 struct QParams {
     // Base pointers are VIRTUAL: base + (global storage row) is the element, whether the matrix is whole or this rank's row
-    // shard (then base = shard - first row).  The *_n bases serve the "next" rows: natural row i + 2 of every row of a shard
-    // lies in ONE other rank's shard (rows of a shard share i mod comm_size), read through its peer pointer over NVLink.
+    // shard (then base = shard - first row).  The *_n bases serve the "next" rows: natural row i + 2 of every row of the launch's
+    // range lies in ONE rank's shard (vgpu_quotient's next-row table), read through its peer pointer over NVLink.
     const uint32_t* main; const uint32_t* main_n; uint64_t mcs;
     const uint32_t* prep; const uint32_t* prep_n; uint64_t pcs;
     const uint32_t* perm; const uint32_t* perm_n; uint64_t qcs;
@@ -207,26 +207,42 @@ extern "C" int32_t vgpu_quotient(vgpu_ctx* ctx, const vgpu_chip_desc* chip, uint
     p.row_begin = split ? main_lde->row0 : 0;
     p.row_end = split ? main_lde->row0 + main_lde->h : 2 * h;
     if ((p.row_begin & 1) || (p.row_end & 1)) VG_FAIL(ctx, "quotient: a row shard must hold whole (x, -x) pairs");
-    int next_rank = ctx->comm_rank;
-    if (split) {   // rank holding natural rows i + 2 of this shard's rows: reverse_bits((reverse_bits(rank) + 2) mod G)
-        int lg = 0; while ((1 << lg) < ctx->comm_size) lg++;
-        const uint32_t rho = bb::reverse_bits((uint32_t)ctx->comm_rank, lg);
-        next_rank = (int)bb::reverse_bits((rho + 2) & (uint32_t)(ctx->comm_size - 1), lg);
+    // The next-row table: the 2h storage rows are V units (ctx.h); unit u holds the rows of natural index i = bitrev(u) mod V, so the
+    // next rows (i + 2) of all its rows lie in unit bitrev((bitrev(u) + 2) mod V), which one rank holds.  Consecutive units of this
+    // rank's run whose next rows one rank holds form one launch: a single launch at a power-of-two comm_size (every unit of a run
+    // then names the same rank), at most one per unit otherwise.  next_rank[k]: the rank holding the next rows of local range k.
+    std::vector<uint64_t> range_end;             // storage rows: range k is [range_end[k - 1] (or row_begin), range_end[k])
+    std::vector<int> next_rank;
+    if (!split) { range_end.push_back(p.row_end); next_rank.push_back(ctx->comm_rank); }
+    else {
+        const int G = ctx->comm_size;
+        const uint64_t V = vg_units(G), urows = 2 * h / V;
+        int lgv = 0; while ((1ull << lgv) < V) lgv++;
+        if (p.row_begin % urows || p.row_end % urows) VG_FAIL(ctx, "quotient: a row shard must hold whole units");
+        for (uint64_t u = p.row_begin / urows; u < p.row_end / urows; u++) {
+            const uint32_t un = bb::reverse_bits((bb::reverse_bits((uint32_t)u, lgv) + 2) & (uint32_t)(V - 1), lgv);
+            int d = 0;
+            while (vg_unit_begin(G, d + 1) <= un) d++;
+            if (!next_rank.empty() && next_rank.back() == d) range_end.back() = (u + 1) * urows;
+            else { range_end.push_back((u + 1) * urows); next_rank.push_back(d); }
+        }
     }
-    // virtual bases of a matrix: local rows, and the rows of `next_rank`
+    // virtual bases of a matrix: local rows, and the rows of rank d
     auto base_of = [&](const vgpu_dmat* m) { return m->d - (split ? m->row0 : 0); };
-    auto next_of = [&](const vgpu_dmat* m) -> const uint32_t* {
-        if (!split || next_rank == ctx->comm_rank) return base_of(m);
+    auto next_of = [&](const vgpu_dmat* m, int d) -> const uint32_t* {
+        if (!split || d == ctx->comm_rank) return base_of(m);
         if (!m->symm) return nullptr;
-        return vg_peer_ptr(ctx, m->d, next_rank) - (uint64_t)next_rank * m->h;
+        return vg_peer_ptr(ctx, m->d, d) - vg_run_bound(m->gh, ctx->comm_size, d);
     };
+    for (int d : next_rank)
+        if (!next_of(main_lde, d) || !next_of(perm_lde, d) || (prep_lde && !next_of(prep_lde, d)))
+            VG_FAIL(ctx, "quotient: a row shard read by a peer must live in the symmetric heap");
     VgMat out;
     VG_TRY(vg_dmat_alloc_run(ctx, h, 10, split, false, &out));
     out->bitrev_rows = true;
-    p.main = base_of(main_lde); p.main_n = next_of(main_lde); p.mcs = main_lde->col_stride;
-    p.prep = prep_lde ? base_of(prep_lde) : nullptr; p.prep_n = prep_lde ? next_of(prep_lde) : nullptr; p.pcs = prep_lde ? prep_lde->col_stride : 0;
-    p.perm = base_of(perm_lde); p.perm_n = next_of(perm_lde); p.qcs = perm_lde->col_stride;
-    if (!p.main_n || !p.perm_n || (prep_lde && !p.prep_n)) VG_FAIL(ctx, "quotient: a row shard read by a peer must live in the symmetric heap");
+    p.main = base_of(main_lde); p.mcs = main_lde->col_stride;
+    p.prep = prep_lde ? base_of(prep_lde) : nullptr; p.pcs = prep_lde ? prep_lde->col_stride : 0;
+    p.perm = base_of(perm_lde); p.qcs = perm_lde->col_stride;
     p.out = out->d - p.row_begin / 2; p.ocs = out->col_stride;
     p.log_h = log_degree;
     p.s = bb::to_monty(bb::GEN_CANON);
@@ -250,9 +266,15 @@ extern "C" int32_t vgpu_quotient(vgpu_ctx* ctx, const vgpu_chip_desc* chip, uint
         const uint64_t stride = (pc + SEL_BATCH - 1) / SEL_BATCH;
         selector_inverse_kernel<<<(unsigned)((stride + 255) / 256), 256, 0, ctx->stream>>>(selinv.as<uint32_t>() - pb, pb, pc, log_degree, p.s, p.glast, p.root_lo, p.root_hi);
         ctx->launches++;
-        air::with_chip(chip->chip_id, [&](auto c) {
-            quotient_kernel<decltype(c)::value><<<(unsigned)((p.row_end - p.row_begin + 127) / 128), 128, 0, ctx->stream>>>(p);
-        });
+        const uint64_t row_begin = p.row_begin, row_end = p.row_end;
+        for (size_t k = 0; k < next_rank.size(); k++) {
+            p.row_begin = k ? range_end[k - 1] : row_begin; p.row_end = range_end[k];
+            p.main_n = next_of(main_lde, next_rank[k]); p.prep_n = prep_lde ? next_of(prep_lde, next_rank[k]) : nullptr; p.perm_n = next_of(perm_lde, next_rank[k]);
+            air::with_chip(chip->chip_id, [&](auto c) {
+                quotient_kernel<decltype(c)::value><<<(unsigned)((p.row_end - p.row_begin + 127) / 128), 128, 0, ctx->stream>>>(p);
+            });
+        }
+        p.row_begin = row_begin; p.row_end = row_end;
     }
     selinv.reset();
     VG_LAUNCH_CHECK(ctx);
