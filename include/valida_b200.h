@@ -242,6 +242,29 @@ int32_t vgpu_check_constraints_local(vgpu_ctx* ctx, const vgpu_chip_desc* chip, 
                                      const vgpu_dmat* perm, const uint32_t challenges[15],
                                      int64_t* first_row, uint32_t* first_constraint, uint64_t* failing_rows);
 
+/* One (row, constraint) on which a chip's check does not vanish. */
+typedef struct vgpu_check_failure {
+    int64_t row;                /* global row of the trace */
+    uint32_t constraint;        /* index in eval order, as vgpu_check_constraints numbers it */
+    uint32_t value[5];          /* the constraint's value on that row, canonical; a base-field constraint has limbs 1..4 = 0 */
+} vgpu_check_failure;
+/* A chip's constraints in eval order: *air_constraints assertions of Air::eval, then one per interaction, then the LogUp transition,
+ * first-row and last-row constraints; *total = air + n_interactions + 3.  Returns -1 for a null argument or an unknown chip id. */
+int32_t vgpu_chip_constraint_count(const vgpu_chip_desc* chip, uint32_t* air_constraints, uint32_t* total);
+/* Every (row, constraint) on which the chip's check does not vanish, not only the first.  Writes:
+ *   - the first min(cap, *total_failures) of them, in ascending (row, constraint) order, into out;
+ *   - *n_out: the number written;
+ *   - rows_per_constraint[c] (may be NULL, else `total` entries of vgpu_chip_constraint_count): the rows on which constraint c fails.
+ * out[0] is vgpu_check_constraints' (first_row, first_constraint), the distinct rows of the list are its failing_rows, and the
+ * per-constraint counts sum to *total_failures.  Takes the arguments of vgpu_check_constraints_local and refuses the same inputs, and
+ * out == NULL with cap > 0 and a null n_out or total_failures, before anything is enqueued and alike on every rank.  On a split context
+ * it is collective and every rank gets identical output (one all-gather of each rank's counts, one of each rank's first min(count,
+ * cap) entries); on any other context it checks whole matrices.  Two sweeps of the traces: one counts (a clean witness costs about one
+ * vgpu_check_constraints), the second, in the parts of the trace whose failures fall below cap only, writes.  Synchronises. */
+int32_t vgpu_check_failures(vgpu_ctx* ctx, const vgpu_chip_desc* chip, const vgpu_dmat* main, const vgpu_dmat* prep_or_null,
+                            const vgpu_dmat* perm, const uint32_t challenges[15], uint64_t cap, vgpu_check_failure* out,
+                            uint64_t* n_out, uint64_t* total_failures, uint64_t* rows_per_constraint);
+
 typedef struct vgpu_check_report {
     int64_t first_row;          /* -1: every constraint vanishes on every row */
     uint32_t first_constraint;

@@ -96,6 +96,18 @@ pub struct vgpu_chip_desc {
     pub interactions: [vgpu_interaction; VGPU_MAX_INTERACTIONS],
 }
 
+/// One (row, constraint) on which a chip's check does not vanish ([`vgpu_check_failures`]).
+#[repr(C)]
+#[derive(Clone, Copy, Debug, Default, PartialEq, Eq)]
+pub struct vgpu_check_failure {
+    /// Global row of the trace.
+    pub row: i64,
+    /// Index in eval order, as [`vgpu_check_constraints`] numbers it.
+    pub constraint: u32,
+    /// The constraint's value on that row, canonical; a base-field constraint has limbs 1..4 = 0.
+    pub value: [u32; 5],
+}
+
 /// One chip's verdict of [`vgpu_check_witness`].
 #[repr(C)]
 #[derive(Clone, Copy, Debug, Default)]
@@ -161,6 +173,8 @@ extern "C" {
     pub fn vgpu_quotient(ctx: *mut vgpu_ctx, chip: *const vgpu_chip_desc, log_degree: u32, prep_lde_or_null: *const vgpu_dmat, main_lde: *const vgpu_dmat, perm_lde: *const vgpu_dmat, cumulative_sum: *const u32, perm_challenges: *const u32, alpha: *const u32, out_chunks: *mut *mut vgpu_dmat) -> i32;
     pub fn vgpu_check_constraints(ctx: *mut vgpu_ctx, chip: *const vgpu_chip_desc, main: *const vgpu_dmat, prep_or_null: *const vgpu_dmat, perm: *const vgpu_dmat, challenges: *const u32, first_row: *mut i64, first_constraint: *mut u32, failing_rows: *mut u64) -> i32;
     pub fn vgpu_check_constraints_local(ctx: *mut vgpu_ctx, chip: *const vgpu_chip_desc, main: *const vgpu_dmat, prep_or_null: *const vgpu_dmat, perm: *const vgpu_dmat, challenges: *const u32, first_row: *mut i64, first_constraint: *mut u32, failing_rows: *mut u64) -> i32;
+    pub fn vgpu_chip_constraint_count(chip: *const vgpu_chip_desc, air_constraints: *mut u32, total: *mut u32) -> i32;
+    pub fn vgpu_check_failures(ctx: *mut vgpu_ctx, chip: *const vgpu_chip_desc, main: *const vgpu_dmat, prep_or_null: *const vgpu_dmat, perm: *const vgpu_dmat, challenges: *const u32, cap: u64, out: *mut vgpu_check_failure, n_out: *mut u64, total_failures: *mut u64, rows_per_constraint: *mut u64) -> i32;
     pub fn vgpu_check_witness(ctx: *mut vgpu_ctx, main: *const *const vgpu_dmat, prep: *const *const vgpu_dmat, challenges: *const u32, report: *mut vgpu_check_report, sums_cancel: *mut i32) -> i32;
 
     // ---- transcript ----

@@ -384,6 +384,29 @@ impl Context {
         Ok((row, constraint, failing))
     }
 
+    /// Every `(row, constraint, value)` on which the check of [`Context::check_constraints_local`] does not vanish, not only the first:
+    /// the first `min(cap, total)` in ascending (row, constraint) order, the total, and per constraint (eval order) the number of rows
+    /// on which it fails.  Same arguments and refusals as `check_constraints_local`; collective on a split context, with the same
+    /// result on every rank.  Synchronises.
+    pub fn check_failures(&self, chip_id: u32, main: &DMat<'_>, prep: Option<&DMat<'_>>, perm: &DMat<'_>, challenges: &[u32; 15], cap: usize)
+                          -> Result<(Vec<sys::vgpu_check_failure>, u64, Vec<u64>)> {
+        let chip = unsafe { sys::vgpu_basic_machine_chip(chip_id) };
+        let (mut air, mut total_constraints) = (0u32, 0u32);
+        if unsafe { sys::vgpu_chip_constraint_count(chip, &mut air, &mut total_constraints) } != 0 {
+            return Err(Error { code: -1, message: format!("check_failures: unknown chip id {chip_id}") });
+        }
+        let prep_ptr = prep.map_or(ptr::null(), |m| m.as_ptr());
+        let mut out = vec![sys::vgpu_check_failure::default(); cap];
+        let mut per = vec![0u64; total_constraints as usize];
+        let (mut n, mut total) = (0u64, 0u64);
+        self.check(unsafe {
+            sys::vgpu_check_failures(self.raw, chip, main.as_ptr(), prep_ptr, perm.as_ptr(), challenges.as_ptr(), cap as u64, out.as_mut_ptr(),
+                                     &mut n, &mut total, per.as_mut_ptr())
+        })?;
+        out.truncate(n as usize);
+        Ok((out, total, per))
+    }
+
     /// The witness check of the reference's debug builds (`check_constraints` of every chip + `check_cumulative_sums`,
     /// `derive/src/lib.rs:246-253,376-377`) without a proof, with the caller's 15 challenge words: one report per chip and whether
     /// the cumulative sums cancel.  `main` / `prep` are whole traces or, on a [`LocalGroup`] rank, its row shards; every rank of a

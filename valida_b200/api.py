@@ -41,6 +41,24 @@ class _CheckReport(C.Structure):
     _fields_ = [("first_row", C.c_int64), ("first_constraint", C.c_uint32), ("failing_rows", C.c_uint64), ("cumulative_sum", C.c_uint32 * 5)]
 
 
+class _PairCol(C.Structure):
+    _fields_ = [("constant", C.c_uint32), ("n_terms", C.c_uint32), ("terms", C.c_uint32 * 12)]
+
+
+class _Interaction(C.Structure):
+    _fields_ = [("n_fields", C.c_uint32), ("fields", _PairCol * 14), ("count", _PairCol), ("bus", C.c_uint32), ("is_send", C.c_uint32)]
+
+
+class _ChipDesc(C.Structure):
+    """vgpu_chip_desc (the fields constraint_label reads)."""
+    _fields_ = [("chip_id", C.c_uint32), ("width", C.c_uint32), ("preprocessed_width", C.c_uint32), ("n_interactions", C.c_uint32),
+                ("interactions", _Interaction * 5)]
+
+
+# vgpu_check_failure: one (row, constraint) on which a chip's check does not vanish, and the constraint's canonical value there
+CHECK_FAILURE_DTYPE = np.dtype([("row", "<i8"), ("constraint", "<u4"), ("value", "<u4", (5,))])
+
+
 def _load():
     if not os.path.exists(lib_path):
         raise VgpuError(
@@ -88,6 +106,8 @@ def _load():
         "vgpu_quotient": (C.c_int32, [vp, vp, C.c_uint32, vp, vp, vp, u32p, u32p, u32p, C.POINTER(vp)]),
         "vgpu_check_constraints": (C.c_int32, [vp, vp, vp, vp, vp, u32p, C.POINTER(C.c_int64), u32p, C.POINTER(u64)]),
         "vgpu_check_constraints_local": (C.c_int32, [vp, vp, vp, vp, vp, u32p, C.POINTER(C.c_int64), u32p, C.POINTER(u64)]),
+        "vgpu_chip_constraint_count": (C.c_int32, [vp, u32p, u32p]),
+        "vgpu_check_failures": (C.c_int32, [vp, vp, vp, vp, vp, u32p, u64, vp, C.POINTER(u64), C.POINTER(u64), C.POINTER(u64)]),
         "vgpu_check_witness": (C.c_int32, [vp, C.POINTER(vp), C.POINTER(vp), u32p, C.POINTER(_CheckReport), C.POINTER(C.c_int32)]),
         "vgpu_ctx_set_debug_checks": (C.c_int32, [vp, C.c_int32]),
         "vgpu_set_challenger": (C.c_int32, [vp, u32p, u32p]),
@@ -599,6 +619,48 @@ def check_constraints_local(ctx, chip_id, main, prep, perm, perm_challenges):
     ctx.check(lib().vgpu_check_constraints_local(ctx._h, chip, main._h, prep._h if prep is not None else None, perm._h,
                                                  _u32arr(perm_challenges, 15), C.byref(row), C.byref(con), C.byref(n)))
     return int(row.value), int(con.value), int(n.value)
+
+
+def constraint_count(chip_id):
+    """(assertions of the chip's Air::eval, all its constraints: those, one per interaction, and the three LogUp constraints)."""
+    air, total = C.c_uint32(), C.c_uint32()
+    if lib().vgpu_chip_constraint_count(lib().vgpu_basic_machine_chip(chip_id), C.byref(air), C.byref(total)) != 0:
+        raise VgpuError("constraint_count: unknown chip id %r" % (chip_id,))
+    return int(air.value), int(total.value)
+
+
+def constraint_label(chip_id, index):
+    """What constraint `index` (eval order, as check_constraints and check_failures number them) of a chip is, from the chip
+    description: "Air::eval assertion i", "interaction m (bus b, send|receive)", "LogUp transition", "LogUp first row" or
+    "LogUp last row"."""
+    air, total = constraint_count(chip_id)
+    if not 0 <= index < total:
+        raise VgpuError("constraint_label: chip %d has %d constraints, not %r" % (chip_id, total, index))
+    if index < air:
+        return "Air::eval assertion %d" % index
+    desc = C.cast(lib().vgpu_basic_machine_chip(chip_id), C.POINTER(_ChipDesc)).contents
+    m = index - air
+    if m < desc.n_interactions:
+        it = desc.interactions[m]
+        return "interaction %d (bus %d, %s)" % (m, it.bus, "send" if it.is_send else "receive")
+    return ("LogUp transition", "LogUp first row", "LogUp last row")[m - desc.n_interactions]
+
+
+def check_failures(ctx, chip_id, main, prep, perm, perm_challenges, cap=1 << 16):
+    """Every (row, constraint) on which check_constraints' constraints do not vanish, not only the first.  Takes what
+    check_constraints_local takes (whole matrices, or on a split context this rank's row shards; collective there, with the same
+    result on every rank).  Returns (failures, total, rows_per_constraint): the first min(cap, total) failures in ascending (row,
+    constraint) order as a CHECK_FAILURE_DTYPE array (value: the constraint's canonical value, limbs 1..4 zero for a base-field
+    constraint), the number of failures, and per constraint the number of rows on which it fails."""
+    chip = lib().vgpu_basic_machine_chip(chip_id)
+    _, total_constraints = constraint_count(chip_id)
+    out = np.zeros(int(cap), dtype=CHECK_FAILURE_DTYPE)
+    per = np.zeros(total_constraints, dtype=np.uint64)
+    n, total = C.c_uint64(), C.c_uint64()
+    ctx.check(lib().vgpu_check_failures(ctx._h, chip, main._h, prep._h if prep is not None else None, perm._h, _u32arr(perm_challenges, 15),
+                                        int(cap), out.ctypes.data_as(C.c_void_p) if cap else None, C.byref(n), C.byref(total),
+                                        per.ctypes.data_as(C.POINTER(C.c_uint64))))
+    return out[:n.value].copy(), int(total.value), per
 
 
 def check_witness(ctx, main, prep, challenges):

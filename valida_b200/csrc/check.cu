@@ -18,6 +18,7 @@
 #include "airs.cuh"
 #include "logup.cuh"
 #include "open.h"
+#include <functional>
 #include <memory>
 
 namespace {
@@ -135,6 +136,190 @@ int32_t enqueue_sweep(vgpu_ctx* ctx, const vgpu_chip_desc* chip, const uint32_t 
     return 0;
 }
 
+// ---- every failure (vgpu_check_failures) ------------------------------------------------------------------------------------------
+// The same rows and text as check_kernel, in kernels of their own so that check_kernel stays as it is.  Pass 1 counts: a CTA keeps a
+// shared histogram of its failures per constraint and, only when it found one, stores its count and adds the histogram to the
+// call's (a clean witness makes no global atomic).  A scan of the per-CTA counts gives each CTA its first entry; pass 2 runs only in
+// the CTAs with failures that start below the cap, counts each thread's failures again, scans them over the CTA and writes each
+// thread's entries in constraint order: the list is ordered by row, then constraint, whatever the schedule.
+struct FParams {
+    CParams c;                               // the run (c.first / c.count unused)
+    uint32_t* cta_count;                     // failures of each CTA of every sweep of the call; this sweep's CTAs from cta0
+    const unsigned long long* cta_off;       // pass 2: exclusive prefix sum of cta_count
+    unsigned long long* hist;                // pass 1: failures per constraint (= failing rows, a constraint fails once per row)
+    vgpu_check_failure* out; uint64_t cap;   // pass 2: entries [0, cap) of the list
+    uint32_t cta0;
+};
+
+__shared__ uint32_t fail_hist[CHECK_MAX_CONSTRAINTS];
+
+struct FailCountBuilder {
+    using V = air::F;
+    const uint32_t* lrow; const uint32_t* nrow; uint64_t cs;
+    F first, last, trans;
+    uint32_t idx; bool active;
+    __device__ __forceinline__ F L(int c) const { return F{__ldg(lrow + (uint64_t)c * cs)}; }
+    __device__ __forceinline__ F N(int c) const { return F{__ldg(nrow + (uint64_t)c * cs)}; }
+    // every lane reaches every constraint (the text has no branch on values): one shared atomic per warp and failing constraint
+    __device__ __forceinline__ void tally(bool bad) {
+        const unsigned v = __ballot_sync(0xffffffffu, active && bad);
+        if (v && (threadIdx.x & 31) == 0) atomicAdd(&fail_hist[idx], (unsigned)__popc(v));
+        idx++;
+    }
+    __device__ __forceinline__ void z(F x) { tally(x.v != 0); }
+    __device__ __forceinline__ void z_ext(const E5& x) { tally(!bb::e5_is_zero(x)); }
+};
+
+// Counts the thread's failures while pos < end is false; then writes those at entries [pos, end) of the CTA's part of the list.
+struct FailWriteBuilder {
+    using V = air::F;
+    const uint32_t* lrow; const uint32_t* nrow; uint64_t cs;
+    F first, last, trans;
+    uint32_t idx, pos, end;
+    vgpu_check_failure* out;                 // the CTA's first entry
+    uint64_t row;
+    __device__ __forceinline__ F L(int c) const { return F{__ldg(lrow + (uint64_t)c * cs)}; }
+    __device__ __forceinline__ F N(int c) const { return F{__ldg(nrow + (uint64_t)c * cs)}; }
+    __device__ __forceinline__ void put(const uint32_t* v, int limbs) {
+        vgpu_check_failure* e = out + pos;
+        e->row = (int64_t)row;
+        e->constraint = idx;
+        for (int l = 0; l < 5; l++) e->value[l] = l < limbs ? bb::from_monty(v[l]) : 0u;
+    }
+    __device__ __forceinline__ void z(F x) {
+        if (x.v != 0) { if (pos < end) put(&x.v, 1); pos++; }
+        idx++;
+    }
+    __device__ __forceinline__ void z_ext(const E5& x) {
+        if (!bb::e5_is_zero(x)) { if (pos < end) put(x.c, 5); pos++; }
+        idx++;
+    }
+};
+
+// the rows of one thread, as check_kernel sets them up
+template <class B>
+__device__ __forceinline__ void fail_rows(const CParams& p, uint64_t i, B& b) {
+    const bool is_last = p.g0 + i + 1 == p.h;
+    const uint64_t n = i + 1 < p.n ? i + 1 : p.wrap;
+    b.lrow = p.main + i; b.nrow = p.main + n; b.cs = p.mcs;
+    b.first = F{p.g0 + i == 0 ? bb::R1 : 0u};
+    b.last = F{is_last ? bb::R1 : 0u};
+    b.trans = F{is_last ? 0u : bb::R1};
+}
+template <int CHIP, class B>
+__device__ __forceinline__ void fail_eval(const CParams& p, uint64_t i, B& b) {
+    const uint64_t n = i + 1 < p.n ? i + 1 : p.wrap;
+    b.idx = 0;
+    air::eval_chip<CHIP>(b);
+    E5 cumsum;
+#pragma unroll
+    for (int l = 0; l < 5; l++) cumsum.c[l] = __ldg(p.cumsum + (uint64_t)l * p.ccs);
+    logup::eval_constraints(b, p.chip, b.lrow, b.nrow, p.mcs, p.prep ? p.prep + i : nullptr, p.prep ? p.prep + n : nullptr, p.pcs,
+                            p.perm + i, p.perm + n, p.qcs, cumsum);
+}
+
+template <int CHIP>
+__global__ void __maxnreg__(128) fail_count_kernel(const __grid_constant__ FParams f) {
+    const CParams& p = f.c;
+    for (uint32_t t = threadIdx.x; t < CHECK_MAX_CONSTRAINTS; t += blockDim.x) fail_hist[t] = 0;
+    __syncthreads();
+    const uint64_t i_raw = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
+    FailCountBuilder b;
+    b.active = i_raw < p.n;
+    const uint64_t i = b.active ? i_raw : p.n - 1;        // idle lanes shadow the last row (the warp vote needs every lane)
+    fail_rows(p, i, b);
+    fail_eval<CHIP>(p, i, b);
+    __syncthreads();
+    __shared__ uint32_t warp_total[4];
+    uint32_t s = 0;
+    for (uint32_t t = threadIdx.x; t < CHECK_MAX_CONSTRAINTS; t += blockDim.x) s += fail_hist[t];
+    s = __reduce_add_sync(0xffffffffu, s);
+    if ((threadIdx.x & 31) == 0) warp_total[threadIdx.x >> 5] = s;
+    __syncthreads();
+    const uint32_t total = warp_total[0] + warp_total[1] + warp_total[2] + warp_total[3];
+    if (!total) return;
+    if (threadIdx.x == 0) f.cta_count[f.cta0 + blockIdx.x] = total;
+    for (uint32_t t = threadIdx.x; t < CHECK_MAX_CONSTRAINTS; t += blockDim.x)
+        if (fail_hist[t]) atomicAdd(f.hist + t, (unsigned long long)fail_hist[t]);
+}
+
+template <int CHIP>
+__global__ void __maxnreg__(128) fail_write_kernel(const __grid_constant__ FParams f) {
+    const CParams& p = f.c;
+    const uint32_t cta = f.cta0 + blockIdx.x, total = f.cta_count[cta];
+    const unsigned long long base = f.cta_off[cta];
+    if (!total || base >= f.cap) return;                  // alike for the whole CTA
+    const uint64_t i_raw = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
+    const bool active = i_raw < p.n;
+    const uint64_t i = active ? i_raw : p.n - 1;
+    FailWriteBuilder b;
+    fail_rows(p, i, b);
+    b.out = f.out + base; b.row = p.g0 + i;
+    b.pos = 0; b.end = 0;
+    fail_eval<CHIP>(p, i, b);
+    // the thread's first entry: the failures of the CTA's lower threads
+    __shared__ uint32_t warp_total[4];
+    const uint32_t mine = active ? b.pos : 0, lane = threadIdx.x & 31;
+    uint32_t x = mine;
+#pragma unroll
+    for (int d = 1; d < 32; d <<= 1) {
+        const uint32_t y = __shfl_up_sync(0xffffffffu, x, d);
+        if (lane >= (uint32_t)d) x += y;
+    }
+    if (lane == 31) warp_total[threadIdx.x >> 5] = x;
+    __syncthreads();
+    uint32_t first = x - mine;
+    for (uint32_t w = 0; w < (threadIdx.x >> 5); w++) first += warp_total[w];
+    const uint32_t end = (uint32_t)min((unsigned long long)total, f.cap - base);
+    if (!mine || first >= end) return;
+    b.pos = first; b.end = end;
+    fail_eval<CHIP>(p, i, b);
+}
+
+// One CTA: the exclusive prefix sum of the m per-CTA counts, their total, and *end = 1 + the last CTA with failures that starts below
+// cap (0: none), which bounds pass 2's grids.
+__global__ void __launch_bounds__(1024) fail_scan_kernel(const uint32_t* count, uint32_t m, uint64_t cap, unsigned long long* off,
+                                                         unsigned long long* total, uint32_t* end) {
+    __shared__ unsigned long long warp_sum[32];
+    __shared__ uint32_t warp_end[32];
+    const uint32_t per = (m + 1023) / 1024, a = min(m, threadIdx.x * per), e = min(m, a + per), lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+    unsigned long long s = 0;
+    for (uint32_t j = a; j < e; j++) s += count[j];
+    unsigned long long x = s;
+#pragma unroll
+    for (int d = 1; d < 32; d <<= 1) {
+        const unsigned long long y = __shfl_up_sync(0xffffffffu, x, d);
+        if (lane >= (uint32_t)d) x += y;
+    }
+    if (lane == 31) warp_sum[warp] = x;
+    __syncthreads();
+    if (warp == 0) {
+        unsigned long long w = warp_sum[lane];
+#pragma unroll
+        for (int d = 1; d < 32; d <<= 1) {
+            const unsigned long long y = __shfl_up_sync(0xffffffffu, w, d);
+            if (lane >= (uint32_t)d) w += y;
+        }
+        warp_sum[lane] = w;
+    }
+    __syncthreads();
+    unsigned long long at = x - s + (warp ? warp_sum[warp - 1] : 0);
+    uint32_t last = 0;
+    for (uint32_t j = a; j < e; j++) {
+        off[j] = at;
+        if (count[j] && at < cap) last = j + 1;
+        at += count[j];
+    }
+    if (threadIdx.x == 1023) *total = at;               // its range ends at m
+    last = __reduce_max_sync(0xffffffffu, last);
+    if (lane == 0) warp_end[warp] = last;
+    __syncthreads();
+    if (warp == 0) {
+        last = __reduce_max_sync(0xffffffffu, warp_end[lane]);
+        if (lane == 0) *end = last;
+    }
+}
+
 }  // namespace
 
 // Validates the arguments (before anything is enqueued) and enqueues the sweep of one chip's whole traces.  d_first / d_count must
@@ -212,8 +397,11 @@ class CheckSet {
         VG_CUDA(ctx_, cudaMemsetAsync(mine + n_, 0, n_ * sizeof(unsigned long long), ctx_->stream));
         return 0;
     }
+    // Launches one run's sweep (p complete but for the chip): vgpu_check_failures' passes; by default enqueue_sweep's check_kernel.
+    using Sweep = std::function<int32_t(const vgpu_chip_desc*, CParams&)>;
     // Enqueues chip i's sweep of this rank's run (arguments validated); what it reads of perm is read before later work on the stream.
-    int32_t sweep(uint32_t i, const vgpu_dmat* main, const vgpu_dmat* prep, const vgpu_dmat* perm, const uint32_t challenges[15]) {
+    int32_t sweep(uint32_t i, const vgpu_dmat* main, const vgpu_dmat* prep, const vgpu_dmat* perm, const uint32_t challenges[15],
+                  const Sweep& run = nullptr) {
         Chip& c = chips_[i];
         VG_TRY(vg_dmat_materialize(ctx_, main));
         VG_TRY(vg_dmat_materialize(ctx_, prep));
@@ -232,7 +420,7 @@ class CheckSet {
         p.n = c.run.split ? cnt - 1 : cnt;
         p.wrap = c.run.split ? p.n : 0;
         p.first = own_verdicts() + i; p.count = own_verdicts() + n_ + i;
-        VG_TRY(enqueue_sweep(ctx_, c.desc, challenges, p));
+        VG_TRY(run ? run(c.desc, p) : enqueue_sweep(ctx_, c.desc, challenges, p));
         if (!c.run.split) return 0;
         // the block this rank sends (first rows, last running sum) and the window's row 0 (this rank's last row)
         uint32_t* blk = block_.as<uint32_t>() + (uint64_t)ctx_->comm_rank * words_ + c.at;
@@ -249,6 +437,12 @@ class CheckSet {
     }
     // The exchange of the boundary blocks, the window sweeps and the exchange of the verdicts.
     int32_t finish(const uint32_t challenges[15]) {
+        if (!any_split_) return 0;
+        VG_TRY(windows(challenges));
+        return vg_comm_allgather_inplace(ctx_, (uint32_t*)verdicts_.p, 4 * (uint64_t)n_);
+    }
+    // The exchange of the boundary blocks and the window sweeps (each the last row of a split chip's run, after its other rows).
+    int32_t windows(const uint32_t challenges[15], const Sweep& run = nullptr) {
         if (!any_split_) return 0;
         const uint32_t N = (uint32_t)ctx_->comm_size, next = ((uint32_t)ctx_->comm_rank + 1) % N;
         VG_TRY(vg_comm_allgather_inplace(ctx_, block_.as<uint32_t>(), words_));
@@ -270,9 +464,9 @@ class CheckSet {
             p.cumsum = block_.as<uint32_t>() + (uint64_t)(N - 1) * words_ + c.at + c.wm + c.wp + c.wq; p.ccs = 1;   // the last rank's
             p.g0 = c.run.begin + c.run.count - 1; p.n = 1; p.h = c.h; p.wrap = 1;
             p.first = own_verdicts() + i; p.count = own_verdicts() + n_ + i;
-            VG_TRY(enqueue_sweep(ctx_, c.desc, challenges, p));
+            VG_TRY(run ? run(c.desc, p) : enqueue_sweep(ctx_, c.desc, challenges, p));
         }
-        return vg_comm_allgather_inplace(ctx_, (uint32_t*)verdicts_.p, 4 * (uint64_t)n_);
+        return 0;
     }
     // every rank's verdicts, as finish() left them on the device
     const void* verdicts() const { return verdicts_.p; }
@@ -388,5 +582,106 @@ extern "C" int32_t vgpu_check_witness(vgpu_ctx* ctx, const vgpu_dmat* const main
         }
     vg_check_reports(chk, cumsum, report);
     *sums_cancel = vg_sums_cancel(cumsum) ? 1 : 0;
+    return 0;
+}
+
+extern "C" int32_t vgpu_chip_constraint_count(const vgpu_chip_desc* chip, uint32_t* air_constraints, uint32_t* total) {
+    if (!chip || !air_constraints || !total || chip->chip_id >= VGPU_NUM_CHIPS || chip->n_interactions > VGPU_MAX_INTERACTIONS) return -1;
+    *air_constraints = vg_chip_base_constraints(chip->chip_id);
+    *total = *air_constraints + chip->n_interactions + 3;
+    return 0;
+}
+
+// Per rank, [total, failures per constraint] (u64 words): all-gathered when the chip is split, and then the totals size one block of
+// entries per rank, which one more all-gather exchanges.  Rank r's entries are rows of its run, below rank r + 1's: the list is the
+// ranks' lists in rank order.
+extern "C" int32_t vgpu_check_failures(vgpu_ctx* ctx, const vgpu_chip_desc* chip, const vgpu_dmat* main, const vgpu_dmat* prep_or_null,
+                                       const vgpu_dmat* perm, const uint32_t challenges[15], uint64_t cap, vgpu_check_failure* out,
+                                       uint64_t* n_out, uint64_t* total_failures, uint64_t* rows_per_constraint) {
+    if (!n_out || !total_failures || (cap && !out)) VG_FAIL(ctx, "check_failures: null output");
+    if (!chip || !main || !perm || !challenges) VG_FAIL(ctx, "check_failures: null argument");
+    VG_TRY(check_shapes(ctx, chip, main, prep_or_null, perm, true));
+    VG_TRY(vg_enter(ctx));
+    const uint32_t nc = vg_chip_base_constraints(chip->chip_id) + chip->n_interactions + 3;
+    const VgRun run = vg_trace_run(ctx, main->gh);
+    const uint32_t N = run.split ? (uint32_t)ctx->comm_size : 1, me = run.split ? (uint32_t)ctx->comm_rank : 0;
+    // the run's sweep of its rows but the last, then the window of the last row, when split; else one sweep of the whole trace
+    const uint32_t ctas = (uint32_t)((run.count - run.split + 127) / 128) + run.split;
+    const uint64_t words = 2 * (1 + (uint64_t)nc);
+    CheckSet set(ctx, 1);
+    set.plan(0, chip, main->gh);
+    VG_TRY(set.alloc());
+    VgBuf counts(ctx), cta(ctx), off(ctx), endb(ctx), ents(ctx);
+    VG_TRY(counts.alloc(N * words * 4));
+    VG_TRY(cta.alloc(ctas * 4ull));
+    VG_TRY(off.alloc(ctas * 8ull));
+    VG_TRY(endb.alloc(4));
+    unsigned long long* mine = counts.as<unsigned long long>() + (uint64_t)me * (1 + nc);
+    VG_CUDA(ctx, cudaMemsetAsync(mine, 0, words * 4, ctx->stream));
+    VG_CUDA(ctx, cudaMemsetAsync(cta.p, 0, ctas * 4ull, ctx->stream));
+    std::vector<std::unique_ptr<FParams>> sweeps;
+    uint32_t used = 0;
+    auto pass1 = [&](const vgpu_chip_desc* d, CParams& p) -> int32_t {
+        if (!p.n) return 0;
+        auto f = std::make_unique<FParams>();
+        f->c = p;
+        VG_TRY(vg_build_devchip(ctx, d, challenges, &f->c.chip));
+        f->cta_count = cta.as<uint32_t>(); f->cta_off = off.as<unsigned long long>(); f->hist = mine + 1; f->cta0 = used;
+        const uint32_t blocks = (uint32_t)((p.n + 127) / 128);
+        used += blocks;
+        KScope ks(ctx, KC_CHECK, 4.0 * (double)p.n * (double)(d->width + d->preprocessed_width + 5.0 * (d->n_interactions + 1)));
+        air::with_chip(d->chip_id, [&](auto c) { fail_count_kernel<decltype(c)::value><<<blocks, 128, 0, ctx->stream>>>(*f); });
+        VG_LAUNCH_CHECK(ctx);
+        sweeps.push_back(std::move(f));
+        return 0;
+    };
+    VG_TRY(set.sweep(0, main, prep_or_null, perm, challenges, pass1));
+    VG_TRY(set.windows(challenges, pass1));
+    {
+        KScope ks(ctx, KC_CHECK, 16.0 * used);
+        fail_scan_kernel<<<1, 1024, 0, ctx->stream>>>(cta.as<uint32_t>(), used, cap, off.as<unsigned long long>(), mine, endb.as<uint32_t>());
+        VG_LAUNCH_CHECK(ctx);
+    }
+    if (run.split) VG_TRY(vg_comm_allgather_inplace(ctx, counts.as<uint32_t>(), words));
+    std::vector<unsigned long long> hc((size_t)N * (1 + nc));
+    uint32_t end = 0;
+    VG_CUDA(ctx, cudaMemcpyAsync(hc.data(), counts.p, hc.size() * 8, cudaMemcpyDeviceToHost, ctx->stream));
+    VG_CUDA(ctx, cudaMemcpyAsync(&end, endb.p, 4, cudaMemcpyDeviceToHost, ctx->stream));
+    VG_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
+    uint64_t total = 0, block = 0;
+    for (uint32_t r = 0; r < N; r++) {
+        const uint64_t t = hc[(size_t)r * (1 + nc)];
+        total += t;
+        block = std::max(block, std::min<uint64_t>(t, cap));
+    }
+    uint64_t n = 0;
+    if (block) {                                          // alike on every rank: from the gathered totals
+        VG_TRY(ents.alloc(N * block * sizeof(vgpu_check_failure)));
+        for (auto& f : sweeps) {
+            if (end <= f->cta0) break;
+            f->out = ents.as<vgpu_check_failure>() + me * block; f->cap = cap;
+            const FParams& fp = *f;
+            const uint32_t grid = std::min<uint32_t>(end - f->cta0, (uint32_t)((f->c.n + 127) / 128));
+            KScope ks(ctx, KC_CHECK, 0.0);
+            air::with_chip(chip->chip_id, [&](auto c) { fail_write_kernel<decltype(c)::value><<<grid, 128, 0, ctx->stream>>>(fp); });
+            VG_LAUNCH_CHECK(ctx);
+        }
+        if (run.split) VG_TRY(vg_comm_allgather_inplace(ctx, ents.as<uint32_t>(), block * sizeof(vgpu_check_failure) / 4));
+        for (uint32_t r = 0; r < N && n < cap; r++) {
+            const uint64_t k = std::min<uint64_t>(std::min<uint64_t>(hc[(size_t)r * (1 + nc)], cap), cap - n);
+            if (k) VG_CUDA(ctx, cudaMemcpyAsync(out + n, ents.as<vgpu_check_failure>() + r * block, k * sizeof(vgpu_check_failure),
+                                                cudaMemcpyDeviceToHost, ctx->stream));
+            n += k;
+        }
+        VG_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
+    }
+    *n_out = n;
+    *total_failures = total;
+    if (rows_per_constraint)
+        for (uint32_t c = 0; c < nc; c++) {
+            uint64_t s = 0;
+            for (uint32_t r = 0; r < N; r++) s += hc[(size_t)r * (1 + nc) + 1 + c];
+            rows_per_constraint[c] = s;
+        }
     return 0;
 }
