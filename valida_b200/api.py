@@ -694,11 +694,12 @@ class StarkConfig:
         return self.pcs_
 
 
-def prove_machine(config, traces, device_resident=None):
+def prove_machine(config, traces, device_resident=None, repr=REPR_CANONICAL):
     """Machine::prove (machine/src/machine.rs:22-24): returns the CBOR bytes of MachineProof.
 
-    traces: MachineTraces (host, row-major canonical).  device_resident: optional pair
-    ([14 DeviceMatrix], [2 DeviceMatrix]) already uploaded (bench's HBM-resident timing)."""
+    traces: MachineTraces (host, row-major; every word in the representation `repr`: REPR_CANONICAL, or REPR_MONTY_R32 as the Rust
+    caller passes BabyBear's own words).  device_resident: optional pair ([14 DeviceMatrix], [2 DeviceMatrix]) already uploaded
+    (bench's HBM-resident timing); `repr` does not apply to it."""
     ctx = config.ctx
     out = C.POINTER(C.c_uint8)()
     n = C.c_uint64()
@@ -711,7 +712,7 @@ def prove_machine(config, traces, device_resident=None):
         keep = [_as_u32(m) for m in traces.main] + [_as_u32(m) for m in traces.preprocessed]
         a = (_Matrix * NUM_CHIPS)(*[_mat(m) for m in keep[:NUM_CHIPS]])
         b = (_Matrix * 2)(*[_mat(m) for m in keep[NUM_CHIPS:]])
-        ctx.check(lib().vgpu_prove(ctx._h, a, b, REPR_CANONICAL, C.byref(out), C.byref(n)))
+        ctx.check(lib().vgpu_prove(ctx._h, a, b, repr, C.byref(out), C.byref(n)))
     proof = C.string_at(out, n.value)
     lib().vgpu_free_bytes(out)
     return proof
@@ -808,15 +809,16 @@ class VerificationError(Exception):
         super().__init__("proof rejected: %s (verdict %d)" % (what, verdict))
 
 
-def verify_machine(config, proof, preprocessed):
+def verify_machine(config, proof, preprocessed, repr=REPR_CANONICAL):
     """Machine::verify (machine/src/machine.rs:26-31): raises VerificationError unless the proof is accepted.
 
-    proof: CBOR bytes of MachineProof; preprocessed: the two preprocessed traces (program, range), row-major canonical."""
+    proof: CBOR bytes of MachineProof; preprocessed: the two preprocessed traces (program, range), row-major, words in the
+    representation `repr` (REPR_CANONICAL or REPR_MONTY_R32)."""
     ctx = config.ctx
     keep = [_as_u32(m) for m in preprocessed]
     b = (_Matrix * 2)(*[_mat(m) for m in keep])
     verdict = C.c_int32(-1)
-    ctx.check(lib().vgpu_verify(ctx._h, bytes(proof), len(proof), b, REPR_CANONICAL, C.byref(verdict)))
+    ctx.check(lib().vgpu_verify(ctx._h, bytes(proof), len(proof), b, repr, C.byref(verdict)))
     if verdict.value != 0:
         raise VerificationError(verdict.value)
 
