@@ -582,12 +582,17 @@ def _u32arr(a, n):
     return (C.c_uint32 * n)(*[int(x) for x in a])
 
 
+def _h(m):
+    """The handle of an optional DeviceMatrix argument."""
+    return m._h if m is not None else None
+
+
 def generate_permutation_trace(ctx, chip_id, main, prep, random_elements):
     """machine/src/chip.rs:121 — returns (flattened perm trace DeviceMatrix, cumulative_sum[5])."""
     chip = lib().vgpu_basic_machine_chip(chip_id)
     out = C.c_void_p()
     cs = (C.c_uint32 * 5)()
-    ctx.check(lib().vgpu_perm_trace(ctx._h, chip, main._h, prep._h if prep is not None else None, _u32arr(random_elements, 15), C.byref(out), cs))
+    ctx.check(lib().vgpu_perm_trace(ctx._h, chip, main._h, _h(prep), _u32arr(random_elements, 15), C.byref(out), cs))
     return DeviceMatrix(ctx, out), np.array(list(cs), dtype=np.uint32)
 
 
@@ -595,30 +600,29 @@ def quotient(ctx, chip_id, log_degree, prep_lde, main_lde, perm_lde, cumulative_
     """machine/src/quotient.rs:18 — returns the h x 10 quotient-chunk DeviceMatrix."""
     chip = lib().vgpu_basic_machine_chip(chip_id)
     out = C.c_void_p()
-    ctx.check(lib().vgpu_quotient(ctx._h, chip, log_degree, prep_lde._h if prep_lde is not None else None, main_lde._h, perm_lde._h,
+    ctx.check(lib().vgpu_quotient(ctx._h, chip, log_degree, _h(prep_lde), main_lde._h, perm_lde._h,
                                   _u32arr(cumulative_sum, 5), _u32arr(perm_challenges, 15), _u32arr(alpha, 5), C.byref(out)))
     return DeviceMatrix(ctx, out)
+
+
+def _check_chip(fn, ctx, chip_id, main, prep, perm, perm_challenges):
+    row, con, n = C.c_int64(), C.c_uint32(), C.c_uint64()
+    ctx.check(fn(ctx._h, lib().vgpu_basic_machine_chip(chip_id), main._h, _h(prep), perm._h, _u32arr(perm_challenges, 15),
+                 C.byref(row), C.byref(con), C.byref(n)))
+    return int(row.value), int(con.value), int(n.value)
 
 
 def check_constraints(ctx, chip_id, main, prep, perm, perm_challenges):
     """machine/src/check_constraints.rs:14-84 on whole device traces (perm: the flattened permutation trace) — returns
     (first failing row or -1, index in eval order of its first failing constraint, number of rows with a failure)."""
-    chip = lib().vgpu_basic_machine_chip(chip_id)
-    row, con, n = C.c_int64(), C.c_uint32(), C.c_uint64()
-    ctx.check(lib().vgpu_check_constraints(ctx._h, chip, main._h, prep._h if prep is not None else None, perm._h,
-                                           _u32arr(perm_challenges, 15), C.byref(row), C.byref(con), C.byref(n)))
-    return int(row.value), int(con.value), int(n.value)
+    return _check_chip(lib().vgpu_check_constraints, ctx, chip_id, main, prep, perm, perm_challenges)
 
 
 def check_constraints_local(ctx, chip_id, main, prep, perm, perm_challenges):
     """check_constraints on a split context: every rank calls it with its own matrices (its row shards of the tall traces, or whole
     matrices) and gets what check_constraints returns for the whole traces on one GPU.  On a context that does not split proofs it is
     check_constraints."""
-    chip = lib().vgpu_basic_machine_chip(chip_id)
-    row, con, n = C.c_int64(), C.c_uint32(), C.c_uint64()
-    ctx.check(lib().vgpu_check_constraints_local(ctx._h, chip, main._h, prep._h if prep is not None else None, perm._h,
-                                                 _u32arr(perm_challenges, 15), C.byref(row), C.byref(con), C.byref(n)))
-    return int(row.value), int(con.value), int(n.value)
+    return _check_chip(lib().vgpu_check_constraints_local, ctx, chip_id, main, prep, perm, perm_challenges)
 
 
 def constraint_count(chip_id):
@@ -657,7 +661,7 @@ def check_failures(ctx, chip_id, main, prep, perm, perm_challenges, cap=1 << 16)
     out = np.zeros(int(cap), dtype=CHECK_FAILURE_DTYPE)
     per = np.zeros(total_constraints, dtype=np.uint64)
     n, total = C.c_uint64(), C.c_uint64()
-    ctx.check(lib().vgpu_check_failures(ctx._h, chip, main._h, prep._h if prep is not None else None, perm._h, _u32arr(perm_challenges, 15),
+    ctx.check(lib().vgpu_check_failures(ctx._h, chip, main._h, _h(prep), perm._h, _u32arr(perm_challenges, 15),
                                         int(cap), out.ctypes.data_as(C.c_void_p) if cap else None, C.byref(n), C.byref(total),
                                         per.ctypes.data_as(C.POINTER(C.c_uint64))))
     return out[:n.value].copy(), int(total.value), per

@@ -11,6 +11,10 @@
 // row's running sum) into a small block, one all-gather exchanges the blocks, and the last row is swept from a 2-row window (own
 // last row, next rank's first row; column-major, stride 2) as a run of one row whose next row is window row 1.  No peer pointers:
 // a borrowed shard is caller memory, outside the symmetric heap.
+// Every call plans its runs in one CheckSet: vgpu_check_constraints takes each chip's whole trace as its run on any context; the
+// other calls take this rank's run.  vgpu_check_witness and prove's debug mode drive one VgMachineCheck (devchip.h), which builds the
+// permutation traces and sweeps them through a CheckSet.  check_kernel and vgpu_check_failures' two passes set up and evaluate a row
+// with the same eval_row.
 // Result per chip: the first failing (row, constraint) as ONE 64-bit key (global row << 8 | constraint, atomicMin) and the number of
 // rows with at least one failure; both are aggregated per warp, so a clean trace costs no atomic at all.
 #include "ctx.h"
@@ -40,13 +44,38 @@ struct CParams {
     DevChip chip;
 };
 
-struct CheckBuilder {
+// What every check kernel's builder holds: the thread's row and its next row (main trace, pointers already offset to the rows),
+// the selectors, and the index of the next constraint.  Each builder adds what it does with a constraint that does not vanish.
+struct RowBuilder {
     using V = air::F;
-    const uint32_t* lrow; const uint32_t* nrow; uint64_t cs;   // pointers already offset to the row
+    const uint32_t* lrow; const uint32_t* nrow; uint64_t cs;
     F first, last, trans;
-    uint32_t idx, bad;                                         // next constraint index; first one that did not vanish
+    uint32_t idx;
     __device__ __forceinline__ F L(int c) const { return F{__ldg(lrow + (uint64_t)c * cs)}; }
     __device__ __forceinline__ F N(int c) const { return F{__ldg(nrow + (uint64_t)c * cs)}; }
+};
+
+// Sets up local row i of the run and evaluates every constraint on it, in eval order, into b.
+template <int CHIP, class B>
+__device__ __forceinline__ void eval_row(const CParams& p, uint64_t i, B& b) {
+    // the global row is p.g0 + i, recomputed where it is used: a register kept for it makes two chips spill
+    const bool is_last = p.g0 + i + 1 == p.h;
+    const uint64_t n = i + 1 < p.n ? i + 1 : p.wrap;       // a one-row chip is its own next row
+    b.lrow = p.main + i; b.nrow = p.main + n; b.cs = p.mcs;
+    b.first = F{p.g0 + i == 0 ? bb::R1 : 0u};
+    b.last = F{is_last ? bb::R1 : 0u};
+    b.trans = F{is_last ? 0u : bb::R1};
+    b.idx = 0;
+    air::eval_chip<CHIP>(b);
+    E5 cumsum;
+#pragma unroll
+    for (int l = 0; l < 5; l++) cumsum.c[l] = __ldg(p.cumsum + (uint64_t)l * p.ccs);
+    logup::eval_constraints(b, p.chip, b.lrow, b.nrow, p.mcs, p.prep ? p.prep + i : nullptr, p.prep ? p.prep + n : nullptr, p.pcs,
+                            p.perm + i, p.perm + n, p.qcs, cumsum);
+}
+
+struct CheckBuilder : RowBuilder {
+    uint32_t bad;                                              // the first constraint that did not vanish
     __device__ __forceinline__ void z(F x) { if (x.v != 0 && bad == CHECK_NONE) bad = idx; idx++; }
     __device__ __forceinline__ void z_ext(const E5& x) { if (!bb::e5_is_zero(x) && bad == CHECK_NONE) bad = idx; idx++; }
 };
@@ -56,21 +85,9 @@ __global__ void __launch_bounds__(128) check_kernel(const __grid_constant__ CPar
     const uint64_t i_raw = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
     const bool active = i_raw < p.n;
     const uint64_t i = active ? i_raw : p.n - 1;          // idle lanes shadow the last row (the warp vote needs every lane)
-    // the global row is p.g0 + i, recomputed where it is used: a register kept for it makes two chips spill
-    const bool is_last = p.g0 + i + 1 == p.h;
-    const uint64_t n = i + 1 < p.n ? i + 1 : p.wrap;       // a one-row chip is its own next row
     CheckBuilder b;
-    b.lrow = p.main + i; b.nrow = p.main + n; b.cs = p.mcs;
-    b.first = F{p.g0 + i == 0 ? bb::R1 : 0u};
-    b.last = F{is_last ? bb::R1 : 0u};
-    b.trans = F{is_last ? 0u : bb::R1};
-    b.idx = 0; b.bad = CHECK_NONE;
-    air::eval_chip<CHIP>(b);
-    E5 cumsum;
-#pragma unroll
-    for (int l = 0; l < 5; l++) cumsum.c[l] = __ldg(p.cumsum + (uint64_t)l * p.ccs);
-    logup::eval_constraints(b, p.chip, b.lrow, b.nrow, p.mcs, p.prep ? p.prep + i : nullptr, p.prep ? p.prep + n : nullptr, p.pcs,
-                            p.perm + i, p.perm + n, p.qcs, cumsum);
+    b.bad = CHECK_NONE;
+    eval_row<CHIP>(p, i, b);
     const bool fail = active && b.bad != CHECK_NONE;
     const unsigned vote = __ballot_sync(0xffffffffu, fail);
     // the lowest failing lane holds the warp's lowest row, hence its smallest key
@@ -153,13 +170,8 @@ struct FParams {
 
 __shared__ uint32_t fail_hist[CHECK_MAX_CONSTRAINTS];
 
-struct FailCountBuilder {
-    using V = air::F;
-    const uint32_t* lrow; const uint32_t* nrow; uint64_t cs;
-    F first, last, trans;
-    uint32_t idx; bool active;
-    __device__ __forceinline__ F L(int c) const { return F{__ldg(lrow + (uint64_t)c * cs)}; }
-    __device__ __forceinline__ F N(int c) const { return F{__ldg(nrow + (uint64_t)c * cs)}; }
+struct FailCountBuilder : RowBuilder {
+    bool active;
     // every lane reaches every constraint (the text has no branch on values): one shared atomic per warp and failing constraint
     __device__ __forceinline__ void tally(bool bad) {
         const unsigned v = __ballot_sync(0xffffffffu, active && bad);
@@ -171,15 +183,10 @@ struct FailCountBuilder {
 };
 
 // Counts the thread's failures while pos < end is false; then writes those at entries [pos, end) of the CTA's part of the list.
-struct FailWriteBuilder {
-    using V = air::F;
-    const uint32_t* lrow; const uint32_t* nrow; uint64_t cs;
-    F first, last, trans;
-    uint32_t idx, pos, end;
+struct FailWriteBuilder : RowBuilder {
+    uint32_t pos, end;
     vgpu_check_failure* out;                 // the CTA's first entry
     uint64_t row;
-    __device__ __forceinline__ F L(int c) const { return F{__ldg(lrow + (uint64_t)c * cs)}; }
-    __device__ __forceinline__ F N(int c) const { return F{__ldg(nrow + (uint64_t)c * cs)}; }
     __device__ __forceinline__ void put(const uint32_t* v, int limbs) {
         vgpu_check_failure* e = out + pos;
         e->row = (int64_t)row;
@@ -196,28 +203,6 @@ struct FailWriteBuilder {
     }
 };
 
-// the rows of one thread, as check_kernel sets them up
-template <class B>
-__device__ __forceinline__ void fail_rows(const CParams& p, uint64_t i, B& b) {
-    const bool is_last = p.g0 + i + 1 == p.h;
-    const uint64_t n = i + 1 < p.n ? i + 1 : p.wrap;
-    b.lrow = p.main + i; b.nrow = p.main + n; b.cs = p.mcs;
-    b.first = F{p.g0 + i == 0 ? bb::R1 : 0u};
-    b.last = F{is_last ? bb::R1 : 0u};
-    b.trans = F{is_last ? 0u : bb::R1};
-}
-template <int CHIP, class B>
-__device__ __forceinline__ void fail_eval(const CParams& p, uint64_t i, B& b) {
-    const uint64_t n = i + 1 < p.n ? i + 1 : p.wrap;
-    b.idx = 0;
-    air::eval_chip<CHIP>(b);
-    E5 cumsum;
-#pragma unroll
-    for (int l = 0; l < 5; l++) cumsum.c[l] = __ldg(p.cumsum + (uint64_t)l * p.ccs);
-    logup::eval_constraints(b, p.chip, b.lrow, b.nrow, p.mcs, p.prep ? p.prep + i : nullptr, p.prep ? p.prep + n : nullptr, p.pcs,
-                            p.perm + i, p.perm + n, p.qcs, cumsum);
-}
-
 template <int CHIP>
 __global__ void __maxnreg__(128) fail_count_kernel(const __grid_constant__ FParams f) {
     const CParams& p = f.c;
@@ -227,8 +212,7 @@ __global__ void __maxnreg__(128) fail_count_kernel(const __grid_constant__ FPara
     FailCountBuilder b;
     b.active = i_raw < p.n;
     const uint64_t i = b.active ? i_raw : p.n - 1;        // idle lanes shadow the last row (the warp vote needs every lane)
-    fail_rows(p, i, b);
-    fail_eval<CHIP>(p, i, b);
+    eval_row<CHIP>(p, i, b);
     __syncthreads();
     __shared__ uint32_t warp_total[4];
     uint32_t s = 0;
@@ -253,10 +237,9 @@ __global__ void __maxnreg__(128) fail_write_kernel(const __grid_constant__ FPara
     const bool active = i_raw < p.n;
     const uint64_t i = active ? i_raw : p.n - 1;
     FailWriteBuilder b;
-    fail_rows(p, i, b);
     b.out = f.out + base; b.row = p.g0 + i;
     b.pos = 0; b.end = 0;
-    fail_eval<CHIP>(p, i, b);
+    eval_row<CHIP>(p, i, b);
     // the thread's first entry: the failures of the CTA's lower threads
     __shared__ uint32_t warp_total[4];
     const uint32_t mine = active ? b.pos : 0, lane = threadIdx.x & 31;
@@ -273,7 +256,7 @@ __global__ void __maxnreg__(128) fail_write_kernel(const __grid_constant__ FPara
     const uint32_t end = (uint32_t)min((unsigned long long)total, f.cap - base);
     if (!mine || first >= end) return;
     b.pos = first; b.end = end;
-    fail_eval<CHIP>(p, i, b);
+    eval_row<CHIP>(p, i, b);
 }
 
 // One CTA: the exclusive prefix sum of the m per-CTA counts, their total, and *end = 1 + the last CTA with failures that starts below
@@ -322,64 +305,19 @@ __global__ void __launch_bounds__(1024) fail_scan_kernel(const uint32_t* count, 
 
 }  // namespace
 
-// Validates the arguments (before anything is enqueued) and enqueues the sweep of one chip's whole traces.  d_first / d_count must
-// hold ~0 / 0.
-int32_t vg_check_enqueue(vgpu_ctx* ctx, const vgpu_chip_desc* chip, const vgpu_dmat* main, const vgpu_dmat* prep, const vgpu_dmat* perm,
-                         const uint32_t challenges[15], unsigned long long* d_first, unsigned long long* d_count) {
-    if (!chip || !main || !perm || !challenges) VG_FAIL(ctx, "check_constraints: null argument");
-    VG_TRY(check_shapes(ctx, chip, main, prep, perm, false));
-    VG_TRY(vg_dmat_materialize(ctx, main));
-    VG_TRY(vg_dmat_materialize(ctx, prep));
-    VG_TRY(vg_dmat_materialize(ctx, perm));
-    auto pp = std::make_unique<CParams>();
-    CParams& p = *pp;
-    const uint64_t h = main->gh, k = chip->n_interactions;
-    p.main = main->d; p.mcs = main->col_stride;
-    p.prep = prep ? prep->d : nullptr; p.pcs = prep ? prep->col_stride : 0;
-    p.perm = perm->d; p.qcs = perm->col_stride;
-    p.cumsum = perm->d + 5 * k * perm->col_stride + h - 1; p.ccs = perm->col_stride;
-    p.g0 = 0; p.n = h; p.h = h; p.wrap = 0;
-    p.first = d_first; p.count = d_count;
-    return enqueue_sweep(ctx, chip, challenges, p);
-}
-
-void vg_check_decode(const unsigned long long first_count[2], int64_t* row, uint32_t* constraint, uint64_t* failing_rows) {
-    const unsigned long long key = first_count[0];
-    *row = key == ~0ull ? -1 : (int64_t)(key >> 8);
-    *constraint = key == ~0ull ? 0 : (uint32_t)(key & 0xff);
-    *failing_rows = first_count[1];
-}
-
-void vg_check_reports(const unsigned long long* chk, const uint32_t cumsum[VGPU_NUM_CHIPS][5], vgpu_check_report out[VGPU_NUM_CHIPS]) {
-    for (int i = 0; i < VGPU_NUM_CHIPS; i++) {
-        const unsigned long long fc[2] = {chk[i], chk[VGPU_NUM_CHIPS + i]};
-        vg_check_decode(fc, &out[i].first_row, &out[i].first_constraint, &out[i].failing_rows);
-        for (int l = 0; l < 5; l++) out[i].cumulative_sum[l] = cumsum[i][l];
-    }
-}
-
-bool vg_sums_cancel(const uint32_t cumsum[VGPU_NUM_CHIPS][5]) {
-    for (int l = 0; l < 5; l++) {
-        uint64_t s = 0;
-        for (int i = 0; i < VGPU_NUM_CHIPS; i++) s += cumsum[i][l];
-        if (s % bb::P) return false;
-    }
-    return true;
-}
-
 // The check of n chips on this rank of a split context (or of a lone one, where every chip is whole and nothing crosses ranks).
 // Per chip, sweep() enqueues the run's rows (all but the last when the chip is split) and packs the split chip's boundary words;
 // finish() then makes ONE all-gather of every split chip's block, sweeps the windows, and makes ONE all-gather of the verdicts.
-// Every rank plans from global heights alone, so all ranks make the same collectives.
-namespace {
+// Every rank plans from global heights alone, so all ranks make the same collectives.  `whole`: every chip is one run of its whole
+// traces, on any context (vgpu_check_constraints); no collective, one verdict slot.
 class CheckSet {
   public:
-    CheckSet(vgpu_ctx* ctx, uint32_t n) : ctx_(ctx), n_(n), chips_(n), block_(ctx), win_(ctx), verdicts_(ctx) {}
+    CheckSet(vgpu_ctx* ctx, uint32_t n, bool whole = false) : ctx_(ctx), n_(n), whole_(whole), chips_(n), block_(ctx), win_(ctx), store_(ctx) {}
 
     // the layout, from the chips and their global heights (before any sweep)
     void plan(uint32_t i, const vgpu_chip_desc* chip, uint64_t h) {
         Chip& c = chips_[i];
-        c.desc = chip; c.run = vg_trace_run(ctx_, h); c.h = h;
+        c.desc = chip; c.run = whole_ ? VgRun{0, h, false} : vg_trace_run(ctx_, h); c.h = h;
         c.wm = chip->width; c.wp = chip->preprocessed_width; c.wq = 5 * (chip->n_interactions + 1);
         if (c.run.split) {
             c.at = words_; words_ += c.wm + c.wp + c.wq + 5;
@@ -387,11 +325,16 @@ class CheckSet {
             any_split_ = true;
         }
     }
-    int32_t alloc() {
+    // verdicts: verdict_bytes() of device memory for the verdicts (VgMachineCheck's copy-back buffer); null: allocated here
+    int32_t alloc(unsigned long long* verdicts = nullptr) {
         const uint32_t N = any_split_ ? (uint32_t)ctx_->comm_size : 1;
         if (words_) VG_TRY(block_.alloc((size_t)N * words_ * 4));
         if (win_words_) VG_TRY(win_.alloc(win_words_ * 4));
-        VG_TRY(verdicts_.alloc((size_t)N * 2 * n_ * sizeof(unsigned long long)));
+        if (!verdicts) {
+            VG_TRY(store_.alloc(verdict_bytes()));
+            verdicts = store_.as<unsigned long long>();
+        }
+        verdicts_ = verdicts;
         unsigned long long* mine = own_verdicts();
         VG_CUDA(ctx_, cudaMemsetAsync(mine, 0xff, n_ * sizeof(unsigned long long), ctx_->stream));
         VG_CUDA(ctx_, cudaMemsetAsync(mine + n_, 0, n_ * sizeof(unsigned long long), ctx_->stream));
@@ -439,7 +382,7 @@ class CheckSet {
     int32_t finish(const uint32_t challenges[15]) {
         if (!any_split_) return 0;
         VG_TRY(windows(challenges));
-        return vg_comm_allgather_inplace(ctx_, (uint32_t*)verdicts_.p, 4 * (uint64_t)n_);
+        return vg_comm_allgather_inplace(ctx_, (uint32_t*)verdicts_, 4 * (uint64_t)n_);
     }
     // The exchange of the boundary blocks and the window sweeps (each the last row of a split chip's run, after its other rows).
     int32_t windows(const uint32_t challenges[15], const Sweep& run = nullptr) {
@@ -469,7 +412,7 @@ class CheckSet {
         return 0;
     }
     // every rank's verdicts, as finish() left them on the device
-    const void* verdicts() const { return verdicts_.p; }
+    const void* verdicts() const { return verdicts_; }
     size_t verdict_bytes() const { return (any_split_ ? (size_t)ctx_->comm_size : 1) * 2 * n_ * sizeof(unsigned long long); }
     // all: verdict_bytes() copied to the host -> out: [first keys n | failing-row counts n].  A split chip's rows are spread over the
     // ranks (min of the keys, sum of the counts); any other chip was swept whole by every rank and counts once, as rank 0 reports it.
@@ -488,34 +431,108 @@ class CheckSet {
   private:
     struct Chip { const vgpu_chip_desc* desc = nullptr; VgRun run{}; uint64_t h = 0, at = 0, win_at = 0; uint32_t wm = 0, wp = 0, wq = 0; };
     unsigned long long* own_verdicts() const {
-        return (unsigned long long*)verdicts_.p + (any_split_ ? (size_t)ctx_->comm_rank : 0) * 2 * n_;
+        return verdicts_ + (any_split_ ? (size_t)ctx_->comm_rank : 0) * 2 * n_;
     }
 
     vgpu_ctx* ctx_;
     uint32_t n_;
+    bool whole_;
     std::vector<Chip> chips_;
     uint64_t words_ = 0, win_words_ = 0;     // per-rank block words; window words of this rank
     bool any_split_ = false;
-    VgBuf block_, win_, verdicts_;
+    VgBuf block_, win_, store_;
+    unsigned long long* verdicts_ = nullptr;
 };
+
+namespace {
+
+void decode(unsigned long long first, unsigned long long count, int64_t* row, uint32_t* constraint, uint64_t* failing_rows) {
+    *row = first == ~0ull ? -1 : (int64_t)(first >> 8);
+    *constraint = first == ~0ull ? 0 : (uint32_t)(first & 0xff);
+    *failing_rows = count;
+}
+
+// One chip's check, its arguments validated: whole traces, or this rank's run (on a lone context, the whole trace).
+int32_t check_chip(vgpu_ctx* ctx, bool whole, const vgpu_chip_desc* chip, const vgpu_dmat* main, const vgpu_dmat* prep, const vgpu_dmat* perm,
+                   const uint32_t challenges[15], int64_t* first_row, uint32_t* first_constraint, uint64_t* failing_rows) {
+    VG_TRY(vg_enter(ctx));
+    CheckSet set(ctx, 1, whole);
+    set.plan(0, chip, main->gh);
+    VG_TRY(set.alloc());
+    VG_TRY(set.sweep(0, main, prep, perm, challenges));
+    VG_TRY(set.finish(challenges));
+    std::vector<unsigned long long> all(set.verdict_bytes() / sizeof(unsigned long long));
+    VG_CUDA(ctx, cudaMemcpyAsync(all.data(), set.verdicts(), set.verdict_bytes(), cudaMemcpyDeviceToHost, ctx->stream));
+    VG_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
+    unsigned long long fc[2];
+    set.reduce(all.data(), fc);
+    decode(fc[0], fc[1], first_row, first_constraint, failing_rows);
+    return 0;
+}
+
 }  // namespace
+
+VgMachineCheck::VgMachineCheck(vgpu_ctx* ctx, const vgpu_dmat* const main[VGPU_NUM_CHIPS], const vgpu_dmat* const prep[2],
+                               const uint32_t challenges[15], bool check)
+    : ctx_(ctx), main_(main), prep_(prep), challenges_(challenges), set_(check ? new CheckSet(ctx, VGPU_NUM_CHIPS) : nullptr), res_(ctx) {}
+
+VgMachineCheck::~VgMachineCheck() = default;
+
+int32_t VgMachineCheck::alloc() {
+    slots_ = vg_perm_totals_ranks(ctx_);
+    if (set_)
+        for (int i = 0; i < VGPU_NUM_CHIPS; i++) set_->plan(i, vgpu_basic_machine_chip(i), main_[i]->gh);
+    tot_at_ = set_ ? set_->verdict_bytes() / 4 : 0;
+    VG_TRY(res_.alloc((tot_at_ + (size_t)VGPU_NUM_CHIPS * slots_ * 5) * 4));
+    return set_ ? set_->alloc(res_.as<unsigned long long>()) : 0;
+}
+
+int32_t VgMachineCheck::perm(int i, VgMat* out) {
+    vgpu_dmat* pm = nullptr;
+    VG_TRY(vg_perm_trace_enqueue(ctx_, vgpu_basic_machine_chip(i), main_[i], prep_for(i), challenges_, &pm,
+                                 res_.as<uint32_t>() + tot_at_ + (size_t)i * slots_ * 5, &nt_[i]));
+    out->reset(pm);
+    return 0;
+}
+
+int32_t VgMachineCheck::sweep(int i, const vgpu_dmat* perm) {
+    // prove's debug mode refuses here what check_constraints refuses; vgpu_check_witness has refused it before enqueueing anything
+    VG_TRY(check_shapes(ctx_, vgpu_basic_machine_chip(i), main_[i], prep_for(i), perm, vg_sharded(ctx_)));
+    return set_->sweep(i, main_[i], prep_for(i), perm, challenges_);
+}
+
+int32_t VgMachineCheck::finish(uint32_t sums[VGPU_NUM_CHIPS][5], vgpu_check_report report[VGPU_NUM_CHIPS]) {
+    if (set_) VG_TRY(set_->finish(challenges_));
+    std::vector<uint32_t> host(tot_at_ + (size_t)VGPU_NUM_CHIPS * slots_ * 5);
+    VG_CUDA(ctx_, cudaMemcpyAsync(host.data(), res_.p, host.size() * 4, cudaMemcpyDeviceToHost, ctx_->stream));
+    VG_CUDA(ctx_, cudaStreamSynchronize(ctx_->stream));
+    unsigned long long chk[2 * VGPU_NUM_CHIPS];
+    for (int i = 0; i < VGPU_NUM_CHIPS; i++) { chk[i] = ~0ull; chk[VGPU_NUM_CHIPS + i] = 0; }
+    if (set_) set_->reduce((const unsigned long long*)host.data(), chk);
+    for (int i = 0; i < VGPU_NUM_CHIPS; i++) {
+        vg_perm_totals_fold(host.data() + tot_at_ + (size_t)i * slots_ * 5, nt_[i], sums[i]);
+        decode(chk[i], chk[VGPU_NUM_CHIPS + i], &report[i].first_row, &report[i].first_constraint, &report[i].failing_rows);
+        for (int l = 0; l < 5; l++) report[i].cumulative_sum[l] = bb::from_monty(sums[i][l]);
+    }
+    return 0;
+}
+
+bool vg_sums_cancel(const vgpu_check_report report[VGPU_NUM_CHIPS]) {
+    for (int l = 0; l < 5; l++) {
+        uint64_t s = 0;
+        for (int i = 0; i < VGPU_NUM_CHIPS; i++) s += report[i].cumulative_sum[l];
+        if (s % bb::P) return false;
+    }
+    return true;
+}
 
 extern "C" int32_t vgpu_check_constraints(vgpu_ctx* ctx, const vgpu_chip_desc* chip, const vgpu_dmat* main, const vgpu_dmat* prep_or_null,
                                           const vgpu_dmat* perm, const uint32_t challenges[15],
                                           int64_t* first_row, uint32_t* first_constraint, uint64_t* failing_rows) {
     if (!first_row || !first_constraint || !failing_rows) VG_FAIL(ctx, "check_constraints: null output");
-    VG_TRY(vg_enter(ctx));
-    VgBuf buf(ctx);
-    VG_TRY(buf.alloc(2 * sizeof(unsigned long long)));
-    unsigned long long* d = buf.as<unsigned long long>();
-    VG_CUDA(ctx, cudaMemsetAsync(d, 0xff, sizeof(unsigned long long), ctx->stream));
-    VG_CUDA(ctx, cudaMemsetAsync(d + 1, 0, sizeof(unsigned long long), ctx->stream));
-    VG_TRY(vg_check_enqueue(ctx, chip, main, prep_or_null, perm, challenges, d, d + 1));
-    unsigned long long h[2];
-    VG_CUDA(ctx, cudaMemcpyAsync(h, d, sizeof h, cudaMemcpyDeviceToHost, ctx->stream));
-    VG_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
-    vg_check_decode(h, first_row, first_constraint, failing_rows);
-    return 0;
+    if (!chip || !main || !perm || !challenges) VG_FAIL(ctx, "check_constraints: null argument");
+    VG_TRY(check_shapes(ctx, chip, main, prep_or_null, perm, false));
+    return check_chip(ctx, true, chip, main, prep_or_null, perm, challenges, first_row, first_constraint, failing_rows);
 }
 
 extern "C" int32_t vgpu_check_constraints_local(vgpu_ctx* ctx, const vgpu_chip_desc* chip, const vgpu_dmat* main, const vgpu_dmat* prep_or_null,
@@ -524,64 +541,27 @@ extern "C" int32_t vgpu_check_constraints_local(vgpu_ctx* ctx, const vgpu_chip_d
     if (!first_row || !first_constraint || !failing_rows) VG_FAIL(ctx, "check_constraints_local: null output");
     if (!chip || !main || !perm || !challenges) VG_FAIL(ctx, "check_constraints_local: null argument");
     VG_TRY(check_shapes(ctx, chip, main, prep_or_null, perm, true));
-    if (!vg_sharded(ctx)) return vgpu_check_constraints(ctx, chip, main, prep_or_null, perm, challenges, first_row, first_constraint, failing_rows);
-    VG_TRY(vg_enter(ctx));
-    CheckSet set(ctx, 1);
-    set.plan(0, chip, main->gh);
-    VG_TRY(set.alloc());
-    VG_TRY(set.sweep(0, main, prep_or_null, perm, challenges));
-    VG_TRY(set.finish(challenges));
-    std::vector<unsigned long long> all(set.verdict_bytes() / sizeof(unsigned long long));
-    VG_CUDA(ctx, cudaMemcpyAsync(all.data(), set.verdicts(), set.verdict_bytes(), cudaMemcpyDeviceToHost, ctx->stream));
-    VG_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
-    unsigned long long fc[2];
-    set.reduce(all.data(), fc);
-    vg_check_decode(fc, first_row, first_constraint, failing_rows);
-    return 0;
+    return check_chip(ctx, false, chip, main, prep_or_null, perm, challenges, first_row, first_constraint, failing_rows);
 }
 
 extern "C" int32_t vgpu_check_witness(vgpu_ctx* ctx, const vgpu_dmat* const main[VGPU_NUM_CHIPS], const vgpu_dmat* const prep[2],
                                       const uint32_t challenges[15], vgpu_check_report report[VGPU_NUM_CHIPS], int32_t* sums_cancel) {
     if (!main || !prep || !challenges || !report || !sums_cancel) VG_FAIL(ctx, "check_witness: null argument");
-    const vgpu_chip_desc* chips[VGPU_NUM_CHIPS];
-    auto prep_for = [&](int i) -> const vgpu_dmat* { return i == 1 ? prep[0] : i == 12 ? prep[1] : nullptr; };
+    VgMachineCheck mc(ctx, main, prep, challenges, true);
     for (int i = 0; i < VGPU_NUM_CHIPS; i++) {
-        chips[i] = vgpu_basic_machine_chip(i);
         if (!main[i]) VG_FAIL(ctx, "check_witness: chip %d has no trace", i);
-        VG_TRY(check_shapes(ctx, chips[i], main[i], prep_for(i), nullptr, true));
+        VG_TRY(check_shapes(ctx, vgpu_basic_machine_chip(i), main[i], mc.prep_for(i), nullptr, true));
     }
     VG_TRY(vg_enter(ctx));
-    CheckSet set(ctx, VGPU_NUM_CHIPS);
-    for (int i = 0; i < VGPU_NUM_CHIPS; i++) set.plan(i, chips[i], main[i]->gh);
-    VG_TRY(set.alloc());
-    const uint32_t slots = vg_perm_totals_ranks(ctx);
-    const size_t tot_words = (size_t)VGPU_NUM_CHIPS * slots * 5, tot_at = (set.verdict_bytes() + 3) / 4;
-    VgBuf res(ctx);                                   // the verdicts, then the LogUp totals: one copy back
-    VG_TRY(res.alloc((tot_at + tot_words) * 4));
-    uint32_t* d_tot = res.as<uint32_t>() + tot_at;
-    uint32_t nt[VGPU_NUM_CHIPS];
+    VG_TRY(mc.alloc());
     for (int i = 0; i < VGPU_NUM_CHIPS; i++) {
-        vgpu_dmat* pm = nullptr;
-        VG_TRY(vg_perm_trace_enqueue(ctx, chips[i], main[i], prep_for(i), challenges, &pm, d_tot + (size_t)i * slots * 5, &nt[i]));
-        VgMat perm(pm);                               // back to the cache once the sweep that reads it is enqueued
-        VG_TRY(set.sweep(i, main[i], prep_for(i), perm.get(), challenges));
+        VgMat perm;                                   // back to the cache once the sweep that reads it is enqueued
+        VG_TRY(mc.perm(i, &perm));
+        VG_TRY(mc.sweep(i, perm.get()));
     }
-    VG_TRY(set.finish(challenges));
-    VG_CUDA(ctx, cudaMemcpyAsync(res.p, set.verdicts(), set.verdict_bytes(), cudaMemcpyDeviceToDevice, ctx->stream));
-    std::vector<uint32_t> host(tot_at + tot_words);
-    VG_CUDA(ctx, cudaMemcpyAsync(host.data(), res.p, host.size() * 4, cudaMemcpyDeviceToHost, ctx->stream));
-    VG_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
-    unsigned long long chk[2 * VGPU_NUM_CHIPS];
-    set.reduce((const unsigned long long*)host.data(), chk);
-    uint32_t cumsum[VGPU_NUM_CHIPS][5];
-    for (int i = 0; i < VGPU_NUM_CHIPS; i++)
-        for (int l = 0; l < 5; l++) {
-            uint32_t a = 0;
-            for (uint32_t r = 0; r < nt[i]; r++) a = bb::add(a, host[tot_at + ((size_t)i * slots + r) * 5 + l]);
-            cumsum[i][l] = bb::from_monty(a);
-        }
-    vg_check_reports(chk, cumsum, report);
-    *sums_cancel = vg_sums_cancel(cumsum) ? 1 : 0;
+    uint32_t sums[VGPU_NUM_CHIPS][5];
+    VG_TRY(mc.finish(sums, report));
+    *sums_cancel = vg_sums_cancel(report) ? 1 : 0;
     return 0;
 }
 

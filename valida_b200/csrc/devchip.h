@@ -28,11 +28,36 @@ int32_t vg_ext_batch_inverse(vgpu_ctx* ctx, uint32_t* data, uint64_t cs, uint64_
 int32_t vg_perm_trace_enqueue(vgpu_ctx* ctx, const vgpu_chip_desc* chip, const vgpu_dmat* main, const vgpu_dmat* prep_or_null,
                               const uint32_t challenges[15], vgpu_dmat** out_perm, uint32_t* d_totals, uint32_t* n_totals);
 uint32_t vg_perm_totals_ranks(const vgpu_ctx* ctx);
-// check.cu — check_constraints of one chip on whole traces; d_first / d_count must hold ~0 / 0 before the sweep
-int32_t vg_check_enqueue(vgpu_ctx* ctx, const vgpu_chip_desc* chip, const vgpu_dmat* main, const vgpu_dmat* prep_or_null, const vgpu_dmat* perm,
-                         const uint32_t challenges[15], unsigned long long* d_first, unsigned long long* d_count);
-void vg_check_decode(const unsigned long long first_count[2], int64_t* row, uint32_t* constraint, uint64_t* failing_rows);
-// the 14 chips' verdicts (first keys [14], then failing-row counts [14]) and canonical cumulative sums -> reports
-void vg_check_reports(const unsigned long long* chk, const uint32_t cumsum[VGPU_NUM_CHIPS][5], vgpu_check_report out[VGPU_NUM_CHIPS]);
+// the cumulative sum (Montgomery) from the n per-rank totals ([rank][limb]) vg_perm_trace_enqueue left for a chip
+void vg_perm_totals_fold(const uint32_t* totals, uint32_t n, uint32_t out[5]);
+
+// check.cu — the permutation traces of a machine witness (14 chips, prep[0] / prep[1] the preprocessed traces of chips 1 / 12) and,
+// when `check`, check_constraints of every chip on this rank's run: vgpu_check_witness and prove's debug mode.  perm(i) enqueues
+// chip i's permutation trace; sweep(i) (checking only) its check, which reads the trace before later work on the stream.  finish()
+// runs the split chips' windows and the verdict all-gather, then brings the LogUp totals and the verdicts back with ONE copy and one
+// synchronisation.  main, prep and challenges must outlive the object.
+class CheckSet;
+class VgMachineCheck {
+  public:
+    VgMachineCheck(vgpu_ctx* ctx, const vgpu_dmat* const main[VGPU_NUM_CHIPS], const vgpu_dmat* const prep[2], const uint32_t challenges[15],
+                   bool check);
+    ~VgMachineCheck();
+    const vgpu_dmat* prep_for(int i) const { return i == 1 ? prep_[0] : i == 12 ? prep_[1] : nullptr; }
+    int32_t alloc();                                  // reads the traces' heights; enqueues nothing unless checking
+    int32_t perm(int i, VgMat* out);
+    int32_t sweep(int i, const vgpu_dmat* perm);
+    // sums: the cumulative sums (Montgomery); report: the same canonical and each chip's verdict (none failing unless checking)
+    int32_t finish(uint32_t sums[VGPU_NUM_CHIPS][5], vgpu_check_report report[VGPU_NUM_CHIPS]);
+
+  private:
+    vgpu_ctx* ctx_;
+    const vgpu_dmat* const* main_;
+    const vgpu_dmat* const* prep_;
+    const uint32_t* challenges_;
+    std::unique_ptr<CheckSet> set_;                   // null unless checking
+    VgBuf res_;                                       // the verdicts (checking only), then the LogUp totals [chip][rank][limb]
+    size_t tot_at_ = 0;                               // words
+    uint32_t slots_ = 0, nt_[VGPU_NUM_CHIPS] = {};
+};
 // check_cumulative_sums (machine/src/check_constraints.rs:87-93): the canonical sums of the 14 chips add to zero
-bool vg_sums_cancel(const uint32_t cumsum[VGPU_NUM_CHIPS][5]);
+bool vg_sums_cancel(const vgpu_check_report report[VGPU_NUM_CHIPS]);

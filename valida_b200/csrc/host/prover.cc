@@ -328,12 +328,10 @@ int32_t debug_mode_allowed(vgpu_ctx* ctx) {
     return 0;
 }
 
-// check_constraints of every chip (first keys [14], then failing-row counts [14]) and check_cumulative_sums
-// (machine/src/check_constraints.rs:87-93): an error naming every failure, or 0.
-int32_t debug_verdict(vgpu_ctx* ctx, const unsigned long long* chk, const uint32_t cumsum[VGPU_NUM_CHIPS][5]) {
+// check_constraints of every chip and check_cumulative_sums (machine/src/check_constraints.rs:87-93): an error naming every failure,
+// or 0.
+int32_t debug_verdict(vgpu_ctx* ctx, const vgpu_check_report rep[VGPU_NUM_CHIPS]) {
     static const char* NAMES[VGPU_NUM_CHIPS] = {"cpu", "program", "mem", "add", "sub", "mul", "div", "shift", "lt", "com", "bitwise", "output", "range", "static_data"};
-    vgpu_check_report rep[VGPU_NUM_CHIPS];
-    vg_check_reports(chk, cumsum, rep);
     std::string msg;
     for (int i = 0; i < VGPU_NUM_CHIPS; i++) {
         if (rep[i].first_row < 0) continue;
@@ -342,7 +340,7 @@ int32_t debug_verdict(vgpu_ctx* ctx, const unsigned long long* chk, const uint32
                  (long long)rep[i].first_row, (unsigned long long)rep[i].failing_rows);
         msg += (msg.empty() ? "" : "; ") + std::string(b);
     }
-    if (!vg_sums_cancel(cumsum)) msg += (msg.empty() ? "" : "; ") + std::string("cumulative sums do not cancel");
+    if (!vg_sums_cancel(rep)) msg += (msg.empty() ? "" : "; ") + std::string("cumulative sums do not cancel");
     if (msg.empty()) return 0;
     ctx->err = "prove: debug checks failed: " + msg;
     return -1;
@@ -411,7 +409,6 @@ static int32_t prove_device(vgpu_ctx* ctx, const vgpu_dmat* const main[VGPU_NUM_
                             vgpu_dmat* const* owned_main, uint8_t** proof_out, uint64_t* proof_len) {
     VG_TRY(debug_mode_allowed(ctx));
     const bool debug = ctx->debug_checks;
-    auto prep_for = [&](int i) -> const vgpu_dmat* { return i == 1 ? prep[0] : i == 12 ? prep[1] : nullptr; };
     if (!ctx->challenger_set) VG_FAIL(ctx, "prove: vgpu_set_challenger has not been called");
     if (!proof_out || !proof_len) VG_FAIL(ctx, "prove: null output");
     VG_TRY(vg_enter(ctx));
@@ -469,37 +466,24 @@ static int32_t prove_device(vgpu_ctx* ctx, const vgpu_dmat* const main[VGPU_NUM_
         std::vector<VgMat> perms;
         {
             Phase ph(ctx, "permutation traces");
-            // the cumulative sums of all chips come back with ONE copy: per chip the per-rank sums of its running sum
-            // (debug mode: the check results of the 14 chips, first keys then failing-row counts, ride in the same buffer and copy)
-            const uint32_t slots = vg_perm_totals_ranks(ctx);
-            const size_t tot_words = (size_t)VGPU_NUM_CHIPS * slots * 5, chk_words = debug ? 4 * VGPU_NUM_CHIPS : 0;
-            VgBuf tot(ctx);
-            VG_TRY(tot.alloc((tot_words + chk_words) * 4));
-            uint32_t nt[VGPU_NUM_CHIPS];
-            for (int i = 0; i < VGPU_NUM_CHIPS; i++) {
-                vgpu_dmat* pm = nullptr;
-                VG_TRY(vg_perm_trace_enqueue(ctx, chips[i], main[i], prep_for(i), perm_challenges, &pm, tot.as<uint32_t>() + (size_t)i * slots * 5, &nt[i]));
-                perms.emplace_back(pm);
-            }
+            // the cumulative sums of all chips come back with ONE copy (debug mode: with the check results of the 14 chips)
+            VgMachineCheck mc(ctx, main, prep, perm_challenges, debug);
+            VG_TRY(mc.alloc());
+            perms.resize(VGPU_NUM_CHIPS);
+            for (int i = 0; i < VGPU_NUM_CHIPS; i++) VG_TRY(mc.perm(i, &perms[i]));
             if (debug) {   // check_constraints (derive/src/lib.rs:246-253) while the main traces are still held
                 Phase pc(ctx, "check constraints");
-                unsigned long long* d_chk = (unsigned long long*)(tot.as<uint32_t>() + tot_words);   // tot_words is even: 8-byte aligned
-                VG_CUDA(ctx, cudaMemsetAsync(d_chk, 0xff, VGPU_NUM_CHIPS * 8, ctx->stream));
-                VG_CUDA(ctx, cudaMemsetAsync(d_chk + VGPU_NUM_CHIPS, 0, VGPU_NUM_CHIPS * 8, ctx->stream));
-                for (int i = 0; i < VGPU_NUM_CHIPS; i++)
-                    VG_TRY(vg_check_enqueue(ctx, chips[i], main[i], prep_for(i), perms[i].get(), perm_challenges, d_chk + i, d_chk + VGPU_NUM_CHIPS + i));
+                for (int i = 0; i < VGPU_NUM_CHIPS; i++) VG_TRY(mc.sweep(i, perms[i].get()));
             }
-            std::vector<uint32_t> ht(tot_words + chk_words);
-            VG_CUDA(ctx, cudaMemcpyAsync(ht.data(), tot.p, ht.size() * 4, cudaMemcpyDeviceToHost, ctx->stream));
-            VG_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
+            uint32_t sums[VGPU_NUM_CHIPS][5];
+            vgpu_check_report rep[VGPU_NUM_CHIPS];
+            VG_TRY(mc.finish(sums, rep));
             for (int i = 0; i < VGPU_NUM_CHIPS; i++)
                 for (int l = 0; l < 5; l++) {
-                    uint32_t a = 0;
-                    for (uint32_t r = 0; r < nt[i]; r++) a = bb::add(a, ht[((size_t)i * slots + r) * 5 + l]);
-                    mp.chip_proofs[i].cumulative_sum.c[l] = a;
-                    cumsum[i][l] = bb::from_monty(a);
+                    mp.chip_proofs[i].cumulative_sum.c[l] = sums[i][l];
+                    cumsum[i][l] = rep[i].cumulative_sum[l];
                 }
-            if (debug) VG_TRY(debug_verdict(ctx, (const unsigned long long*)(ht.data() + tot_words), cumsum));
+            if (debug) VG_TRY(debug_verdict(ctx, rep));
             // later work reuses the released blocks in stream order, i.e. after the permutation kernels that read them
             for (int i = 0; owned_main && i < VGPU_NUM_CHIPS; i++) {
                 vgpu_dmat* m = owned_main[i];

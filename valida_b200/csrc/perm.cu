@@ -276,6 +276,14 @@ int32_t vg_perm_trace_enqueue(vgpu_ctx* ctx, const vgpu_chip_desc* chip, const v
 }
 uint32_t vg_perm_totals_ranks(const vgpu_ctx* ctx) { return vg_sharded(ctx) ? (uint32_t)ctx->comm_size : 1; }
 
+void vg_perm_totals_fold(const uint32_t* totals, uint32_t n, uint32_t out[5]) {
+    for (int l = 0; l < 5; l++) {
+        uint32_t a = 0;
+        for (uint32_t r = 0; r < n; r++) a = bb::add(a, totals[r * 5 + l]);
+        out[l] = a;
+    }
+}
+
 extern "C" int32_t vgpu_perm_trace(vgpu_ctx* ctx, const vgpu_chip_desc* chip, const vgpu_dmat* main, const vgpu_dmat* prep_or_null,
                                    const uint32_t challenges[15], vgpu_dmat** out_perm, uint32_t cumulative_sum_out[5]) {
     VG_TRY(vg_enter(ctx));
@@ -289,11 +297,8 @@ extern "C" int32_t vgpu_perm_trace(vgpu_ctx* ctx, const vgpu_chip_desc* chip, co
         cudaError_t e = cudaMemcpyAsync(tot, d_tot.p, nt * 5 * 4, cudaMemcpyDeviceToHost, ctx->stream);
         if (e == cudaSuccess) e = cudaStreamSynchronize(ctx->stream);
         if (e != cudaSuccess) VG_FAIL(ctx, "perm_trace: reading the cumulative sum failed: %s", cudaGetErrorString(e));
-        for (int l = 0; l < 5; l++) {
-            uint32_t a = 0;
-            for (uint32_t p = 0; p < nt; p++) a = bb::add(a, tot[p * 5 + l]);
-            cumulative_sum_out[l] = bb::from_monty(a);
-        }
+        vg_perm_totals_fold(tot, nt, cumulative_sum_out);
+        for (int l = 0; l < 5; l++) cumulative_sum_out[l] = bb::from_monty(cumulative_sum_out[l]);
     }
     return 0;
 }
