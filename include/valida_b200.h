@@ -282,6 +282,39 @@ typedef struct vgpu_check_report {
 int32_t vgpu_check_witness(vgpu_ctx* ctx, const vgpu_dmat* const main[VGPU_NUM_CHIPS], const vgpu_dmat* const prep[2],
                            const uint32_t challenges[15], vgpu_check_report report[VGPU_NUM_CHIPS], int32_t* sums_cancel);
 
+/* One EVENT of a machine witness: a row of a chip and one of its interactions whose multiplicity (the count VirtualPairCol on the
+ * row) is not zero.  Its tuple is the interaction's fields on the row; send counts +, receive -. */
+typedef struct vgpu_bus_event {
+    uint32_t chip, interaction;   /* chip id; index in the chip's interaction list */
+    int64_t row;                  /* global trace row */
+    uint32_t multiplicity;        /* canonical, != 0 */
+    uint32_t is_send;
+} vgpu_bus_event;
+/* A tuple whose sends minus receives are not 0 mod p.  Two events carry the same tuple when the LogUp denominator cannot tell them
+ * apart: the same bus and equal field vectors once zero-padded to VGPU_MAX_FIELDS (trailing zeros do not distinguish tuples). */
+typedef struct vgpu_bus_imbalance {
+    uint32_t bus;
+    uint32_t fields[VGPU_MAX_FIELDS];  /* canonical, zero-padded */
+    uint32_t net;                      /* sends - receives mod p, canonical, != 0 */
+    uint64_t first_event, n_events;    /* this tuple's events: events[first_event, first_event + n_events) */
+} vgpu_bus_imbalance;
+/* Every bus tuple a machine witness leaves unbalanced, with every event that sends or receives it: where vgpu_check_witness can only
+ * say that the cumulative sums do not cancel, this names the bus, the tuple and the rows.  Takes what vgpu_check_witness takes (whole
+ * matrices, or this rank's row shards on a split context) and refuses what it refuses, and null outputs (tuples and events only when
+ * cap > 0), before anything is enqueued and alike on every rank.  Writes:
+ *   - tuples[0, *n_tuples): unbalanced tuples in ascending (bus, fields) order;
+ *   - events[0, *n_events): their events, each tuple's in ascending (chip, row, interaction) order;
+ *   - *unexamined: the number of candidate groups (tuples sharing a hash bucket whose weighted sum is not zero) whose events did
+ *     not fit under cap, which bounds both arrays; 0: the list is complete.  A reported tuple's net is always computed from all
+ *     of its events.
+ * The list is empty exactly when the LogUp sums cancel (with overwhelming probability over the 15 challenge words, which weight the
+ * buckets).  Collective on a split context, with byte-identical output on every rank (all-gathers of the bucket sums, the candidate
+ * counts and the examined events).  Synchronises; the traces are left untouched. */
+int32_t vgpu_check_buses(vgpu_ctx* ctx, const vgpu_dmat* const main[VGPU_NUM_CHIPS], const vgpu_dmat* const prep[2],
+                         const uint32_t challenges[15], uint64_t cap,
+                         vgpu_bus_imbalance* tuples, uint64_t* n_tuples,
+                         vgpu_bus_event* events, uint64_t* n_events, uint64_t* unexamined);
+
 /* ---- Fiat-Shamir transcript owned by the context (DuplexChallenger; config.challenger() clone) ------
  * reset() restores the initial sponge of vgpu_set_challenger; values are canonical words. */
 int32_t vgpu_challenger_reset(vgpu_ctx* ctx);

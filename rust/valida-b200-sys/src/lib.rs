@@ -120,6 +120,35 @@ pub struct vgpu_check_report {
     pub cumulative_sum: [u32; 5],
 }
 
+/// One event of a machine witness ([`vgpu_check_buses`]): a row of a chip and one of its interactions with a non-zero multiplicity.
+#[repr(C)]
+#[derive(Clone, Copy, Debug, Default, PartialEq, Eq)]
+pub struct vgpu_bus_event {
+    /// Chip id.
+    pub chip: u32,
+    /// Index in the chip's interaction list.
+    pub interaction: u32,
+    /// Global trace row.
+    pub row: i64,
+    /// Canonical, non-zero.
+    pub multiplicity: u32,
+    pub is_send: u32,
+}
+
+/// A bus tuple whose sends minus receives are not 0 mod p ([`vgpu_check_buses`]).
+#[repr(C)]
+#[derive(Clone, Copy, Debug, Default, PartialEq, Eq)]
+pub struct vgpu_bus_imbalance {
+    pub bus: u32,
+    /// Canonical, zero-padded.
+    pub fields: [u32; VGPU_MAX_FIELDS],
+    /// Sends minus receives mod p, canonical, non-zero.
+    pub net: u32,
+    /// This tuple's events are `events[first_event..first_event + n_events]`.
+    pub first_event: u64,
+    pub n_events: u64,
+}
+
 extern "C" {
     // ---- context ----
     pub fn vgpu_ctx_create(device: i32, cuda_stream: *mut c_void, out: *mut *mut vgpu_ctx) -> i32;
@@ -176,6 +205,7 @@ extern "C" {
     pub fn vgpu_chip_constraint_count(chip: *const vgpu_chip_desc, air_constraints: *mut u32, total: *mut u32) -> i32;
     pub fn vgpu_check_failures(ctx: *mut vgpu_ctx, chip: *const vgpu_chip_desc, main: *const vgpu_dmat, prep_or_null: *const vgpu_dmat, perm: *const vgpu_dmat, challenges: *const u32, cap: u64, out: *mut vgpu_check_failure, n_out: *mut u64, total_failures: *mut u64, rows_per_constraint: *mut u64) -> i32;
     pub fn vgpu_check_witness(ctx: *mut vgpu_ctx, main: *const *const vgpu_dmat, prep: *const *const vgpu_dmat, challenges: *const u32, report: *mut vgpu_check_report, sums_cancel: *mut i32) -> i32;
+    pub fn vgpu_check_buses(ctx: *mut vgpu_ctx, main: *const *const vgpu_dmat, prep: *const *const vgpu_dmat, challenges: *const u32, cap: u64, tuples: *mut vgpu_bus_imbalance, n_tuples: *mut u64, events: *mut vgpu_bus_event, n_events: *mut u64, unexamined: *mut u64) -> i32;
 
     // ---- transcript ----
     pub fn vgpu_challenger_reset(ctx: *mut vgpu_ctx) -> i32;

@@ -420,6 +420,26 @@ impl Context {
         Ok((reports, cancel != 0))
     }
 
+    /// Every bus tuple the witness leaves unbalanced, with every event that sends or receives it: the tuples in ascending (bus,
+    /// fields) order, the events (tuple `t`'s at `t.first_event..t.first_event + t.n_events`, ascending by (chip, row, interaction))
+    /// and the number of candidate groups whose events did not fit under `cap` (0: the list is complete).  Takes what
+    /// [`Context::check_witness`] takes; collective on a split context, with the same result on every rank.  Synchronises.
+    pub fn check_buses(&self, main: &[&DMat<'_>; sys::VGPU_NUM_CHIPS], prep: &[&DMat<'_>; 2], challenges: &[u32; 15], cap: usize)
+                       -> Result<(Vec<sys::vgpu_bus_imbalance>, Vec<sys::vgpu_bus_event>, u64)> {
+        let main_raw: Vec<*const vgpu_dmat> = main.iter().map(|m| m.as_ptr()).collect();
+        let prep_raw: Vec<*const vgpu_dmat> = prep.iter().map(|m| m.as_ptr()).collect();
+        let mut tuples = vec![sys::vgpu_bus_imbalance::default(); cap];
+        let mut events = vec![sys::vgpu_bus_event::default(); cap];
+        let (mut nt, mut ne, mut unexamined) = (0u64, 0u64, 0u64);
+        self.check(unsafe {
+            sys::vgpu_check_buses(self.raw, main_raw.as_ptr(), prep_raw.as_ptr(), challenges.as_ptr(), cap as u64, tuples.as_mut_ptr(), &mut nt,
+                                  events.as_mut_ptr(), &mut ne, &mut unexamined)
+        })?;
+        tuples.truncate(nt as usize);
+        events.truncate(ne as usize);
+        Ok((tuples, events, unexamined))
+    }
+
     /// Kernels launched by this context so far.
     pub fn launch_count(&self) -> u64 {
         unsafe { sys::vgpu_ctx_launch_count(self.raw) }

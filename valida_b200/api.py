@@ -8,6 +8,7 @@ Reference interfaces mirrored (names and argument meaning kept):
 Errors: the reference panics (derive/src/lib.rs:319,364,396); here every non-zero status raises
 VgpuError carrying vgpu_last_error().
 """
+import collections
 import ctypes as C
 import os
 import weakref
@@ -57,6 +58,12 @@ class _ChipDesc(C.Structure):
 
 # vgpu_check_failure: one (row, constraint) on which a chip's check does not vanish, and the constraint's canonical value there
 CHECK_FAILURE_DTYPE = np.dtype([("row", "<i8"), ("constraint", "<u4"), ("value", "<u4", (5,))])
+# vgpu_bus_event / vgpu_bus_imbalance (include/valida_b200.h)
+BUS_EVENT_DTYPE = np.dtype([("chip", "<u4"), ("interaction", "<u4"), ("row", "<i8"), ("multiplicity", "<u4"), ("is_send", "<u4")])
+BUS_IMBALANCE_DTYPE = np.dtype([("bus", "<u4"), ("fields", "<u4", (14,)), ("net", "<u4"), ("first_event", "<u8"), ("n_events", "<u8")], align=True)
+# BasicMachine's chips and buses (basic/src/lib.rs:151-166, 1190-1212), by id
+CHIP_NAMES = ("cpu", "program", "memory", "add", "sub", "mul", "div", "shift", "lt", "com", "bitwise", "output", "range", "static_data")
+BUS_NAMES = ("general", "program", "memory", "range")
 
 
 def _load():
@@ -109,6 +116,7 @@ def _load():
         "vgpu_chip_constraint_count": (C.c_int32, [vp, u32p, u32p]),
         "vgpu_check_failures": (C.c_int32, [vp, vp, vp, vp, vp, u32p, u64, vp, C.POINTER(u64), C.POINTER(u64), C.POINTER(u64)]),
         "vgpu_check_witness": (C.c_int32, [vp, C.POINTER(vp), C.POINTER(vp), u32p, C.POINTER(_CheckReport), C.POINTER(C.c_int32)]),
+        "vgpu_check_buses": (C.c_int32, [vp, C.POINTER(vp), C.POINTER(vp), u32p, u64, vp, C.POINTER(u64), vp, C.POINTER(u64), C.POINTER(u64)]),
         "vgpu_ctx_set_debug_checks": (C.c_int32, [vp, C.c_int32]),
         "vgpu_set_challenger": (C.c_int32, [vp, u32p, u32p]),
         "vgpu_ctx_set_merkle_hash": (C.c_int32, [vp, C.c_int32]),
@@ -678,6 +686,41 @@ def check_witness(ctx, main, prep, challenges):
     ctx.check(lib().vgpu_check_witness(ctx._h, a, b, _u32arr(challenges, 15), rep, C.byref(cancel)))
     return ([(int(r.first_row), int(r.first_constraint), int(r.failing_rows), np.array(list(r.cumulative_sum), dtype=np.uint32)) for r in rep],
             bool(cancel.value))
+
+
+BusEvent = collections.namedtuple("BusEvent", "chip chip_name interaction row multiplicity send")
+BusImbalance = collections.namedtuple("BusImbalance", "bus bus_name fields net events")
+BusCheck = collections.namedtuple("BusCheck", "tuples complete unexamined")
+
+
+def check_buses(ctx, main, prep, challenges, cap=1 << 16):
+    """Every bus tuple the witness leaves unbalanced (sends minus receives not 0 mod p), with every event that sends or receives it.
+    Takes what check_witness takes (whole traces, or this rank's row shards on a split context, where every rank calls it and gets
+    the same answer).  Returns BusCheck(tuples, complete, unexamined): tuples in ascending (bus, fields) order, each a
+    BusImbalance(bus, bus_name, fields trimmed of trailing zeros, net as a signed integer in (-p/2, p/2], events), its events
+    BusEvent(chip, chip_name, interaction, row, multiplicity, send) in ascending (chip, row, interaction) order.  cap bounds the events
+    (and so the tuples) examined; complete is False when unexamined > 0 candidate groups did not fit, and every tuple listed is exact
+    either way.  The list is empty exactly when the LogUp sums cancel."""
+    a = (C.c_void_p * NUM_CHIPS)(*[m._h for m in main])
+    b = (C.c_void_p * 2)(*[m._h for m in prep])
+    cap = int(cap)
+    tup = np.zeros(cap, dtype=BUS_IMBALANCE_DTYPE)
+    ev = np.zeros(cap, dtype=BUS_EVENT_DTYPE)
+    nt, ne, un = C.c_uint64(), C.c_uint64(), C.c_uint64()
+    ctx.check(lib().vgpu_check_buses(ctx._h, a, b, _u32arr(challenges, 15), cap, tup.ctypes.data_as(C.c_void_p) if cap else None,
+                                     C.byref(nt), ev.ctypes.data_as(C.c_void_p) if cap else None, C.byref(ne), C.byref(un)))
+    out = []
+    for t in tup[:nt.value]:
+        fields = [int(x) for x in t["fields"]]
+        while fields and fields[-1] == 0:
+            fields.pop()
+        net = int(t["net"])
+        e0 = int(t["first_event"])
+        events = [BusEvent(int(e["chip"]), CHIP_NAMES[int(e["chip"])], int(e["interaction"]), int(e["row"]), int(e["multiplicity"]), bool(e["is_send"]))
+                  for e in ev[e0:e0 + int(t["n_events"])]]
+        out.append(BusImbalance(int(t["bus"]), BUS_NAMES[int(t["bus"])] if t["bus"] < len(BUS_NAMES) else "bus %d" % t["bus"], fields,
+                                net - BABYBEAR_P if net > BABYBEAR_P // 2 else net, events))
+    return BusCheck(out, un.value == 0, int(un.value))
 
 
 class StarkConfig:

@@ -517,6 +517,10 @@ int32_t VgMachineCheck::finish(uint32_t sums[VGPU_NUM_CHIPS][5], vgpu_check_repo
     return 0;
 }
 
+int32_t vg_check_shapes(vgpu_ctx* ctx, const vgpu_chip_desc* chip, const vgpu_dmat* main, const vgpu_dmat* prep, const vgpu_dmat* perm, bool shards) {
+    return check_shapes(ctx, chip, main, prep, perm, shards);
+}
+
 bool vg_sums_cancel(const vgpu_check_report report[VGPU_NUM_CHIPS]) {
     for (int l = 0; l < 5; l++) {
         uint64_t s = 0;

@@ -31,6 +31,12 @@ uint32_t vg_perm_totals_ranks(const vgpu_ctx* ctx);
 // the cumulative sum (Montgomery) from the n per-rank totals ([rank][limb]) vg_perm_trace_enqueue left for a chip
 void vg_perm_totals_fold(const uint32_t* totals, uint32_t n, uint32_t out[5]);
 
+// The preprocessed trace of machine chip i (prep[0] / prep[1]: chips 1 / 12), null for the others.
+inline const vgpu_dmat* vg_machine_prep(const vgpu_dmat* const prep[2], int i) { return i == 1 ? prep[0] : i == 12 ? prep[1] : nullptr; }
+// check.cu — refuses, before anything is enqueued and alike on every rank, what the check sweep cannot read (perm may be null;
+// shards: this rank's row shards are accepted)
+int32_t vg_check_shapes(vgpu_ctx* ctx, const vgpu_chip_desc* chip, const vgpu_dmat* main, const vgpu_dmat* prep, const vgpu_dmat* perm, bool shards);
+
 // check.cu — the permutation traces of a machine witness (14 chips, prep[0] / prep[1] the preprocessed traces of chips 1 / 12) and,
 // when `check`, check_constraints of every chip on this rank's run: vgpu_check_witness and prove's debug mode.  perm(i) enqueues
 // chip i's permutation trace; sweep(i) (checking only) its check, which reads the trace before later work on the stream.  finish()
@@ -42,7 +48,7 @@ class VgMachineCheck {
     VgMachineCheck(vgpu_ctx* ctx, const vgpu_dmat* const main[VGPU_NUM_CHIPS], const vgpu_dmat* const prep[2], const uint32_t challenges[15],
                    bool check);
     ~VgMachineCheck();
-    const vgpu_dmat* prep_for(int i) const { return i == 1 ? prep_[0] : i == 12 ? prep_[1] : nullptr; }
+    const vgpu_dmat* prep_for(int i) const { return vg_machine_prep(prep_, i); }
     int32_t alloc();                                  // reads the traces' heights; enqueues nothing unless checking
     int32_t perm(int i, VgMat* out);
     int32_t sweep(int i, const vgpu_dmat* perm);
