@@ -265,6 +265,44 @@ int32_t vgpu_check_failures(vgpu_ctx* ctx, const vgpu_chip_desc* chip, const vgp
                             const vgpu_dmat* perm, const uint32_t challenges[15], uint64_t cap, vgpu_check_failure* out,
                             uint64_t* n_out, uint64_t* total_failures, uint64_t* rows_per_constraint);
 
+/* ---- what a failed constraint reads ----------------------------------------------------------------------------------------
+ * A chip's constraints catalogued from the same AIR text the check and quotient kernels evaluate, so constraint c here is constraint c
+ * of vgpu_check_constraints / vgpu_check_failures.  A CELL is one trace column on the local row or on the next row ((row + 1) mod h). */
+#define VGPU_TRACE_MAIN 0
+#define VGPU_TRACE_PREPROCESSED 1
+#define VGPU_TRACE_PERMUTATION 2
+#define VGPU_CELL_ABSENT 4294967295u      /* 0xffffffff, not a field element: a permutation-trace cell when no permutation trace was passed */
+typedef struct vgpu_cell {
+    uint32_t trace;             /* VGPU_TRACE_* */
+    uint32_t next;              /* 0: the row itself, 1: the next row */
+    uint32_t column;
+} vgpu_cell;
+/* The name of a column of the chip's main, preprocessed or flattened permutation trace (after the reference's column structs, e.g.
+ * "mem_channels[1].value[2]"; permutation column 5m + l is "interactions[m].reciprocal[l]", or "running_sum[l]" for m = k), or NULL
+ * when the column or trace is out of range.  Static strings.  Host only: no context, no GPU. */
+const char* vgpu_chip_column_name(const vgpu_chip_desc* chip, int32_t trace, uint32_t column);
+/* Constraint c's label and the cells it reads, in ascending (trace, next, column) order: writes min(cap, count) cells and sets *n to
+ * the count.  An Air::eval assertion's label names the block of the reference's eval it transcribes (e.g. "CpuChip::eval_pc"); the
+ * others read "interaction m (bus b, send|receive)", "LogUp transition", "LogUp first row" and "LogUp last row".  Interaction m reads
+ * its fields' columns and permutation element m (columns 5m..5m+4) on the local row; the transition reads the running sum on both
+ * rows and every element and count on the next row; the first-row constraint the running sum and every element and count on the
+ * local row; the last-row constraint the running sum on the local row (which the check also takes as the cumulative sum on row h-1,
+ * so on a trace it always vanishes).  The label lives as long as the process.  Returns -1 for a null argument, an unknown chip id
+ * or c >= total.  Host only. */
+int32_t vgpu_chip_constraint_cells(const vgpu_chip_desc* chip, uint32_t constraint, const char** label, vgpu_cell* cells, uint32_t cap,
+                                   uint32_t* n);
+/* The values of the cells behind n (row, constraint) items (the `value` field is ignored: vgpu_check_failures' output as it is; a bus
+ * event of vgpu_check_buses is item (row, air_constraints + interaction)).  Item i's values go to values[first[i], first[i + 1]) in
+ * vgpu_chip_constraint_cells order, canonical; a next-row cell is read at row (row + 1) mod h.  perm_or_null NULL: permutation cells
+ * are VGPU_CELL_ABSENT.  Takes whole matrices or this rank's row shards (borrowed ones too), like vgpu_check_failures, and refuses what
+ * it refuses of the traces, a row >= h or a constraint >= total (naming the item), null outputs when n > 0 and cap below the values
+ * needed (*n_values is that count), before anything is enqueued and alike on every rank.  Collective on a split context: every rank
+ * passes the same items and gets byte-identical output; each cell is reported by the rank that holds its row (rank 0 of a whole
+ * matrix) and one all-gather, summed, brings them together.  Synchronises once. */
+int32_t vgpu_explain_failures(vgpu_ctx* ctx, const vgpu_chip_desc* chip, const vgpu_dmat* main, const vgpu_dmat* prep_or_null,
+                              const vgpu_dmat* perm_or_null, const vgpu_check_failure* items, uint64_t n, uint64_t* first /* n + 1 */,
+                              uint32_t* values, uint64_t cap, uint64_t* n_values);
+
 typedef struct vgpu_check_report {
     int64_t first_row;          /* -1: every constraint vanishes on every row */
     uint32_t first_constraint;

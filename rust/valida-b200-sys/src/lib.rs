@@ -32,6 +32,12 @@ pub const VGPU_REJECT_FRI_FINAL: i32 = -6;
 pub const VGPU_REJECT_CUMULATIVE_SUM: i32 = -7;
 /// chip i's constraints at zeta: `-100 - i` (the reference's `OodEvaluationMismatch`)
 pub const VGPU_REJECT_CONSTRAINTS_CHIP0: i32 = -100;
+/// Traces of [`vgpu_cell::trace`].
+pub const VGPU_TRACE_MAIN: u32 = 0;
+pub const VGPU_TRACE_PREPROCESSED: u32 = 1;
+pub const VGPU_TRACE_PERMUTATION: u32 = 2;
+/// `0xffffffff`, not a field element: [`vgpu_explain_failures`]' value of a permutation-trace cell when no permutation trace was passed.
+pub const VGPU_CELL_ABSENT: u32 = 4294967295;
 
 #[repr(C)] pub struct vgpu_ctx { _opaque: [u8; 0] }
 #[repr(C)] pub struct vgpu_dmat { _opaque: [u8; 0] }
@@ -106,6 +112,17 @@ pub struct vgpu_check_failure {
     pub constraint: u32,
     /// The constraint's value on that row, canonical; a base-field constraint has limbs 1..4 = 0.
     pub value: [u32; 5],
+}
+
+/// One trace cell a constraint reads ([`vgpu_chip_constraint_cells`]).
+#[repr(C)]
+#[derive(Clone, Copy, Debug, Default, PartialEq, Eq)]
+pub struct vgpu_cell {
+    /// `VGPU_TRACE_MAIN`, `VGPU_TRACE_PREPROCESSED` or `VGPU_TRACE_PERMUTATION`.
+    pub trace: u32,
+    /// 0: the row itself, 1: the next row, `(row + 1) mod h`.
+    pub next: u32,
+    pub column: u32,
 }
 
 /// One chip's verdict of [`vgpu_check_witness`].
@@ -204,6 +221,9 @@ extern "C" {
     pub fn vgpu_check_constraints_local(ctx: *mut vgpu_ctx, chip: *const vgpu_chip_desc, main: *const vgpu_dmat, prep_or_null: *const vgpu_dmat, perm: *const vgpu_dmat, challenges: *const u32, first_row: *mut i64, first_constraint: *mut u32, failing_rows: *mut u64) -> i32;
     pub fn vgpu_chip_constraint_count(chip: *const vgpu_chip_desc, air_constraints: *mut u32, total: *mut u32) -> i32;
     pub fn vgpu_check_failures(ctx: *mut vgpu_ctx, chip: *const vgpu_chip_desc, main: *const vgpu_dmat, prep_or_null: *const vgpu_dmat, perm: *const vgpu_dmat, challenges: *const u32, cap: u64, out: *mut vgpu_check_failure, n_out: *mut u64, total_failures: *mut u64, rows_per_constraint: *mut u64) -> i32;
+    pub fn vgpu_chip_column_name(chip: *const vgpu_chip_desc, trace: i32, column: u32) -> *const c_char;
+    pub fn vgpu_chip_constraint_cells(chip: *const vgpu_chip_desc, constraint: u32, label: *mut *const c_char, cells: *mut vgpu_cell, cap: u32, n: *mut u32) -> i32;
+    pub fn vgpu_explain_failures(ctx: *mut vgpu_ctx, chip: *const vgpu_chip_desc, main: *const vgpu_dmat, prep_or_null: *const vgpu_dmat, perm_or_null: *const vgpu_dmat, items: *const vgpu_check_failure, n: u64, first: *mut u64, values: *mut u32, cap: u64, n_values: *mut u64) -> i32;
     pub fn vgpu_check_witness(ctx: *mut vgpu_ctx, main: *const *const vgpu_dmat, prep: *const *const vgpu_dmat, challenges: *const u32, report: *mut vgpu_check_report, sums_cancel: *mut i32) -> i32;
     pub fn vgpu_check_buses(ctx: *mut vgpu_ctx, main: *const *const vgpu_dmat, prep: *const *const vgpu_dmat, challenges: *const u32, cap: u64, tuples: *mut vgpu_bus_imbalance, n_tuples: *mut u64, events: *mut vgpu_bus_event, n_events: *mut u64, unexamined: *mut u64) -> i32;
 

@@ -440,6 +440,31 @@ impl Context {
         Ok((tuples, events, unexamined))
     }
 
+    /// The values of the cells each `(row, constraint)` item reads (the items' `value` fields are ignored: [`Context::check_failures`]'
+    /// list as it is; a bus event of [`Context::check_buses`] is `(row, air_constraints + interaction)`), per item in
+    /// [`constraint_cells`] order, canonical; a next-row cell is read at `(row + 1) mod h`.  Without `perm` the permutation cells are
+    /// `None`.  Takes what `check_failures` takes and refuses the same traces, a row or constraint out of range, before anything is
+    /// enqueued; collective on a split context (every rank passes the same items and gets the same values).  Synchronises once.
+    pub fn explain_failures(&self, chip_id: u32, main: &DMat<'_>, prep: Option<&DMat<'_>>, perm: Option<&DMat<'_>>,
+                            items: &[sys::vgpu_check_failure]) -> Result<Vec<Vec<Option<u32>>>> {
+        let chip = unsafe { sys::vgpu_basic_machine_chip(chip_id) };
+        let mut need = 0u64;
+        for it in items {
+            // an item out of range is left for the call to refuse, naming it
+            need += constraint_cells(chip_id, it.constraint).map_or(0, |(_, c)| c.len() as u64);
+        }
+        let mut first = vec![0u64; items.len() + 1];
+        let mut values = vec![0u32; need.max(1) as usize];
+        let mut n_values = 0u64;
+        self.check(unsafe {
+            sys::vgpu_explain_failures(self.raw, chip, main.as_ptr(), prep.map_or(ptr::null(), |m| m.as_ptr()), perm.map_or(ptr::null(), |m| m.as_ptr()),
+                                       items.as_ptr(), items.len() as u64, first.as_mut_ptr(), values.as_mut_ptr(), need, &mut n_values)
+        })?;
+        Ok((0..items.len())
+            .map(|i| values[first[i] as usize..first[i + 1] as usize].iter().map(|&v| if v == sys::VGPU_CELL_ABSENT { None } else { Some(v) }).collect())
+            .collect())
+    }
+
     /// Kernels launched by this context so far.
     pub fn launch_count(&self) -> u64 {
         unsafe { sys::vgpu_ctx_launch_count(self.raw) }
@@ -451,6 +476,31 @@ impl Context {
         self.check(unsafe { sys::vgpu_ctx_memory_stats(self.raw, out.as_mut_ptr(), reset as i32) })?;
         Ok(MemoryStats { live: out[0], peak: out[1], cached: out[2], symm_peak: out[3] })
     }
+}
+
+/// The name of a column of a BasicMachine chip's trace (`sys::VGPU_TRACE_MAIN`, `VGPU_TRACE_PREPROCESSED` or `VGPU_TRACE_PERMUTATION`),
+/// after the reference's column structs (e.g. `mem_channels[1].value[2]`); `None` out of range.  Host only.
+pub fn column_name(chip_id: u32, trace: u32, column: u32) -> Option<String> {
+    let p = unsafe { sys::vgpu_chip_column_name(sys::vgpu_basic_machine_chip(chip_id), trace as i32, column) };
+    if p.is_null() { None } else { Some(unsafe { CStr::from_ptr(p) }.to_string_lossy().into_owned()) }
+}
+
+/// Constraint `constraint` of a BasicMachine chip (eval order, as [`Context::check_failures`] numbers it): its label (the block of the
+/// reference's eval for an AIR assertion, e.g. `CpuChip::eval_pc`) and the cells it reads, in ascending (trace, next, column) order.
+/// Host only.
+pub fn constraint_cells(chip_id: u32, constraint: u32) -> Result<(String, Vec<sys::vgpu_cell>)> {
+    let chip = unsafe { sys::vgpu_basic_machine_chip(chip_id) };
+    let mut label: *const std::ffi::c_char = ptr::null();
+    let mut n = 0u32;
+    let refused = || Error { code: -1, message: format!("constraint_cells: chip {chip_id} has no constraint {constraint}") };
+    if unsafe { sys::vgpu_chip_constraint_cells(chip, constraint, &mut label, ptr::null_mut(), 0, &mut n) } != 0 {
+        return Err(refused());
+    }
+    let mut cells = vec![sys::vgpu_cell::default(); n as usize];
+    if unsafe { sys::vgpu_chip_constraint_cells(chip, constraint, &mut label, cells.as_mut_ptr(), n, &mut n) } != 0 {
+        return Err(refused());
+    }
+    Ok((unsafe { CStr::from_ptr(label) }.to_string_lossy().into_owned(), cells))
 }
 
 /// What [`Context::memory_stats`] returns.

@@ -64,6 +64,10 @@ BUS_IMBALANCE_DTYPE = np.dtype([("bus", "<u4"), ("fields", "<u4", (14,)), ("net"
 # BasicMachine's chips and buses (basic/src/lib.rs:151-166, 1190-1212), by id
 CHIP_NAMES = ("cpu", "program", "memory", "add", "sub", "mul", "div", "shift", "lt", "com", "bitwise", "output", "range", "static_data")
 BUS_NAMES = ("general", "program", "memory", "range")
+# vgpu_cell (include/valida_b200.h): which trace, the row itself (0) or the next row (1), the column
+TRACE_MAIN, TRACE_PREPROCESSED, TRACE_PERMUTATION = 0, 1, 2
+CELL_DTYPE = np.dtype([("trace", "<u4"), ("next", "<u4"), ("column", "<u4")])
+CELL_ABSENT = 0xFFFFFFFF      # vgpu_explain_failures' word for a permutation cell when no permutation trace was passed
 
 
 def _load():
@@ -115,6 +119,9 @@ def _load():
         "vgpu_check_constraints_local": (C.c_int32, [vp, vp, vp, vp, vp, u32p, C.POINTER(C.c_int64), u32p, C.POINTER(u64)]),
         "vgpu_chip_constraint_count": (C.c_int32, [vp, u32p, u32p]),
         "vgpu_check_failures": (C.c_int32, [vp, vp, vp, vp, vp, u32p, u64, vp, C.POINTER(u64), C.POINTER(u64), C.POINTER(u64)]),
+        "vgpu_chip_column_name": (C.c_char_p, [vp, C.c_int32, C.c_uint32]),
+        "vgpu_chip_constraint_cells": (C.c_int32, [vp, C.c_uint32, C.POINTER(C.c_char_p), vp, C.c_uint32, u32p]),
+        "vgpu_explain_failures": (C.c_int32, [vp, vp, vp, vp, vp, vp, u64, C.POINTER(u64), u32p, u64, C.POINTER(u64)]),
         "vgpu_check_witness": (C.c_int32, [vp, C.POINTER(vp), C.POINTER(vp), u32p, C.POINTER(_CheckReport), C.POINTER(C.c_int32)]),
         "vgpu_check_buses": (C.c_int32, [vp, C.POINTER(vp), C.POINTER(vp), u32p, u64, vp, C.POINTER(u64), vp, C.POINTER(u64), C.POINTER(u64)]),
         "vgpu_ctx_set_debug_checks": (C.c_int32, [vp, C.c_int32]),
@@ -673,6 +680,80 @@ def check_failures(ctx, chip_id, main, prep, perm, perm_challenges, cap=1 << 16)
                                         int(cap), out.ctypes.data_as(C.c_void_p) if cap else None, C.byref(n), C.byref(total),
                                         per.ctypes.data_as(C.POINTER(C.c_uint64))))
     return out[:n.value].copy(), int(total.value), per
+
+
+def column_name(chip_id, trace, column):
+    """The name of a column of the chip's main, preprocessed or flattened permutation trace (TRACE_MAIN / TRACE_PREPROCESSED /
+    TRACE_PERMUTATION), after the reference's column structs, e.g. "mem_channels[1].value[2]"; permutation column 5m + l is
+    "interactions[m].reciprocal[l]", or "running_sum[l]" for m = k.  None when the column is out of range."""
+    name = lib().vgpu_chip_column_name(lib().vgpu_basic_machine_chip(chip_id), int(trace), int(column))
+    return name.decode() if name is not None else None
+
+
+Cell = collections.namedtuple("Cell", "trace next column name")
+CellValue = collections.namedtuple("CellValue", "trace next column name value")
+Explanation = collections.namedtuple("Explanation", "row constraint label cells")
+
+
+def _constraint_cells(chip, chip_id, index):
+    label, n = C.c_char_p(), C.c_uint32()
+    if lib().vgpu_chip_constraint_cells(chip, int(index), C.byref(label), None, 0, C.byref(n)) != 0:
+        raise VgpuError("constraint_cells: chip %r has no constraint %r" % (chip_id, index))
+    cells = np.zeros(n.value, dtype=CELL_DTYPE)
+    lib().vgpu_chip_constraint_cells(chip, int(index), C.byref(label), cells.ctypes.data_as(C.c_void_p), n.value, C.byref(n))
+    return label.value.decode(), cells
+
+
+def constraint_cells(chip_id, index):
+    """What constraint `index` of a chip (eval order, as check_constraints and check_failures number it) reads, from the same AIR text
+    the kernels evaluate: (label, [Cell(trace, next, column, name)]) in ascending (trace, next, column) order.  An Air::eval
+    assertion's label names the block of the reference's eval it transcribes (e.g. "CpuChip::eval_pc"); the others are worded as
+    constraint_label words them."""
+    _, total = constraint_count(chip_id)
+    if not 0 <= index < total:
+        raise VgpuError("constraint_cells: chip %d has %d constraints, not %r" % (chip_id, total, index))
+    label, cells = _constraint_cells(lib().vgpu_basic_machine_chip(chip_id), chip_id, index)
+    return label, [Cell(int(c["trace"]), bool(c["next"]), int(c["column"]), column_name(chip_id, c["trace"], c["column"])) for c in cells]
+
+
+def explain_failures(ctx, chip_id, main, prep, perm, items):
+    """For each (row, constraint) item, the constraint's label and the values of the cells it reads on that row (a next-row cell at
+    row (row + 1) mod h): one Explanation(row, constraint, label, cells=[CellValue(trace, next, column, name, value)]) per item,
+    values canonical.  items: check_failures' array (its values are ignored) or a list of (row, constraint) pairs; a bus event of
+    check_buses is (row, air_constraints + interaction).  perm None: permutation cells have value None.  Takes what check_failures
+    takes (whole matrices, or on a split context this rank's row shards; collective there, every rank passing the same items and
+    getting the same answer)."""
+    chip = lib().vgpu_basic_machine_chip(chip_id)
+    if isinstance(items, np.ndarray) and items.dtype == CHECK_FAILURE_DTYPE:
+        arr = np.ascontiguousarray(items)
+    else:
+        pairs = list(items)
+        arr = np.zeros(len(pairs), dtype=CHECK_FAILURE_DTYPE)
+        for i, (row, con) in enumerate(pairs):
+            arr[i]["row"], arr[i]["constraint"] = row, con
+    n = len(arr)
+    first = np.zeros(n + 1, dtype=np.uint64)
+    # the catalogue sizes the output exactly (an out-of-range item is left for the call to refuse, naming it)
+    _, total = constraint_count(chip_id)
+    cat = {}
+    for c in set(int(x) for x in arr["constraint"]):
+        if 0 <= c < total:
+            cat[c] = _constraint_cells(chip, chip_id, c)
+    cap = sum(len(cat[int(c)][1]) for c in arr["constraint"] if int(c) in cat)
+    values = np.zeros(max(cap, 1), dtype=np.uint32)
+    nv = C.c_uint64()
+    ctx.check(lib().vgpu_explain_failures(ctx._h, chip, main._h, _h(prep), _h(perm), arr.ctypes.data_as(C.c_void_p) if n else None, n,
+                                          first.ctypes.data_as(C.POINTER(C.c_uint64)), values.ctypes.data_as(C.POINTER(C.c_uint32)), cap,
+                                          C.byref(nv)))
+    out = []
+    for i in range(n):
+        c = int(arr[i]["constraint"])
+        label, cells = cat[c]
+        vals = values[int(first[i]):int(first[i + 1])]
+        out.append(Explanation(int(arr[i]["row"]), c, label,
+                               [CellValue(int(x["trace"]), bool(x["next"]), int(x["column"]), column_name(chip_id, x["trace"], x["column"]),
+                                          None if int(v) == CELL_ABSENT else int(v)) for x, v in zip(cells, vals)]))
+    return out
 
 
 def check_witness(ctx, main, prep, challenges):

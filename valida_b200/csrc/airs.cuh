@@ -5,6 +5,8 @@
 //     B::L(c) / B::N(c)      main-trace cell of the local / next row (column c)
 //     b.first/last/trans     selector values (is_first_row, is_last_row, is_transition)
 //     b.z(x)                 AirBuilder::assert_zero(x)
+//     b.section(name)        names the block of the reference's eval that the assertions after it transcribe (a no-op for
+//                            every builder but the host catalogue's, explain.cu)
 // Filters (`when`, `when_ne`, `when_transition`, ...) are multiplied in explicitly, which is what
 // p3-air's FilteredAirBuilder lowers to.  Constraint ORDER is part of the result (alpha-folding,
 // machine/src/folding_builder.rs:62-66) and follows each eval() line by line.
@@ -72,7 +74,7 @@ template <class B> BB_HD void eval_cpu(B& b) {
     const V rv1 = word_be(b, false, R1V), rv2 = word_be(b, false, R2V), wv = word_be(b, false, WV);
     const V npc = b.N(1), nfp = b.N(2);
 
-    // eval_pc
+    b.section("CpuChip::eval_pc");
     const V inc_pc = pc + one;
     b.z(tr * (is_imm32 + is_loadfp + is_bus + is_advice) * (npc - inc_pc));
     const V equal = one - not_equal;
@@ -80,16 +82,16 @@ template <class B> BB_HD void eval_cpu(B& b) {
     b.z(tr * is_bne * (bpi * npc - (bpi * equal * inc_pc + not_equal * opa)));
     b.z(tr * is_jal * (bpi * npc - opb));
     b.z(tr * is_jalv * (bpi * npc - rv1));
-    // eval_fp
+    b.section("CpuChip::eval_fp");
     b.z(tr * is_jal * (nfp - (fp + opc)));
     b.z(tr * is_jalv * (nfp - (fp + rv2)));
     b.z(tr * (one - is_jal - is_jalv) * (nfp - fp));
-    // eval_equality
+    b.section("CpuChip::eval_equality");
     b.z(diff - sqdiff4(b, R1V, R2V));
     b.z(not_equal * (not_equal - one));
     b.z(not_equal - diff * diff_inv);
     b.z((one - not_equal) * diff);
-    // eval_memory_channels
+    b.section("CpuChip::eval_memory_channels");
     b.z(is_load * (is_load - one)); b.z(is_store * (is_store - one)); b.z(is_jal * (is_jal - one)); b.z(is_jalv * (is_jalv - one));
     b.z(is_beq * (is_beq - one)); b.z(is_bne * (is_bne - one)); b.z(is_imm32 * (is_imm32 - one)); b.z(is_loadfp * (is_loadfp - one));
     b.z(is_imm * (is_imm - one)); b.z(is_limm * (is_limm - one)); b.z(is_bus * (is_bus - one));
@@ -118,16 +120,16 @@ template <class B> BB_HD void eval_cpu(B& b) {
     b.z(is_loadfp * (addr_b - wv));
     b.z((is_store + is_load + is_jal + is_jalv + is_imm32 + is_loadfp + is_bus) * (w_used - one));
     b.z((is_beq + is_bne) * w_used);
-    // clock
+    b.section("CpuChip::eval clock");
     b.z(b.first * clk);
     b.z(tr * (clk + one - b.N(0)));
     b.z(is_bus_mem * (clk - b.L(50)));
     b.z((one - is_bus_mem) * b.L(50));
-    // immediates
+    b.section("CpuChip::eval immediates");
     b.z((is_imm + is_limm) * (is_imm + is_limm - one));
     b.z(is_imm * (opc - rv2));
     b.z(is_limm * (opb - rv1));
-    // stop
+    b.section("CpuChip::eval stop");
     b.z(tr * is_stop * (npc - pc));
     b.z(b.last * (is_stop - one));
 }
@@ -141,7 +143,9 @@ template <class B> BB_HD void eval_add(B& b) {
     const V o1 = b.L(2) + b.L(6) - b.L(13) + c1;
     const V o2 = b.L(1) + b.L(5) - b.L(12) + c2;
     const V o3 = b.L(0) + b.L(4) - b.L(11) + c3;
+    b.section("Add32Chip::eval limbs");
     b.z(o0 * (o0 - base)); b.z(o1 * (o1 - base)); b.z(o2 * (o2 - base)); b.z(o3 * (o3 - base));
+    b.section("Add32Chip::eval carries");
     b.z(o0 * (c1 - one) + (o0 - base) * c1);
     b.z(o1 * (c2 - one) + (o1 - base) * c2);
     b.z(o2 * (c3 - one) + (o2 - base) * c3);
@@ -153,6 +157,7 @@ template <class B> BB_HD void eval_sub(B& b) {
     using V = typename B::V;
     const V one = ONE<V>(), base = K<V, 256>();
     const V w1 = b.L(8), w2 = b.L(9), w3 = b.L(10);
+    b.section("Sub32Chip::eval");
     b.z(b.L(14) - (base * w1 + b.L(3) - b.L(7)));
     b.z(b.L(13) - (base * w2 + b.L(2) - b.L(6) - w1));
     b.z(b.L(12) - (base * w3 + b.L(1) - b.L(5) - w2));
@@ -171,8 +176,10 @@ template <class B> BB_HD void eval_mul(B& b) {
             if (i < 2 && j < 2 && i + j < 2) pi2 = pi2 + wgt[i + j] * b.L(3 - i) * b.L(7 - j);
         }
     for (int i = 0; i < 4; i++) { sg4 = sg4 + wgt[i] * b.L(11 - i); if (i < 2) sg2 = sg2 + wgt[i] * b.L(11 - i); }
+    b.section("Mul32Chip::eval congruences");
     b.z(pi4 - sg4 - b.L(12) * K<V, 2>());
     b.z(pi2 - sg2 - b.L(13) * wgt[2]);
+    b.section("Mul32Chip::eval counter");
     b.z(b.first * (b.L(17) - ONE<V>()));
     const V cd = b.N(17) - b.L(17);
     b.z(b.trans * (cd * (cd - ONE<V>())));
@@ -186,8 +193,10 @@ template <class B> BB_HD void eval_shift(B& b) {
     V byte2 = ZERO<V>();
     const V p2[8] = {K<V, 1>(), K<V, 2>(), K<V, 4>(), K<V, 8>(), K<V, 16>(), K<V, 32>(), K<V, 64>(), K<V, 128>()};
     for (int i = 0; i < 8; i++) byte2 = byte2 + b.L(12 + i) * p2[i];
+    b.section("Shift32Chip::eval bits_2");
     b.z(b.L(7) - byte2);
     for (int i = 0; i < 8; i++) { V t = b.L(12 + i); b.z(t * (t - one)); }
+    b.section("Shift32Chip::eval power_of_two");
     const V t1 = (b.L(12) * K<V, 2>()) * (b.L(13) * K<V, 4>()) * (b.L(14) * K<V, 16>());
     b.z(b.L(20) - t1);
     const V b3 = b.L(15), b4 = b.L(16), tmp = b.L(20);
@@ -196,6 +205,7 @@ template <class B> BB_HD void eval_shift(B& b) {
     b.z(b.L(23) - tmp * (one - b3) * b4);
     b.z(b.L(24) - tmp * b3 * b4);
     const V shl = b.L(25), shr = b.L(26), sra = b.L(27);
+    b.section("Shift32Chip::eval opcode flags");
     b.z(shl * (shl - one)); b.z(shr * (shr - one)); b.z(sra * (sra - one));
     const V s = shl + shr + sra;
     b.z(s * (s - one));
@@ -211,6 +221,7 @@ template <class B> BB_HD void eval_lt(B& b) {
     for (int i = 0; i < 9; i++) bit_comp = bit_comp + b.L(12 + i) * p2[i];
     const V f0 = b.L(8), f1 = b.L(9), f2 = b.L(10), f3 = b.L(11);
     const V flag_sum = f0 + f1 + f2 + f3;
+    b.section("Lt32Chip::eval byte_flag");
     b.z(flag_sum * (flag_sum - one));
     b.z((f0 - one) * (b.L(0) - b.L(4)));
     b.z((f0 + f1 - one) * (b.L(1) - b.L(5)));
@@ -224,24 +235,29 @@ template <class B> BB_HD void eval_lt(B& b) {
         b.z(fl * (fl - one));
     }
     V top1 = ZERO<V>(), top2 = ZERO<V>();
+    b.section("Lt32Chip::eval top bits");
     for (int i = 0; i < 8; i++) { top1 = top1 + b.L(28 + i) * p2[i]; top2 = top2 + b.L(36 + i) * p2[i]; }
     b.z(top1 - b.L(0));
     b.z(top2 - b.L(4));
     const V is_lt = b.L(23), is_lte = b.L(24), is_slt = b.L(25), is_sle = b.L(26), ds = b.L(44), out = b.L(21), bit8 = b.L(20);
     const V is_signed = is_slt + is_sle, is_unsigned = one - is_signed, same_sign = one - ds, are_equal = one - flag_sum;
+    b.section("Lt32Chip::eval different_signs");
     b.z(is_unsigned * ds);
     b.z(is_signed * (b.L(35) - b.L(43)) * (ds - one));
     b.z(ds * (f0 - one));
     b.z(ds * (b.L(35) + b.L(43) - one));
+    b.section("Lt32Chip::eval opcode flags");
     b.z(is_lt * (is_lt - one)); b.z(is_lte * (is_lte - one)); b.z(is_slt * (is_slt - one)); b.z(is_sle * (is_sle - one));
     const V opsum = is_lt + is_lte + is_slt + is_sle;
     b.z(opsum * (opsum - one));
+    b.section("Lt32Chip::eval output");
     b.z(bit8 * (is_unsigned + same_sign) * out);
     b.z(bit8 * ds * (out - one));
     b.z((bit8 + are_equal - one) * (is_unsigned + same_sign) * (out - one));
     b.z((bit8 + are_equal - one) * ds * out);
     b.z(are_equal * (is_lte + is_sle) * (out - one));
     b.z(are_equal * (is_lt + is_slt) * out);
+    b.section("Lt32Chip::eval bits booleans");
     for (int i = 0; i < 9; i++) { V t = b.L(12 + i); b.z(t * (t - one)); }
     for (int i = 0; i < 8; i++) { V t = b.L(28 + i); b.z(t * (t - one)); }
     for (int i = 0; i < 8; i++) { V t = b.L(36 + i); b.z(t * (t - one)); }
@@ -252,6 +268,7 @@ template <class B> BB_HD void eval_com(B& b) {
     using V = typename B::V;
     const V one = ONE<V>();
     const V ne = b.L(10), is_ne = b.L(12), is_eq = b.L(13);
+    b.section("Com32Chip::eval");
     b.z(b.L(8) - sqdiff4(b, 0, 4));
     b.z(ne * (ne - one));
     b.z(ne - b.L(8) * b.L(9));
@@ -267,6 +284,7 @@ template <class B> BB_HD void eval_bitwise(B& b) {
     const V one = ONE<V>();
     const V p2[8] = {K<V, 1>(), K<V, 2>(), K<V, 4>(), K<V, 8>(), K<V, 16>(), K<V, 32>(), K<V, 64>(), K<V, 128>()};
     const V is_and = b.L(76), is_or = b.L(77), is_xor = b.L(78);
+    b.section("Bitwise32Chip::eval bytes");
     for (int i = 0; i < 4; i++) {
         V byte1 = ZERO<V>(), byte2 = ZERO<V>(), band = ZERO<V>();
         for (int k = 0; k < 8; k++) {
@@ -282,6 +300,7 @@ template <class B> BB_HD void eval_bitwise(B& b) {
         for (int k = 0; k < 8; k++) { V t = b.L(8 + 8 * i + k); b.z(t * (t - one)); }
         for (int k = 0; k < 8; k++) { V t = b.L(40 + 8 * i + k); b.z(t * (t - one)); }
     }
+    b.section("Bitwise32Chip::eval opcode flags");
     b.z(is_and * (is_and - one)); b.z(is_or * (is_or - one)); b.z(is_xor * (is_xor - one));
     const V s = is_and + is_or + is_xor;
     b.z(s * (s - one));
@@ -290,14 +309,17 @@ template <class B> BB_HD void eval_bitwise(B& b) {
 // ---- 11: OutputChip — clk 0, value 1, is_real 2, diff 3, counter 4, counter_mult 5, opcode 6 -----------
 template <class B> BB_HD void eval_output(B& b) {
     using V = typename B::V;
+    b.section("OutputChip::eval range check");
     b.z(b.trans * (b.L(3) - (b.N(0) - b.L(0))));
     b.z(b.trans * (b.N(4) - (b.L(4) + ONE<V>())));
+    b.section("OutputChip::eval bus opcode");
     b.z(b.L(2) * (b.L(6) - K<V, 300>()));
 }
 
 // ---- 13: StaticDataChip — addr 0, value 1..4, is_real 5 ---------------------------------------------------
 template <class B> BB_HD void eval_static_data(B& b) {
     using V = typename B::V;
+    b.section("StaticDataChip::eval_main");
     b.z(b.trans * (b.L(5) * b.N(5)) * (b.N(0) - (b.L(0) + ONE<V>() + ONE<V>() + ONE<V>() + ONE<V>())));
 }
 

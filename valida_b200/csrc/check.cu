@@ -53,6 +53,7 @@ struct RowBuilder {
     uint32_t idx;
     __device__ __forceinline__ F L(int c) const { return F{__ldg(lrow + (uint64_t)c * cs)}; }
     __device__ __forceinline__ F N(int c) const { return F{__ldg(nrow + (uint64_t)c * cs)}; }
+    __device__ __forceinline__ void section(const char*) {}
 };
 
 // Sets up local row i of the run and evaluates every constraint on it, in eval order, into b.

@@ -67,6 +67,7 @@ struct DevBuilder {
     __device__ __forceinline__ E5 pw() const { E5 a; for (int l = 0; l < 5; l++) a.c[l] = apow[idx][l]; return a; }
     __device__ __forceinline__ void z(F x) { acc.fma_base(pw(), x.v); idx++; }
     __device__ __forceinline__ void z_ext(const E5& x) { acc.fma_ext(pw(), x, bb::e5_dbl(x)); idx++; }
+    __device__ __forceinline__ void section(const char*) {}
 };
 
 __device__ __forceinline__ uint32_t qroot_pow(const QParams& p, uint64_t e) {
@@ -173,6 +174,7 @@ struct CountBuilder {
     BB_HD F L(int) const { return F{0}; }
     BB_HD F N(int) const { return F{0}; }
     BB_HD void z(F) { n++; }
+    BB_HD void section(const char*) {}
 };
 
 }  // namespace

@@ -24,6 +24,7 @@ struct VerifierFolder {
     X N(int c) const { return X{nrow[c]}; }
     void z(const X& x) { acc = bb::e5_add(bb::e5_mul(acc, alpha), x.e); }   // Horner, folding_builder.rs:196-200
     void z_ext(const E5& x) { acc = bb::e5_add(bb::e5_mul(acc, alpha), x); }
+    void section(const char*) {}
 };
 
 // VirtualPairCol::apply over extension-valued rows (p3_air::VirtualPairCol; machine/src/chip.rs:76-80)
