@@ -465,6 +465,44 @@ int32_t vgpu_vmlog_traces(vgpu_vmlog* log, vgpu_traces** out, char* err, uint64_
 int32_t vgpu_witness_device(vgpu_ctx* ctx, const vgpu_vmlog* log, vgpu_dmat* main_out[VGPU_NUM_CHIPS], vgpu_dmat* prep_out[2]);
 void vgpu_vmlog_free(vgpu_vmlog* log);
 
+/* ---- which cells of a witness differ from its run's ----------------------------------------------------------------------------
+ * One cell of a caller's witness that differs from what Chip::generate_trace writes for the run (vgpu_witness_device's trace). */
+typedef struct vgpu_cell_diff {
+    uint32_t chip;              /* 0..13 */
+    uint32_t trace;             /* VGPU_TRACE_MAIN, or VGPU_TRACE_PREPROCESSED (the program trace of chip 1, the range trace of chip 12) */
+    uint32_t column;
+    int64_t row;                /* global row */
+    uint32_t have, want;        /* canonical: the caller's word, and generate_trace's word for this run */
+} vgpu_cell_diff;
+typedef struct vgpu_diff_summary {  /* one per chip */
+    uint64_t height_have, height_want;  /* the chip's cells are compared only when these agree */
+    uint64_t cells;                     /* differing cells, main + preprocessed */
+    int64_t first_row;                  /* the lowest row with a differing cell, -1: none */
+} vgpu_diff_summary;
+/* The length of vgpu_diff_witness' per-column counts: the main columns of chips 0..13 in chip order, then the 7 program and the 1
+ * range preprocessed columns (the sum of the chips' widths + 8).  Host only. */
+uint64_t vgpu_witness_column_count(void);
+/* Every cell of the caller's witness (main[14], prep[2]) that differs from the trace Chip::generate_trace builds for the run `log`
+ * records, with both words.  Writes:
+ *   - out[0, *n_out): the first min(cap, *total) differing cells in ascending (chip, trace, row, column) order, so the first CPU entry
+ *     is on the first cycle whose row differs;
+ *   - summary[c]: chip c's heights, its differing cells and its lowest differing row.  A chip whose height differs from the run's is
+ *     reported there (a wrong padding length is a finding) and its cells are not compared; the other chips still are;
+ *   - per_column_or_null (may be NULL, else vgpu_witness_column_count() entries): the differing cells of each column.
+ * Takes what vgpu_check_buses takes (whole matrices, or this rank's row shards; uploaded, imported or borrowed, with any column
+ * stride).  Refuses, before anything is enqueued and alike on every rank, a missing trace, a width that is not the chip's, a matrix
+ * stored with bit-reversed rows, a row shard that is not this context's run, a run without cycles, and null outputs (out only when
+ * cap > 0).  The expected witness is built on the device from the logs one chip at a time, and each chip is compared before the
+ * next is built: besides the logs and the memory chip's address sort, the call holds one chip's trace (this rank's run of it on a
+ * split context), never a second witness.  Words are compared as stored (Montgomery); only the reported words are converted.
+ * Collective on a split context, with byte-identical output on every rank: each rank compares its run of the split chips and rank
+ * 0 the chips every rank holds whole; one all-gather brings the per-rank counts (per chip and per column), and, when some rank found
+ * a difference and cap > 0, one more each rank's first min(count, cap) cells.  Synchronises; the caller's traces are left
+ * untouched. */
+int32_t vgpu_diff_witness(vgpu_ctx* ctx, const vgpu_vmlog* log, const vgpu_dmat* const main[VGPU_NUM_CHIPS], const vgpu_dmat* const prep[2],
+                          uint64_t cap, vgpu_cell_diff* out, uint64_t* n_out, uint64_t* total,
+                          vgpu_diff_summary summary[VGPU_NUM_CHIPS], uint64_t* per_column_or_null);
+
 /* fib_program of basic/tests/test_prover.rs:35-188 with `imm32 -8(fp)` = n; returns the instruction count (23). */
 uint64_t vgpu_fib_program(uint32_t n, int32_t* out_words /* >= 23*6 */);
 

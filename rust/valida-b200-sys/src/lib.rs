@@ -166,6 +166,36 @@ pub struct vgpu_bus_imbalance {
     pub n_events: u64,
 }
 
+/// One cell of a caller's witness that differs from what `Chip::generate_trace` writes for the run ([`vgpu_diff_witness`]).
+#[repr(C)]
+#[derive(Clone, Copy, Debug, Default, PartialEq, Eq)]
+pub struct vgpu_cell_diff {
+    /// Chip id, 0..13.
+    pub chip: u32,
+    /// `VGPU_TRACE_MAIN`, or `VGPU_TRACE_PREPROCESSED` (the program trace of chip 1, the range trace of chip 12).
+    pub trace: u32,
+    pub column: u32,
+    /// Global row.
+    pub row: i64,
+    /// Canonical: the caller's word.
+    pub have: u32,
+    /// Canonical: `generate_trace`'s word for this run.
+    pub want: u32,
+}
+
+/// One chip's part of [`vgpu_diff_witness`]' answer.
+#[repr(C)]
+#[derive(Clone, Copy, Debug, Default, PartialEq, Eq)]
+pub struct vgpu_diff_summary {
+    /// The chip's cells are compared only when the two heights agree.
+    pub height_have: u64,
+    pub height_want: u64,
+    /// Differing cells, main + preprocessed.
+    pub cells: u64,
+    /// The lowest row with a differing cell, `-1`: none.
+    pub first_row: i64,
+}
+
 extern "C" {
     // ---- context ----
     pub fn vgpu_ctx_create(device: i32, cuda_stream: *mut c_void, out: *mut *mut vgpu_ctx) -> i32;
@@ -269,5 +299,7 @@ extern "C" {
     pub fn vgpu_vmlog_traces(log: *mut vgpu_vmlog, out: *mut *mut vgpu_traces, err: *mut c_char, err_len: u64) -> i32;
     pub fn vgpu_witness_device(ctx: *mut vgpu_ctx, log: *const vgpu_vmlog, main_out: *mut *mut vgpu_dmat, prep_out: *mut *mut vgpu_dmat) -> i32;
     pub fn vgpu_vmlog_free(log: *mut vgpu_vmlog);
+    pub fn vgpu_witness_column_count() -> u64;
+    pub fn vgpu_diff_witness(ctx: *mut vgpu_ctx, log: *const vgpu_vmlog, main: *const *const vgpu_dmat, prep: *const *const vgpu_dmat, cap: u64, out: *mut vgpu_cell_diff, n_out: *mut u64, total: *mut u64, summary: *mut vgpu_diff_summary, per_column_or_null: *mut u64) -> i32;
     pub fn vgpu_fib_program(n: u32, out_words: *mut i32) -> u64;
 }

@@ -465,6 +465,28 @@ impl Context {
             .collect())
     }
 
+    /// Every cell of the witness `main` / `prep` that differs from what `Chip::generate_trace` writes for the run `log` records:
+    /// the first `min(cap, total)` cells in ascending (chip, trace, row, column) order (so the first CPU cell is on the first cycle
+    /// whose row differs), their total, one summary per chip (a chip whose height differs from the run's is reported there and not
+    /// compared) and the differing cells of each column ([`witness_column_count`] entries).  Takes what [`Context::check_buses`]
+    /// takes; collective on a split context, with the same result on every rank.  The expected witness is built and compared on the
+    /// device one chip at a time.  Synchronises.
+    pub fn diff_witness(&self, log: &VmLog, main: &[&DMat<'_>; sys::VGPU_NUM_CHIPS], prep: &[&DMat<'_>; 2], cap: usize)
+                        -> Result<(Vec<sys::vgpu_cell_diff>, u64, [sys::vgpu_diff_summary; sys::VGPU_NUM_CHIPS], Vec<u64>)> {
+        let main_raw: Vec<*const vgpu_dmat> = main.iter().map(|m| m.as_ptr()).collect();
+        let prep_raw: Vec<*const vgpu_dmat> = prep.iter().map(|m| m.as_ptr()).collect();
+        let mut out = vec![sys::vgpu_cell_diff::default(); cap];
+        let mut summary = [sys::vgpu_diff_summary::default(); sys::VGPU_NUM_CHIPS];
+        let mut per_column = vec![0u64; witness_column_count()];
+        let (mut n, mut total) = (0u64, 0u64);
+        self.check(unsafe {
+            sys::vgpu_diff_witness(self.raw, log.raw, main_raw.as_ptr(), prep_raw.as_ptr(), cap as u64, out.as_mut_ptr(), &mut n, &mut total,
+                                   summary.as_mut_ptr(), per_column.as_mut_ptr())
+        })?;
+        out.truncate(n as usize);
+        Ok((out, total, summary, per_column))
+    }
+
     /// Kernels launched by this context so far.
     pub fn launch_count(&self) -> u64 {
         unsafe { sys::vgpu_ctx_launch_count(self.raw) }
@@ -501,6 +523,45 @@ pub fn constraint_cells(chip_id: u32, constraint: u32) -> Result<(String, Vec<sy
         return Err(refused());
     }
     Ok((unsafe { CStr::from_ptr(label) }.to_string_lossy().into_owned(), cells))
+}
+
+/// The length of [`Context::diff_witness`]' per-column counts: the main columns of chips 0..13 in chip order, then the 7 program and
+/// the 1 range preprocessed columns.  Host only.
+pub fn witness_column_count() -> usize {
+    unsafe { sys::vgpu_witness_column_count() as usize }
+}
+
+/// The logs of one run of `Machine::run` (the interpreter on the host): what the device witness builder and
+/// [`Context::diff_witness`] expand into the traces.
+pub struct VmLog {
+    raw: *mut sys::vgpu_vmlog,
+}
+
+unsafe impl Send for VmLog {}
+unsafe impl Sync for VmLog {}
+
+impl VmLog {
+    /// Runs `program` (`n_instr` x 6 words: opcode, a, b, c, d, e) with the static cells `(address, value)` preloaded, ascending by address.
+    pub fn run(program: &[[i32; 6]], initial_pc: u32, initial_fp: u32, max_cycles: u64, static_data: &[(u32, u32)]) -> Result<Self> {
+        let addrs: Vec<u32> = static_data.iter().map(|&(a, _)| a).collect();
+        let values: Vec<u32> = static_data.iter().map(|&(_, v)| v).collect();
+        let mut raw = ptr::null_mut();
+        let mut err = [0 as std::ffi::c_char; 512];
+        let code = unsafe {
+            sys::vgpu_vm_run(program.as_ptr() as *const i32, program.len() as u64, initial_pc, initial_fp, max_cycles, addrs.as_ptr(), values.as_ptr(),
+                             static_data.len() as u64, &mut raw, err.as_mut_ptr(), err.len() as u64)
+        };
+        if code != 0 {
+            return Err(Error { code, message: unsafe { CStr::from_ptr(err.as_ptr()) }.to_string_lossy().into_owned() });
+        }
+        Ok(VmLog { raw })
+    }
+}
+
+impl Drop for VmLog {
+    fn drop(&mut self) {
+        unsafe { sys::vgpu_vmlog_free(self.raw) }
+    }
 }
 
 /// What [`Context::memory_stats`] returns.

@@ -68,6 +68,9 @@ BUS_NAMES = ("general", "program", "memory", "range")
 TRACE_MAIN, TRACE_PREPROCESSED, TRACE_PERMUTATION = 0, 1, 2
 CELL_DTYPE = np.dtype([("trace", "<u4"), ("next", "<u4"), ("column", "<u4")])
 CELL_ABSENT = 0xFFFFFFFF      # vgpu_explain_failures' word for a permutation cell when no permutation trace was passed
+# vgpu_cell_diff / vgpu_diff_summary (include/valida_b200.h)
+CELL_DIFF_DTYPE = np.dtype([("chip", "<u4"), ("trace", "<u4"), ("column", "<u4"), ("row", "<i8"), ("have", "<u4"), ("want", "<u4")], align=True)
+DIFF_SUMMARY_DTYPE = np.dtype([("height_have", "<u8"), ("height_want", "<u8"), ("cells", "<u8"), ("first_row", "<i8")])
 
 
 def _load():
@@ -157,6 +160,8 @@ def _load():
         "vgpu_vmlog_stats": (None, [vp, u32p, u32p, u32p]),
         "vgpu_vmlog_traces": (C.c_int32, [vp, C.POINTER(vp), C.c_char_p, u64]),
         "vgpu_witness_device": (C.c_int32, [vp, vp, C.POINTER(vp), C.POINTER(vp)]),
+        "vgpu_witness_column_count": (u64, []),
+        "vgpu_diff_witness": (C.c_int32, [vp, vp, C.POINTER(vp), C.POINTER(vp), u64, vp, C.POINTER(u64), C.POINTER(u64), vp, C.POINTER(u64)]),
         "vgpu_vmlog_free": (None, [vp]),
     }
     for name, (res, args) in sig.items():
@@ -804,6 +809,52 @@ def check_buses(ctx, main, prep, challenges, cap=1 << 16):
     return BusCheck(out, un.value == 0, int(un.value))
 
 
+CellDiff = collections.namedtuple("CellDiff", "chip chip_name trace column column_name row have want")
+ChipDiff = collections.namedtuple("ChipDiff", "chip chip_name height_have height_want cells first_row")
+WitnessDiff = collections.namedtuple("WitnessDiff", "cells total complete chips per_column")
+
+
+def witness_column_count():
+    """The length of diff_witness' per-column counts: the main columns of chips 0..13 in chip order, then the 7 program and the 1
+    range preprocessed columns."""
+    return int(lib().vgpu_witness_column_count())
+
+
+def diff_witness(ctx, log, main, prep, cap=1 << 16):
+    """Every cell of a witness (main / prep: the 14 + 2 DeviceMatrix traces, whole or this rank's row shards on a split context, where
+    every rank calls it and gets the same answer) that differs from what Chip::generate_trace writes for the run `log` (a VmLog)
+    records.  Returns WitnessDiff(cells, total, complete, chips, per_column):
+      - cells: the first min(cap, total) CellDiff(chip, chip_name, trace, column, column_name, row, have, want) in ascending (chip,
+        trace, row, column) order (trace TRACE_MAIN, or TRACE_PREPROCESSED for the program and range traces; have: the witness' word,
+        want: generate_trace's, both canonical), so the first CPU entry is on the first cycle whose row differs;
+      - total: the number of differing cells, complete: whether cells holds them all;
+      - chips: one ChipDiff(chip, chip_name, height_have, height_want, cells, first_row) per chip (first_row -1: none).  A chip whose
+        height differs from the run's is reported there and its cells are not compared;
+      - per_column: the differing cells of each column (witness_column_count() entries).
+    The expected witness is built on the GPU one chip at a time and compared there; nothing is downloaded but the result."""
+    a = (C.c_void_p * NUM_CHIPS)(*[m._h for m in main])
+    b = (C.c_void_p * 2)(*[m._h for m in prep])
+    cap = int(cap)
+    out = np.zeros(cap, dtype=CELL_DIFF_DTYPE)
+    summ = np.zeros(NUM_CHIPS, dtype=DIFF_SUMMARY_DTYPE)
+    per = np.zeros(witness_column_count(), dtype=np.uint64)
+    n, total = C.c_uint64(), C.c_uint64()
+    ctx.check(lib().vgpu_diff_witness(ctx._h, log._h, a, b, cap, out.ctypes.data_as(C.c_void_p) if cap else None, C.byref(n), C.byref(total),
+                                      summ.ctypes.data_as(C.c_void_p), per.ctypes.data_as(C.POINTER(C.c_uint64))))
+    names = {}
+
+    def name(chip, trace, column):
+        key = (chip, trace, column)
+        if key not in names:
+            names[key] = column_name(chip, trace, column)
+        return names[key]
+
+    cells = [CellDiff(int(e["chip"]), CHIP_NAMES[int(e["chip"])], int(e["trace"]), int(e["column"]), name(int(e["chip"]), int(e["trace"]), int(e["column"])),
+                      int(e["row"]), int(e["have"]), int(e["want"])) for e in out[:n.value]]
+    chips = [ChipDiff(c, CHIP_NAMES[c], int(x["height_have"]), int(x["height_want"]), int(x["cells"]), int(x["first_row"])) for c, x in enumerate(summ)]
+    return WitnessDiff(cells, int(total.value), n.value == total.value, chips, per)
+
+
 class StarkConfig:
     """StarkConfigImpl (machine/src/config.rs:33-76): the PCS plus the initial challenger.
 
@@ -1020,6 +1071,10 @@ class VmLog:
         prep = (C.c_void_p * 2)()
         ctx.check(lib().vgpu_witness_device(ctx._h, self._h, main, prep))
         return [DeviceMatrix(ctx, C.c_void_p(main[i])) for i in range(NUM_CHIPS)], [DeviceMatrix(ctx, C.c_void_p(prep[i])) for i in range(2)]
+
+    def diff_witness(self, ctx, main, prep, cap=1 << 16):
+        """diff_witness(ctx, self, main, prep, cap): the cells of a witness that differ from this run's."""
+        return diff_witness(ctx, self, main, prep, cap)
 
     def free(self):
         if self._h:

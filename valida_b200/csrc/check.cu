@@ -522,6 +522,13 @@ int32_t vg_check_shapes(vgpu_ctx* ctx, const vgpu_chip_desc* chip, const vgpu_dm
     return check_shapes(ctx, chip, main, prep, perm, shards);
 }
 
+int32_t vg_cta_scan(vgpu_ctx* ctx, const uint32_t* count, uint32_t m, uint64_t cap, unsigned long long* off, unsigned long long* total, uint32_t* end) {
+    KScope ks(ctx, KC_CHECK, 16.0 * m);
+    fail_scan_kernel<<<1, 1024, 0, ctx->stream>>>(count, m, cap, off, total, end);
+    VG_LAUNCH_CHECK(ctx);
+    return 0;
+}
+
 bool vg_sums_cancel(const vgpu_check_report report[VGPU_NUM_CHIPS]) {
     for (int l = 0; l < 5; l++) {
         uint64_t s = 0;
@@ -622,11 +629,7 @@ extern "C" int32_t vgpu_check_failures(vgpu_ctx* ctx, const vgpu_chip_desc* chip
     };
     VG_TRY(set.sweep(0, main, prep_or_null, perm, challenges, pass1));
     VG_TRY(set.windows(challenges, pass1));
-    {
-        KScope ks(ctx, KC_CHECK, 16.0 * used);
-        fail_scan_kernel<<<1, 1024, 0, ctx->stream>>>(cta.as<uint32_t>(), used, cap, off.as<unsigned long long>(), mine, endb.as<uint32_t>());
-        VG_LAUNCH_CHECK(ctx);
-    }
+    VG_TRY(vg_cta_scan(ctx, cta.as<uint32_t>(), used, cap, off.as<unsigned long long>(), mine, endb.as<uint32_t>()));
     if (run.split) VG_TRY(vg_comm_allgather_inplace(ctx, counts.as<uint32_t>(), words));
     std::vector<unsigned long long> hc((size_t)N * (1 + nc));
     uint32_t end = 0;

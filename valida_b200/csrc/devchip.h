@@ -36,6 +36,9 @@ inline const vgpu_dmat* vg_machine_prep(const vgpu_dmat* const prep[2], int i) {
 // check.cu — refuses, before anything is enqueued and alike on every rank, what the check sweep cannot read (perm may be null;
 // shards: this rank's row shards are accepted)
 int32_t vg_check_shapes(vgpu_ctx* ctx, const vgpu_chip_desc* chip, const vgpu_dmat* main, const vgpu_dmat* prep, const vgpu_dmat* perm, bool shards);
+// check.cu — one CTA (vgpu_check_failures' scan): off[j] = the exclusive prefix sum of the m per-CTA counts, *total their sum, *end = 1 +
+// the last CTA with a count that starts below cap (0: none)
+int32_t vg_cta_scan(vgpu_ctx* ctx, const uint32_t* count, uint32_t m, uint64_t cap, unsigned long long* off, unsigned long long* total, uint32_t* end);
 
 // check.cu — the permutation traces of a machine witness (14 chips, prep[0] / prep[1] the preprocessed traces of chips 1 / 12) and,
 // when `check`, check_constraints of every chip on this rank's run: vgpu_check_witness and prove's debug mode.  perm(i) enqueues

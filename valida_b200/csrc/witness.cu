@@ -12,8 +12,11 @@
 // The short chips (program, mul floor, range, static data, the empty ones) are built on the host (vg_short_chip_traces, a few KB)
 // and uploaded.  Parity: every trace equals the host builder's word for word (tests/test_gpu_witness.py; digests in
 // tests/golden/trace_hashes.json).
+// The host side builds one chip per call (VgWitnessBuilder, witness.h): vgpu_witness_device builds them all, vgpu_diff_witness one at a
+// time, comparing each before it builds the next.
 #include "ctx.h"
 #include "chip_rows.cuh"
+#include "witness.h"
 #include <algorithm>
 #include <memory>
 
@@ -208,6 +211,104 @@ int32_t sort_log_by_addr(vgpu_ctx* ctx, const VgMemOp* d_mem, uint64_t n, VgBuf&
 
 }  // namespace
 
+struct VgWitnessBuilder::Impl {
+    vgpu_ctx* ctx;
+    const VgVmLogs& L;
+    VgBuf d_prog, d_cpu, d_mem, d_adds, d_subs, d_lts, d_bits, d_sa, d_sv;
+    std::unique_ptr<vgpu_traces, void (*)(vgpu_traces*)> st{nullptr, vgpu_traces_free};
+    Impl(vgpu_ctx* c, const VgVmLogs& l)
+        : ctx(c), L(l), d_prog(c), d_cpu(c), d_mem(c), d_adds(c), d_subs(c), d_lts(c), d_bits(c), d_sa(c), d_sv(c) {}
+    // a tall chip's trace: whole, or this rank's run of rows (split proof)
+    int32_t alloc_rows(uint64_t h, uint64_t w, VgMat* out, RowRange* rr) {
+        VG_TRY(vg_dmat_alloc_run(ctx, h, w, vg_trace_run(ctx, h).split, false, out));
+        rr->row0 = (*out)->row0; rr->rows = (*out)->h; rr->out = (*out)->d; rr->cs = (*out)->col_stride;
+        return 0;
+    }
+    int32_t upload(const vgpu_matrix* hm, VgMat* out) {
+        vgpu_dmat* m = nullptr;
+        VG_TRY(vgpu_dmat_upload(ctx, hm, VGPU_REPR_CANONICAL, &m));
+        out->reset(m);
+        return 0;
+    }
+};
+
+VgWitnessBuilder::VgWitnessBuilder(vgpu_ctx* ctx, const VgVmLogs& L) : impl_(new Impl(ctx, L)) {}
+VgWitnessBuilder::~VgWitnessBuilder() = default;
+
+int32_t VgWitnessBuilder::start() {
+    Impl& w = *impl_;
+    const VgVmLogs& L = w.L;
+    VG_TRY(w.d_prog.upload(L.program, 6 * L.n_instr));
+    VG_TRY(w.d_cpu.upload(L.cpu, L.n_cpu));
+    VG_TRY(w.d_mem.upload(L.mem, L.n_mem));
+    VG_TRY(w.d_adds.upload(L.adds, L.n_adds));
+    VG_TRY(w.d_subs.upload(L.subs, L.n_subs));
+    VG_TRY(w.d_lts.upload(L.lts, L.n_lts));
+    VG_TRY(w.d_bits.upload(L.bits, L.n_bits));
+    VG_TRY(w.d_sa.upload(L.static_addr, L.n_static));
+    VG_TRY(w.d_sv.upload(L.static_value, L.n_static));
+    w.st.reset(vg_short_chip_traces(L));
+    return 0;
+}
+
+uint64_t VgWitnessBuilder::height(int c) const {
+    const VgVmLogs& L = impl_->L;
+    switch (c) {
+        case 0: return next_pow2(L.n_cpu);
+        case 2: return next_pow2(L.n_static + L.n_mem);
+        case 3: return next_pow2(L.n_adds);
+        case 4: return next_pow2(L.n_subs);
+        case 8: return next_pow2(L.n_lts);
+        case 10: return next_pow2(L.n_bits);
+        default: return vgpu_traces_main(impl_->st.get(), (uint32_t)c)->height;
+    }
+}
+
+int32_t VgWitnessBuilder::main(int c, VgMat* out) {
+    Impl& w = *impl_;
+    vgpu_ctx* ctx = w.ctx;
+    const VgVmLogs& L = w.L;
+    RowRange rr{};
+    switch (c) {
+        case 0:
+            VG_TRY(w.alloc_rows(height(0), 51, out, &rr));
+            cpu_rows_kernel<<<(unsigned)((rr.rows + 127) / 128), 128, 0, ctx->stream>>>(w.d_cpu.as<VgCpuRec>(), w.d_mem.as<VgMemOp>(), w.d_prog.as<int32_t>(), L.n_cpu, L.n_mem, rr);
+            VG_LAUNCH_CHECK(ctx);
+            return 0;
+        case 2: {   // sort by address (stable), then the rows
+            VgBuf d_order(ctx);
+            VG_TRY(sort_log_by_addr(ctx, w.d_mem.as<VgMemOp>(), L.n_mem, d_order));
+            VG_TRY(w.alloc_rows(height(2), 14, out, &rr));
+            mem_rows_kernel<<<(unsigned)((rr.rows + 255) / 256), 256, 0, ctx->stream>>>(w.d_mem.as<VgMemOp>(), d_order.as<uint32_t>(), L.n_mem, w.d_sa.as<uint32_t>(), w.d_sv.as<uint32_t>(), L.n_static, rr);
+            VG_LAUNCH_CHECK(ctx);
+            return 0;
+        }
+        case 3: case 4: {
+            const int which = c - 3;
+            VG_TRY(w.alloc_rows(height(c), 16, out, &rr));
+            addsub_rows_kernel<<<(unsigned)((rr.rows + 255) / 256), 256, 0, ctx->stream>>>(which ? w.d_subs.as<VgAluRec>() : w.d_adds.as<VgAluRec>(), which ? L.n_subs : L.n_adds, which == 0, rr);
+            VG_LAUNCH_CHECK(ctx);
+            return 0;
+        }
+        case 8:
+            VG_TRY(w.alloc_rows(height(8), 45, out, &rr));
+            lt_rows_kernel<<<(unsigned)((rr.rows + 127) / 128), 128, 0, ctx->stream>>>(w.d_lts.as<VgAluOpRec>(), L.n_lts, rr);
+            VG_LAUNCH_CHECK(ctx);
+            return 0;
+        case 10:
+            VG_TRY(w.alloc_rows(height(10), 79, out, &rr));
+            bitwise_rows_kernel<<<(unsigned)((rr.rows + 127) / 128), 128, 0, ctx->stream>>>(w.d_bits.as<VgAluOpRec>(), L.n_bits, rr);
+            VG_LAUNCH_CHECK(ctx);
+            return 0;
+        default:    // the short chips: built on the host by start() and uploaded whole
+            return w.upload(vgpu_traces_main(w.st.get(), (uint32_t)c), out);
+    }
+}
+
+int32_t VgWitnessBuilder::prep(int which, VgMat* out) {
+    return impl_->upload(vgpu_traces_preprocessed(impl_->st.get(), (uint32_t)which), out);
+}
+
 extern "C" {
 
 // Chip::generate_trace x14 from the interpreter's logs, on the device: main_out[14] / prep_out[2] receive device matrices (column-major
@@ -220,66 +321,12 @@ int32_t vgpu_witness_device(vgpu_ctx* ctx, const vgpu_vmlog* log, vgpu_dmat* mai
     prep_out[0] = prep_out[1] = nullptr;
     if (!L.n_cpu) VG_FAIL(ctx, "witness: the run has no cycles");
     VgMat main[VGPU_NUM_CHIPS], prep[2];                   // handed out only once every trace is built
-    // a tall chip's trace: whole, or this rank's run of rows (split proof)
-    auto alloc_rows = [&](uint64_t h, uint64_t w, VgMat* out, RowRange* rr) -> int32_t {
-        VG_TRY(vg_dmat_alloc_run(ctx, h, w, vg_trace_run(ctx, h).split, false, out));
-        rr->row0 = (*out)->row0; rr->rows = (*out)->h; rr->out = (*out)->d; rr->cs = (*out)->col_stride;
-        return 0;
-    };
-    VgBuf d_prog(ctx), d_cpu(ctx), d_mem(ctx), d_adds(ctx), d_subs(ctx), d_lts(ctx), d_bits(ctx), d_sa(ctx), d_sv(ctx), d_order(ctx);
-    VG_TRY(d_prog.upload(L.program, 6 * L.n_instr));
-    VG_TRY(d_cpu.upload(L.cpu, L.n_cpu));
-    VG_TRY(d_mem.upload(L.mem, L.n_mem));
-    VG_TRY(d_adds.upload(L.adds, L.n_adds));
-    VG_TRY(d_subs.upload(L.subs, L.n_subs));
-    VG_TRY(d_lts.upload(L.lts, L.n_lts));
-    VG_TRY(d_bits.upload(L.bits, L.n_bits));
-    VG_TRY(d_sa.upload(L.static_addr, L.n_static));
-    VG_TRY(d_sv.upload(L.static_value, L.n_static));
-    RowRange rr{};
-    {   // 0 cpu
-        const uint64_t h = next_pow2(L.n_cpu);
-        VG_TRY(alloc_rows(h, 51, &main[0], &rr));
-        cpu_rows_kernel<<<(unsigned)((rr.rows + 127) / 128), 128, 0, ctx->stream>>>(d_cpu.as<VgCpuRec>(), d_mem.as<VgMemOp>(), d_prog.as<int32_t>(), L.n_cpu, L.n_mem, rr);
-        VG_LAUNCH_CHECK(ctx);
-    }
-    {   // 2 memory: sort by address (stable), then the rows
-        VG_TRY(sort_log_by_addr(ctx, d_mem.as<VgMemOp>(), L.n_mem, d_order));
-        const uint64_t h = next_pow2(L.n_static + L.n_mem);
-        VG_TRY(alloc_rows(h, 14, &main[2], &rr));
-        mem_rows_kernel<<<(unsigned)((rr.rows + 255) / 256), 256, 0, ctx->stream>>>(d_mem.as<VgMemOp>(), d_order.as<uint32_t>(), L.n_mem, d_sa.as<uint32_t>(), d_sv.as<uint32_t>(), L.n_static, rr);
-        VG_LAUNCH_CHECK(ctx);
-    }
-    for (int which = 0; which < 2; which++) {   // 3 add, 4 sub
-        const uint64_t n = which ? L.n_subs : L.n_adds, h = next_pow2(n);
-        VG_TRY(alloc_rows(h, 16, &main[3 + which], &rr));
-        addsub_rows_kernel<<<(unsigned)((rr.rows + 255) / 256), 256, 0, ctx->stream>>>(which ? d_subs.as<VgAluRec>() : d_adds.as<VgAluRec>(), n, which == 0, rr);
-        VG_LAUNCH_CHECK(ctx);
-    }
-    {   // 8 lt
-        const uint64_t h = next_pow2(L.n_lts);
-        VG_TRY(alloc_rows(h, 45, &main[8], &rr));
-        lt_rows_kernel<<<(unsigned)((rr.rows + 127) / 128), 128, 0, ctx->stream>>>(d_lts.as<VgAluOpRec>(), L.n_lts, rr);
-        VG_LAUNCH_CHECK(ctx);
-    }
-    {   // 10 bitwise
-        const uint64_t h = next_pow2(L.n_bits);
-        VG_TRY(alloc_rows(h, 79, &main[10], &rr));
-        bitwise_rows_kernel<<<(unsigned)((rr.rows + 127) / 128), 128, 0, ctx->stream>>>(d_bits.as<VgAluOpRec>(), L.n_bits, rr);
-        VG_LAUNCH_CHECK(ctx);
-    }
-    {   // the short chips: built on the host (a few KB) and uploaded whole
-        std::unique_ptr<vgpu_traces, void (*)(vgpu_traces*)> st(vg_short_chip_traces(L), vgpu_traces_free);
-        auto upload = [&](const vgpu_matrix* hm, VgMat* out) -> int32_t {
-            vgpu_dmat* m = nullptr;
-            VG_TRY(vgpu_dmat_upload(ctx, hm, VGPU_REPR_CANONICAL, &m));
-            out->reset(m);
-            return 0;
-        };
-        for (uint32_t c = 0; c < VGPU_NUM_CHIPS; c++)
-            if (!main[c]) VG_TRY(upload(vgpu_traces_main(st.get(), c), &main[c]));     // the tall chips are built above
-        for (uint32_t w = 0; w < 2; w++) VG_TRY(upload(vgpu_traces_preprocessed(st.get(), w), &prep[w]));
-    }
+    VgWitnessBuilder wb(ctx, L);
+    VG_TRY(wb.start());
+    for (int c : {0, 2, 3, 4, 8, 10}) VG_TRY(wb.main(c, &main[c]));     // the tall chips, built from the logs on the device
+    for (int c = 0; c < VGPU_NUM_CHIPS; c++)
+        if (!main[c]) VG_TRY(wb.main(c, &main[c]));
+    for (int w = 0; w < 2; w++) VG_TRY(wb.prep(w, &prep[w]));
     VG_CUDA(ctx, cudaStreamSynchronize(ctx->stream));      // the logs are the caller's (pageable) memory: they may go once this returns
     for (int i = 0; i < VGPU_NUM_CHIPS; i++) main_out[i] = main[i].release();
     for (int i = 0; i < 2; i++) prep_out[i] = prep[i].release();
