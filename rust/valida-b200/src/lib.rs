@@ -358,10 +358,14 @@ impl Context {
         self.check(sys::vgpu_ctx_record_event(self.raw, cuda_event))
     }
 
+    /// The handle arrays of a machine witness (14 main and 2 preprocessed traces), as the calls that take one want them.
+    fn witness_ptrs(main: &[&DMat<'_>; sys::VGPU_NUM_CHIPS], prep: &[&DMat<'_>; 2]) -> ([*const vgpu_dmat; sys::VGPU_NUM_CHIPS], [*const vgpu_dmat; 2]) {
+        (std::array::from_fn(|i| main[i].as_ptr()), std::array::from_fn(|i| prep[i].as_ptr()))
+    }
+
     /// `Machine::prove` from traces already on the device (imported or borrowed): the same bytes as [`Context::prove_bytes`].
     pub fn prove_device_bytes(&self, main: &[&DMat<'_>; sys::VGPU_NUM_CHIPS], prep: &[&DMat<'_>; 2]) -> Result<Vec<u8>> {
-        let main_raw: Vec<*const vgpu_dmat> = main.iter().map(|m| m.as_ptr()).collect();
-        let prep_raw: Vec<*const vgpu_dmat> = prep.iter().map(|m| m.as_ptr()).collect();
+        let (main_raw, prep_raw) = Self::witness_ptrs(main, prep);
         let (mut bytes, mut len) = (ptr::null_mut::<u8>(), 0u64);
         let code = unsafe { sys::vgpu_prove_device(self.raw, main_raw.as_ptr(), prep_raw.as_ptr(), &mut bytes, &mut len) };
         self.check(code)?;
@@ -412,8 +416,7 @@ impl Context {
     /// the cumulative sums cancel.  `main` / `prep` are whole traces or, on a [`LocalGroup`] rank, its row shards; every rank of a
     /// split proof makes the call and gets the same reports.  A host that splits proofs runs this in debug builds.
     pub fn check_witness(&self, main: &[&DMat<'_>; sys::VGPU_NUM_CHIPS], prep: &[&DMat<'_>; 2], challenges: &[u32; 15]) -> Result<([sys::vgpu_check_report; sys::VGPU_NUM_CHIPS], bool)> {
-        let main_raw: Vec<*const vgpu_dmat> = main.iter().map(|m| m.as_ptr()).collect();
-        let prep_raw: Vec<*const vgpu_dmat> = prep.iter().map(|m| m.as_ptr()).collect();
+        let (main_raw, prep_raw) = Self::witness_ptrs(main, prep);
         let mut reports = [sys::vgpu_check_report::default(); sys::VGPU_NUM_CHIPS];
         let mut cancel = 0i32;
         self.check(unsafe { sys::vgpu_check_witness(self.raw, main_raw.as_ptr(), prep_raw.as_ptr(), challenges.as_ptr(), reports.as_mut_ptr(), &mut cancel) })?;
@@ -426,8 +429,7 @@ impl Context {
     /// [`Context::check_witness`] takes; collective on a split context, with the same result on every rank.  Synchronises.
     pub fn check_buses(&self, main: &[&DMat<'_>; sys::VGPU_NUM_CHIPS], prep: &[&DMat<'_>; 2], challenges: &[u32; 15], cap: usize)
                        -> Result<(Vec<sys::vgpu_bus_imbalance>, Vec<sys::vgpu_bus_event>, u64)> {
-        let main_raw: Vec<*const vgpu_dmat> = main.iter().map(|m| m.as_ptr()).collect();
-        let prep_raw: Vec<*const vgpu_dmat> = prep.iter().map(|m| m.as_ptr()).collect();
+        let (main_raw, prep_raw) = Self::witness_ptrs(main, prep);
         let mut tuples = vec![sys::vgpu_bus_imbalance::default(); cap];
         let mut events = vec![sys::vgpu_bus_event::default(); cap];
         let (mut nt, mut ne, mut unexamined) = (0u64, 0u64, 0u64);
@@ -473,8 +475,7 @@ impl Context {
     /// device one chip at a time.  Synchronises.
     pub fn diff_witness(&self, log: &VmLog, main: &[&DMat<'_>; sys::VGPU_NUM_CHIPS], prep: &[&DMat<'_>; 2], cap: usize)
                         -> Result<(Vec<sys::vgpu_cell_diff>, u64, [sys::vgpu_diff_summary; sys::VGPU_NUM_CHIPS], Vec<u64>)> {
-        let main_raw: Vec<*const vgpu_dmat> = main.iter().map(|m| m.as_ptr()).collect();
-        let prep_raw: Vec<*const vgpu_dmat> = prep.iter().map(|m| m.as_ptr()).collect();
+        let (main_raw, prep_raw) = Self::witness_ptrs(main, prep);
         let mut out = vec![sys::vgpu_cell_diff::default(); cap];
         let mut summary = [sys::vgpu_diff_summary::default(); sys::VGPU_NUM_CHIPS];
         let mut per_column = vec![0u64; witness_column_count()];

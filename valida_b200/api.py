@@ -607,6 +607,11 @@ def _h(m):
     return m._h if m is not None else None
 
 
+def _witness_handles(main, prep):
+    """The handle arrays of a machine witness: 14 main and 2 preprocessed DeviceMatrix traces."""
+    return (C.c_void_p * NUM_CHIPS)(*[m._h for m in main]), (C.c_void_p * 2)(*[m._h for m in prep])
+
+
 def generate_permutation_trace(ctx, chip_id, main, prep, random_elements):
     """machine/src/chip.rs:121 — returns (flattened perm trace DeviceMatrix, cumulative_sum[5])."""
     chip = lib().vgpu_basic_machine_chip(chip_id)
@@ -765,11 +770,9 @@ def check_witness(ctx, main, prep, challenges):
     """check_constraints of the 14 chips and check_cumulative_sums over a machine witness (the reference's debug-build check), without
     a proof: main / prep are the 14 + 2 DeviceMatrix traces (whole, or this rank's row shards on a split context, where every rank
     calls it).  Returns ([(first row or -1, constraint, failing rows, cumulative sum [5]) per chip], sums_cancel)."""
-    a = (C.c_void_p * NUM_CHIPS)(*[m._h for m in main])
-    b = (C.c_void_p * 2)(*[m._h for m in prep])
     rep = (_CheckReport * NUM_CHIPS)()
     cancel = C.c_int32()
-    ctx.check(lib().vgpu_check_witness(ctx._h, a, b, _u32arr(challenges, 15), rep, C.byref(cancel)))
+    ctx.check(lib().vgpu_check_witness(ctx._h, *_witness_handles(main, prep), _u32arr(challenges, 15), rep, C.byref(cancel)))
     return ([(int(r.first_row), int(r.first_constraint), int(r.failing_rows), np.array(list(r.cumulative_sum), dtype=np.uint32)) for r in rep],
             bool(cancel.value))
 
@@ -787,13 +790,11 @@ def check_buses(ctx, main, prep, challenges, cap=1 << 16):
     BusEvent(chip, chip_name, interaction, row, multiplicity, send) in ascending (chip, row, interaction) order.  cap bounds the events
     (and so the tuples) examined; complete is False when unexamined > 0 candidate groups did not fit, and every tuple listed is exact
     either way.  The list is empty exactly when the LogUp sums cancel."""
-    a = (C.c_void_p * NUM_CHIPS)(*[m._h for m in main])
-    b = (C.c_void_p * 2)(*[m._h for m in prep])
     cap = int(cap)
     tup = np.zeros(cap, dtype=BUS_IMBALANCE_DTYPE)
     ev = np.zeros(cap, dtype=BUS_EVENT_DTYPE)
     nt, ne, un = C.c_uint64(), C.c_uint64(), C.c_uint64()
-    ctx.check(lib().vgpu_check_buses(ctx._h, a, b, _u32arr(challenges, 15), cap, tup.ctypes.data_as(C.c_void_p) if cap else None,
+    ctx.check(lib().vgpu_check_buses(ctx._h, *_witness_handles(main, prep), _u32arr(challenges, 15), cap, tup.ctypes.data_as(C.c_void_p) if cap else None,
                                      C.byref(nt), ev.ctypes.data_as(C.c_void_p) if cap else None, C.byref(ne), C.byref(un)))
     out = []
     for t in tup[:nt.value]:
@@ -832,14 +833,12 @@ def diff_witness(ctx, log, main, prep, cap=1 << 16):
         height differs from the run's is reported there and its cells are not compared;
       - per_column: the differing cells of each column (witness_column_count() entries).
     The expected witness is built on the GPU one chip at a time and compared there; nothing is downloaded but the result."""
-    a = (C.c_void_p * NUM_CHIPS)(*[m._h for m in main])
-    b = (C.c_void_p * 2)(*[m._h for m in prep])
     cap = int(cap)
     out = np.zeros(cap, dtype=CELL_DIFF_DTYPE)
     summ = np.zeros(NUM_CHIPS, dtype=DIFF_SUMMARY_DTYPE)
     per = np.zeros(witness_column_count(), dtype=np.uint64)
     n, total = C.c_uint64(), C.c_uint64()
-    ctx.check(lib().vgpu_diff_witness(ctx._h, log._h, a, b, cap, out.ctypes.data_as(C.c_void_p) if cap else None, C.byref(n), C.byref(total),
+    ctx.check(lib().vgpu_diff_witness(ctx._h, log._h, *_witness_handles(main, prep), cap, out.ctypes.data_as(C.c_void_p) if cap else None, C.byref(n), C.byref(total),
                                       summ.ctypes.data_as(C.c_void_p), per.ctypes.data_as(C.POINTER(C.c_uint64))))
     names = {}
 
@@ -883,10 +882,7 @@ def prove_machine(config, traces, device_resident=None, repr=REPR_CANONICAL):
     out = C.POINTER(C.c_uint8)()
     n = C.c_uint64()
     if device_resident is not None:
-        dm, dp = device_resident
-        a = (C.c_void_p * NUM_CHIPS)(*[m._h for m in dm])
-        b = (C.c_void_p * 2)(*[m._h for m in dp])
-        ctx.check(lib().vgpu_prove_device(ctx._h, a, b, C.byref(out), C.byref(n)))
+        ctx.check(lib().vgpu_prove_device(ctx._h, *_witness_handles(*device_resident), C.byref(out), C.byref(n)))
     else:
         keep = [_as_u32(m) for m in traces.main] + [_as_u32(m) for m in traces.preprocessed]
         a = (_Matrix * NUM_CHIPS)(*[_mat(m) for m in keep[:NUM_CHIPS]])

@@ -3,8 +3,8 @@
 // zero: its bus, its tuple (the interaction's fields on the row, zero-padded to VGPU_MAX_FIELDS, so trailing zeros do not tell
 // tuples apart, as they do not in the LogUp denominator r1^(bus+1) + sum_f r2^f field_f) and its sign (send +, receive -).  A tuple
 // is unbalanced when its sends minus its receives are not 0 mod p; the LogUp sums cancel iff no tuple is (whp over the challenges).
-// Three sweeps of every row of this rank's run (vg_trace_run; a chip every rank holds whole is swept by rank 0 only,
-// vg_reports_replicated), each one thread per row over the chip's DevChip (logup::pair_col), no per-chip template:
+// Three sweeps of every row of this rank's run (a chip every rank holds whole is swept by rank 0 only: vg_reports_trace), each one
+// thread per row over the chip's DevChip (logup::pair_col), no per-chip template:
 //   1. bucket: each event adds +-mult / (z - L) into the bucket hash(bus, tuple) mod B, with L = limb 0 of the tuple's LogUp
 //      denominator and z = limb 0 of the first challenge.  The buckets (reduced to canonical words, all-gathered on a split
 //      context) that do not sum to zero are the CANDIDATES, numbered in bucket order.
@@ -13,6 +13,7 @@
 // The host groups the events by exact tuple, drops the balanced ones that shared a bucket with an unbalanced one, and sorts.
 #include "ctx.h"
 #include "devchip.h"
+#include "lists.cuh"
 #include "logup.cuh"
 #include <array>
 #include <map>
@@ -143,10 +144,7 @@ extern "C" int32_t vgpu_check_buses(vgpu_ctx* ctx, const vgpu_dmat* const main[V
                                     vgpu_bus_event* events, uint64_t* n_events, uint64_t* unexamined) {
     if (!main || !prep || !challenges) VG_FAIL(ctx, "check_buses: null argument");
     if (!n_tuples || !n_events || !unexamined || (cap && (!tuples || !events))) VG_FAIL(ctx, "check_buses: null output");
-    for (int i = 0; i < VGPU_NUM_CHIPS; i++) {
-        if (!main[i]) VG_FAIL(ctx, "check_buses: chip %d has no trace", i);
-        VG_TRY(vg_check_shapes(ctx, vgpu_basic_machine_chip(i), main[i], vg_machine_prep(prep, i), nullptr, true));
-    }
+    VG_TRY(vg_check_machine(ctx, "check_buses", main, prep));
     VG_TRY(vg_enter(ctx));
     // the plan, from global heights and the run rule alone: alike on every rank
     const bool gather = vg_sharded(ctx);
@@ -161,15 +159,13 @@ extern "C" int32_t vgpu_check_buses(vgpu_ctx* ctx, const vgpu_dmat* const main[V
     for (int i = 0; i < VGPU_NUM_CHIPS; i++) {
         const vgpu_chip_desc* d = vgpu_basic_machine_chip(i);
         const vgpu_dmat *m = main[i], *pr = vg_machine_prep(prep, i);
-        const VgRun run = vg_trace_run(ctx, m->gh);
-        if (!d->n_interactions || (!run.split && !vg_reports_replicated(ctx))) continue;
+        VgRun run;
+        if (!d->n_interactions || !vg_reports_trace(ctx, m->gh, &run)) continue;
         VG_TRY(vg_dmat_materialize(ctx, m));
         VG_TRY(vg_dmat_materialize(ctx, pr));
         auto p = std::make_unique<BParams>();
-        // first row of the run: a shard starts there, a whole trace is entered at run.begin
-        auto rows_of = [&](const vgpu_dmat* x) -> const uint32_t* { return x ? x->d + (x->dist == VG_ROWS ? 0 : run.begin) : nullptr; };
-        p->main = rows_of(m); p->mcs = m->col_stride;
-        p->prep = rows_of(pr); p->pcs = pr ? pr->col_stride : 0;
+        p->main = vg_run_rows(m, run); p->mcs = m->col_stride;
+        p->prep = vg_run_rows(pr, run); p->pcs = pr ? pr->col_stride : 0;
         p->g0 = run.begin; p->n = run.count;
         p->z = z; p->log_b = log_b;
         for (uint32_t k = 0; k < d->n_interactions; k++) p->bus[k] = d->interactions[k].bus;
@@ -244,31 +240,25 @@ extern "C" int32_t vgpu_check_buses(vgpu_ctx* ctx, const vgpu_dmat* const main[V
     *unexamined = K - J;
     if (!J) return 0;
     std::vector<uint64_t> per(N, 0);
-    uint64_t block = 0;
-    for (uint32_t r = 0; r < N; r++) {
+    for (uint32_t r = 0; r < N; r++)
         for (uint32_t c = 0; c < J; c++) per[r] += hc[(size_t)r * K + c];
-        block = std::max(block, per[r]);
-    }
-    VgBuf ents(ctx), wpos(ctx);
-    VG_TRY(ents.alloc(std::max<uint64_t>(N * block, 1) * sizeof(BusEventRec)));
-    VG_TRY(wpos.alloc(8));
-    VG_CUDA(ctx, cudaMemsetAsync(wpos.p, 0, 8, ctx->stream));
-    for (auto& p : sweeps) { p->examined = J; p->wpos = wpos.as<unsigned long long>(); p->out = ents.as<BusEventRec>() + (uint64_t)me * block; }
-    VG_TRY(launch(bus_write_kernel));
-    if (gather && block) VG_TRY(vg_comm_allgather_inplace(ctx, ents.as<uint32_t>(), block * sizeof(BusEventRec) / 4));
-    std::vector<BusEventRec> he((size_t)N * block);
-    if (!he.empty()) VG_CUDA(ctx, cudaMemcpyAsync(he.data(), ents.p, he.size() * sizeof(BusEventRec), cudaMemcpyDeviceToHost, ctx->stream));
-    VG_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
+    std::vector<BusEventRec> he(fit);
+    uint64_t gathered = 0;
+    VG_TRY(vg_gather_lists(ctx, gather, per, cap, [&](BusEventRec* slot) -> int32_t {
+        VgBuf wpos(ctx);
+        VG_TRY(wpos.alloc(8));
+        VG_CUDA(ctx, cudaMemsetAsync(wpos.p, 0, 8, ctx->stream));
+        for (auto& p : sweeps) { p->examined = J; p->wpos = wpos.as<unsigned long long>(); p->out = slot; }
+        return launch(bus_write_kernel);
+    }, he.data(), fit, &gathered));
     // group by exact tuple (bus, fields): ascending, as the map orders its keys
     std::map<std::array<uint32_t, 1 + VGPU_MAX_FIELDS>, std::vector<const BusEventRec*>> groups;
-    for (uint32_t r = 0; r < N; r++)
-        for (uint64_t e = 0; e < per[r]; e++) {
-            const BusEventRec& x = he[(size_t)r * block + e];
-            std::array<uint32_t, 1 + VGPU_MAX_FIELDS> key;
-            key[0] = x.bus;
-            std::copy(x.fields, x.fields + VGPU_MAX_FIELDS, key.begin() + 1);
-            groups[key].push_back(&x);
-        }
+    for (const BusEventRec& x : he) {
+        std::array<uint32_t, 1 + VGPU_MAX_FIELDS> key;
+        key[0] = x.bus;
+        std::copy(x.fields, x.fields + VGPU_MAX_FIELDS, key.begin() + 1);
+        groups[key].push_back(&x);
+    }
     uint64_t nt = 0, ne = 0;
     for (auto& [key, evs] : groups) {
         uint32_t net = 0;

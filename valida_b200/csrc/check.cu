@@ -21,6 +21,7 @@
 #include "devchip.h"
 #include "airs.cuh"
 #include "logup.cuh"
+#include "lists.cuh"
 #include "open.h"
 #include <functional>
 #include <memory>
@@ -115,35 +116,6 @@ int32_t copy_segments(vgpu_ctx* ctx, const CopyList& l, int nseg) {
     return 0;
 }
 
-// Refuses, before anything is enqueued and alike on every rank (global shapes and this context's run rule only), what the sweep
-// cannot check.  perm may be null (vgpu_check_witness builds it).  shards: row shards of this rank's run are accepted.
-int32_t check_shapes(vgpu_ctx* ctx, const vgpu_chip_desc* chip, const vgpu_dmat* main, const vgpu_dmat* prep, const vgpu_dmat* perm, bool shards) {
-    if (chip->chip_id >= VGPU_NUM_CHIPS) VG_FAIL(ctx, "check_constraints: unknown chip id %u", chip->chip_id);
-    for (const vgpu_dmat* m : {main, prep, perm}) {
-        if (!m) continue;
-        if (!shards && (m->dist != VG_FULL || m->bitrev_rows)) VG_FAIL(ctx, "check_constraints: whole matrices in natural row order only (not row shards)");
-        if (m->bitrev_rows) VG_FAIL(ctx, "check_constraints: a matrix stores its rows bit-reversed (quotient chunks); the check reads traces in natural row order");
-    }
-    if (main->gw != chip->width) VG_FAIL(ctx, "check_constraints: main width %llu != chip width %u", (unsigned long long)main->gw, chip->width);
-    const uint64_t pw = 5ull * (chip->n_interactions + 1);
-    if (perm && perm->gw != pw) VG_FAIL(ctx, "check_constraints: permutation trace width %llu != 5 (k + 1) = %llu", (unsigned long long)perm->gw, (unsigned long long)pw);
-    if (chip->preprocessed_width && !prep) VG_FAIL(ctx, "check_constraints: chip %u needs its preprocessed trace (%u columns)", chip->chip_id, chip->preprocessed_width);
-    if (!chip->preprocessed_width && prep) VG_FAIL(ctx, "check_constraints: chip %u has no preprocessed trace", chip->chip_id);
-    if (prep && prep->gw != chip->preprocessed_width) VG_FAIL(ctx, "check_constraints: preprocessed width %llu != %u", (unsigned long long)prep->gw, chip->preprocessed_width);
-    const uint64_t h = main->gh;
-    if (h == 0 || (h & (h - 1))) VG_FAIL(ctx, "check_constraints: trace height %llu is not a power of two", (unsigned long long)h);
-    if ((perm && perm->gh != h) || (prep && prep->gh != h)) VG_FAIL(ctx, "check_constraints: the main, preprocessed and permutation traces differ in height");
-    const VgRun run = vg_trace_run(ctx, h);
-    for (const vgpu_dmat* m : {main, prep, perm})
-        if (m && m->dist == VG_ROWS && !(run.split && m->row0 == run.begin && m->h == run.count))
-            VG_FAIL(ctx, "check_constraints: a row shard holding rows [%llu, %llu) of a trace of height %llu is not this context's run of that "
-                    "height, rows [%llu, %llu)%s", (unsigned long long)m->row0, (unsigned long long)(m->row0 + m->h), (unsigned long long)h,
-                    (unsigned long long)run.begin, (unsigned long long)(run.begin + run.count), run.split ? "" : " (the trace is not split here)");
-    const uint32_t N = vg_chip_base_constraints(chip->chip_id) + chip->n_interactions + 3;
-    if (N > CHECK_MAX_CONSTRAINTS) VG_FAIL(ctx, "check_constraints: %u constraints exceed the 8-bit index (%u)", N, CHECK_MAX_CONSTRAINTS);
-    return 0;
-}
-
 // Enqueues one run's sweep; p holds everything but the chip, which is built here from the challenges.
 int32_t enqueue_sweep(vgpu_ctx* ctx, const vgpu_chip_desc* chip, const uint32_t challenges[15], CParams& p) {
     if (!p.n) return 0;
@@ -215,13 +187,9 @@ __global__ void __maxnreg__(128) fail_count_kernel(const __grid_constant__ FPara
     const uint64_t i = b.active ? i_raw : p.n - 1;        // idle lanes shadow the last row (the warp vote needs every lane)
     eval_row<CHIP>(p, i, b);
     __syncthreads();
-    __shared__ uint32_t warp_total[4];
     uint32_t s = 0;
     for (uint32_t t = threadIdx.x; t < CHECK_MAX_CONSTRAINTS; t += blockDim.x) s += fail_hist[t];
-    s = __reduce_add_sync(0xffffffffu, s);
-    if ((threadIdx.x & 31) == 0) warp_total[threadIdx.x >> 5] = s;
-    __syncthreads();
-    const uint32_t total = warp_total[0] + warp_total[1] + warp_total[2] + warp_total[3];
+    const uint32_t total = vg_cta_total<4>(s);
     if (!total) return;
     if (threadIdx.x == 0) f.cta_count[f.cta0 + blockIdx.x] = total;
     for (uint32_t t = threadIdx.x; t < CHECK_MAX_CONSTRAINTS; t += blockDim.x)
@@ -242,18 +210,7 @@ __global__ void __maxnreg__(128) fail_write_kernel(const __grid_constant__ FPara
     b.pos = 0; b.end = 0;
     eval_row<CHIP>(p, i, b);
     // the thread's first entry: the failures of the CTA's lower threads
-    __shared__ uint32_t warp_total[4];
-    const uint32_t mine = active ? b.pos : 0, lane = threadIdx.x & 31;
-    uint32_t x = mine;
-#pragma unroll
-    for (int d = 1; d < 32; d <<= 1) {
-        const uint32_t y = __shfl_up_sync(0xffffffffu, x, d);
-        if (lane >= (uint32_t)d) x += y;
-    }
-    if (lane == 31) warp_total[threadIdx.x >> 5] = x;
-    __syncthreads();
-    uint32_t first = x - mine;
-    for (uint32_t w = 0; w < (threadIdx.x >> 5); w++) first += warp_total[w];
+    const uint32_t mine = active ? b.pos : 0, first = vg_cta_exclusive<4>(mine);
     const uint32_t end = (uint32_t)min((unsigned long long)total, f.cap - base);
     if (!mine || first >= end) return;
     b.pos = first; b.end = end;
@@ -351,9 +308,7 @@ class CheckSet {
         VG_TRY(vg_dmat_materialize(ctx_, prep));
         VG_TRY(vg_dmat_materialize(ctx_, perm));
         const uint64_t row0 = c.run.begin, cnt = c.run.count, k = c.desc->n_interactions;
-        // first row of the run: a shard starts there, a whole trace is entered at row0 (perm.cu's rule)
-        auto rows_of = [&](const vgpu_dmat* m) -> const uint32_t* { return m ? m->d + (m->dist == VG_ROWS ? 0 : row0) : nullptr; };
-        const uint32_t *md = rows_of(main), *pd = rows_of(prep), *qd = rows_of(perm);
+        const uint32_t *md = vg_run_rows(main, c.run), *pd = vg_run_rows(prep, c.run), *qd = vg_run_rows(perm, c.run);
         const uint64_t mcs = main->col_stride, pcs = prep ? prep->col_stride : 0, qcs = perm->col_stride;
         auto pp = std::make_unique<CParams>();
         CParams& p = *pp;
@@ -498,7 +453,7 @@ int32_t VgMachineCheck::perm(int i, VgMat* out) {
 
 int32_t VgMachineCheck::sweep(int i, const vgpu_dmat* perm) {
     // prove's debug mode refuses here what check_constraints refuses; vgpu_check_witness has refused it before enqueueing anything
-    VG_TRY(check_shapes(ctx_, vgpu_basic_machine_chip(i), main_[i], prep_for(i), perm, vg_sharded(ctx_)));
+    VG_TRY(vg_check_shapes(ctx_, vgpu_basic_machine_chip(i), main_[i], prep_for(i), perm, vg_sharded(ctx_)));
     return set_->sweep(i, main_[i], prep_for(i), perm, challenges_);
 }
 
@@ -518,8 +473,41 @@ int32_t VgMachineCheck::finish(uint32_t sums[VGPU_NUM_CHIPS][5], vgpu_check_repo
     return 0;
 }
 
+// Refuses, before anything is enqueued and alike on every rank (global shapes and this context's run rule only), what the sweep
+// cannot check.  perm may be null (vgpu_check_witness builds it).  shards: row shards of this rank's run are accepted.
 int32_t vg_check_shapes(vgpu_ctx* ctx, const vgpu_chip_desc* chip, const vgpu_dmat* main, const vgpu_dmat* prep, const vgpu_dmat* perm, bool shards) {
-    return check_shapes(ctx, chip, main, prep, perm, shards);
+    if (chip->chip_id >= VGPU_NUM_CHIPS) VG_FAIL(ctx, "check_constraints: unknown chip id %u", chip->chip_id);
+    for (const vgpu_dmat* m : {main, prep, perm}) {
+        if (!m) continue;
+        if (!shards && (m->dist != VG_FULL || m->bitrev_rows)) VG_FAIL(ctx, "check_constraints: whole matrices in natural row order only (not row shards)");
+        if (m->bitrev_rows) VG_FAIL(ctx, "check_constraints: a matrix stores its rows bit-reversed (quotient chunks); the check reads traces in natural row order");
+    }
+    if (main->gw != chip->width) VG_FAIL(ctx, "check_constraints: main width %llu != chip width %u", (unsigned long long)main->gw, chip->width);
+    const uint64_t pw = 5ull * (chip->n_interactions + 1);
+    if (perm && perm->gw != pw) VG_FAIL(ctx, "check_constraints: permutation trace width %llu != 5 (k + 1) = %llu", (unsigned long long)perm->gw, (unsigned long long)pw);
+    if (chip->preprocessed_width && !prep) VG_FAIL(ctx, "check_constraints: chip %u needs its preprocessed trace (%u columns)", chip->chip_id, chip->preprocessed_width);
+    if (!chip->preprocessed_width && prep) VG_FAIL(ctx, "check_constraints: chip %u has no preprocessed trace", chip->chip_id);
+    if (prep && prep->gw != chip->preprocessed_width) VG_FAIL(ctx, "check_constraints: preprocessed width %llu != %u", (unsigned long long)prep->gw, chip->preprocessed_width);
+    const uint64_t h = main->gh;
+    if (h == 0 || (h & (h - 1))) VG_FAIL(ctx, "check_constraints: trace height %llu is not a power of two", (unsigned long long)h);
+    if ((perm && perm->gh != h) || (prep && prep->gh != h)) VG_FAIL(ctx, "check_constraints: the main, preprocessed and permutation traces differ in height");
+    const VgRun run = vg_trace_run(ctx, h);
+    for (const vgpu_dmat* m : {main, prep, perm})
+        if (m && m->dist == VG_ROWS && !(run.split && m->row0 == run.begin && m->h == run.count))
+            VG_FAIL(ctx, "check_constraints: a row shard holding rows [%llu, %llu) of a trace of height %llu is not this context's run of that "
+                    "height, rows [%llu, %llu)%s", (unsigned long long)m->row0, (unsigned long long)(m->row0 + m->h), (unsigned long long)h,
+                    (unsigned long long)run.begin, (unsigned long long)(run.begin + run.count), run.split ? "" : " (the trace is not split here)");
+    const uint32_t N = vg_chip_constraints(chip);
+    if (N > CHECK_MAX_CONSTRAINTS) VG_FAIL(ctx, "check_constraints: %u constraints exceed the 8-bit index (%u)", N, CHECK_MAX_CONSTRAINTS);
+    return 0;
+}
+
+int32_t vg_check_machine(vgpu_ctx* ctx, const char* what, const vgpu_dmat* const main[VGPU_NUM_CHIPS], const vgpu_dmat* const prep[2]) {
+    for (int i = 0; i < VGPU_NUM_CHIPS; i++) {
+        if (!main[i]) VG_FAIL(ctx, "%s: chip %d has no trace", what, i);
+        VG_TRY(vg_check_shapes(ctx, vgpu_basic_machine_chip(i), main[i], vg_machine_prep(prep, i), nullptr, true));
+    }
+    return 0;
 }
 
 int32_t vg_cta_scan(vgpu_ctx* ctx, const uint32_t* count, uint32_t m, uint64_t cap, unsigned long long* off, unsigned long long* total, uint32_t* end) {
@@ -543,7 +531,7 @@ extern "C" int32_t vgpu_check_constraints(vgpu_ctx* ctx, const vgpu_chip_desc* c
                                           int64_t* first_row, uint32_t* first_constraint, uint64_t* failing_rows) {
     if (!first_row || !first_constraint || !failing_rows) VG_FAIL(ctx, "check_constraints: null output");
     if (!chip || !main || !perm || !challenges) VG_FAIL(ctx, "check_constraints: null argument");
-    VG_TRY(check_shapes(ctx, chip, main, prep_or_null, perm, false));
+    VG_TRY(vg_check_shapes(ctx, chip, main, prep_or_null, perm, false));
     return check_chip(ctx, true, chip, main, prep_or_null, perm, challenges, first_row, first_constraint, failing_rows);
 }
 
@@ -552,18 +540,15 @@ extern "C" int32_t vgpu_check_constraints_local(vgpu_ctx* ctx, const vgpu_chip_d
                                                 int64_t* first_row, uint32_t* first_constraint, uint64_t* failing_rows) {
     if (!first_row || !first_constraint || !failing_rows) VG_FAIL(ctx, "check_constraints_local: null output");
     if (!chip || !main || !perm || !challenges) VG_FAIL(ctx, "check_constraints_local: null argument");
-    VG_TRY(check_shapes(ctx, chip, main, prep_or_null, perm, true));
+    VG_TRY(vg_check_shapes(ctx, chip, main, prep_or_null, perm, true));
     return check_chip(ctx, false, chip, main, prep_or_null, perm, challenges, first_row, first_constraint, failing_rows);
 }
 
 extern "C" int32_t vgpu_check_witness(vgpu_ctx* ctx, const vgpu_dmat* const main[VGPU_NUM_CHIPS], const vgpu_dmat* const prep[2],
                                       const uint32_t challenges[15], vgpu_check_report report[VGPU_NUM_CHIPS], int32_t* sums_cancel) {
     if (!main || !prep || !challenges || !report || !sums_cancel) VG_FAIL(ctx, "check_witness: null argument");
+    VG_TRY(vg_check_machine(ctx, "check_witness", main, prep));
     VgMachineCheck mc(ctx, main, prep, challenges, true);
-    for (int i = 0; i < VGPU_NUM_CHIPS; i++) {
-        if (!main[i]) VG_FAIL(ctx, "check_witness: chip %d has no trace", i);
-        VG_TRY(check_shapes(ctx, vgpu_basic_machine_chip(i), main[i], mc.prep_for(i), nullptr, true));
-    }
     VG_TRY(vg_enter(ctx));
     VG_TRY(mc.alloc());
     for (int i = 0; i < VGPU_NUM_CHIPS; i++) {
@@ -578,23 +563,22 @@ extern "C" int32_t vgpu_check_witness(vgpu_ctx* ctx, const vgpu_dmat* const main
 }
 
 extern "C" int32_t vgpu_chip_constraint_count(const vgpu_chip_desc* chip, uint32_t* air_constraints, uint32_t* total) {
-    if (!chip || !air_constraints || !total || chip->chip_id >= VGPU_NUM_CHIPS || chip->n_interactions > VGPU_MAX_INTERACTIONS) return -1;
+    if (!vg_chip_ok(chip) || !air_constraints || !total) return -1;
     *air_constraints = vg_chip_base_constraints(chip->chip_id);
-    *total = *air_constraints + chip->n_interactions + 3;
+    *total = vg_chip_constraints(chip);
     return 0;
 }
 
-// Per rank, [total, failures per constraint] (u64 words): all-gathered when the chip is split, and then the totals size one block of
-// entries per rank, which one more all-gather exchanges.  Rank r's entries are rows of its run, below rank r + 1's: the list is the
-// ranks' lists in rank order.
+// Per rank, [total, failures per constraint] (u64 words), all-gathered when the chip is split; then the ranks' lists, gathered.  Rank
+// r's entries are rows of its run, below rank r + 1's: the list is the ranks' lists in rank order.
 extern "C" int32_t vgpu_check_failures(vgpu_ctx* ctx, const vgpu_chip_desc* chip, const vgpu_dmat* main, const vgpu_dmat* prep_or_null,
                                        const vgpu_dmat* perm, const uint32_t challenges[15], uint64_t cap, vgpu_check_failure* out,
                                        uint64_t* n_out, uint64_t* total_failures, uint64_t* rows_per_constraint) {
     if (!n_out || !total_failures || (cap && !out)) VG_FAIL(ctx, "check_failures: null output");
     if (!chip || !main || !perm || !challenges) VG_FAIL(ctx, "check_failures: null argument");
-    VG_TRY(check_shapes(ctx, chip, main, prep_or_null, perm, true));
+    VG_TRY(vg_check_shapes(ctx, chip, main, prep_or_null, perm, true));
     VG_TRY(vg_enter(ctx));
-    const uint32_t nc = vg_chip_base_constraints(chip->chip_id) + chip->n_interactions + 3;
+    const uint32_t nc = vg_chip_constraints(chip);
     const VgRun run = vg_trace_run(ctx, main->gh);
     const uint32_t N = run.split ? (uint32_t)ctx->comm_size : 1, me = run.split ? (uint32_t)ctx->comm_rank : 0;
     // the run's sweep of its rows but the last, then the window of the last row, when split; else one sweep of the whole trace
@@ -603,7 +587,7 @@ extern "C" int32_t vgpu_check_failures(vgpu_ctx* ctx, const vgpu_chip_desc* chip
     CheckSet set(ctx, 1);
     set.plan(0, chip, main->gh);
     VG_TRY(set.alloc());
-    VgBuf counts(ctx), cta(ctx), off(ctx), endb(ctx), ents(ctx);
+    VgBuf counts(ctx), cta(ctx), off(ctx), endb(ctx);
     VG_TRY(counts.alloc(N * words * 4));
     VG_TRY(cta.alloc(ctas * 4ull));
     VG_TRY(off.alloc(ctas * 8ull));
@@ -636,34 +620,21 @@ extern "C" int32_t vgpu_check_failures(vgpu_ctx* ctx, const vgpu_chip_desc* chip
     VG_CUDA(ctx, cudaMemcpyAsync(hc.data(), counts.p, hc.size() * 8, cudaMemcpyDeviceToHost, ctx->stream));
     VG_CUDA(ctx, cudaMemcpyAsync(&end, endb.p, 4, cudaMemcpyDeviceToHost, ctx->stream));
     VG_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
-    uint64_t total = 0, block = 0;
-    for (uint32_t r = 0; r < N; r++) {
-        const uint64_t t = hc[(size_t)r * (1 + nc)];
-        total += t;
-        block = std::max(block, std::min<uint64_t>(t, cap));
-    }
-    uint64_t n = 0;
-    if (block) {                                          // alike on every rank: from the gathered totals
-        VG_TRY(ents.alloc(N * block * sizeof(vgpu_check_failure)));
+    std::vector<uint64_t> found(N);
+    uint64_t total = 0;
+    for (uint32_t r = 0; r < N; r++) total += found[r] = hc[(size_t)r * (1 + nc)];
+    VG_TRY(vg_gather_lists(ctx, run.split, found, cap, [&](vgpu_check_failure* slot) -> int32_t {
         for (auto& f : sweeps) {
             if (end <= f->cta0) break;
-            f->out = ents.as<vgpu_check_failure>() + me * block; f->cap = cap;
+            f->out = slot; f->cap = cap;
             const FParams& fp = *f;
             const uint32_t grid = std::min<uint32_t>(end - f->cta0, (uint32_t)((f->c.n + 127) / 128));
             KScope ks(ctx, KC_CHECK, 0.0);
             air::with_chip(chip->chip_id, [&](auto c) { fail_write_kernel<decltype(c)::value><<<grid, 128, 0, ctx->stream>>>(fp); });
             VG_LAUNCH_CHECK(ctx);
         }
-        if (run.split) VG_TRY(vg_comm_allgather_inplace(ctx, ents.as<uint32_t>(), block * sizeof(vgpu_check_failure) / 4));
-        for (uint32_t r = 0; r < N && n < cap; r++) {
-            const uint64_t k = std::min<uint64_t>(std::min<uint64_t>(hc[(size_t)r * (1 + nc)], cap), cap - n);
-            if (k) VG_CUDA(ctx, cudaMemcpyAsync(out + n, ents.as<vgpu_check_failure>() + r * block, k * sizeof(vgpu_check_failure),
-                                                cudaMemcpyDeviceToHost, ctx->stream));
-            n += k;
-        }
-        VG_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
-    }
-    *n_out = n;
+        return 0;
+    }, out, cap, n_out));
     *total_failures = total;
     if (rows_per_constraint)
         for (uint32_t c = 0; c < nc; c++) {

@@ -226,8 +226,17 @@ inline bool vg_layer_split(uint64_t len, int nranks) {
     return true;
 }
 inline VgRun vg_layer_run(uint64_t len, int nranks, int rank) { return vg_run(len, nranks, rank, vg_layer_split(len, nranks)); }
+// The first row of this rank's run in m (null for no matrix): a row shard starts there, a whole matrix is entered at run.begin.
+inline const uint32_t* vg_run_rows(const vgpu_dmat* m, const VgRun& run) { return m ? m->d + (m->dist == VG_ROWS ? 0 : run.begin) : nullptr; }
 // A query answer is summed over the ranks, so of data every rank holds only rank 0 reports its words.
 inline bool vg_reports_replicated(const vgpu_ctx* ctx) { return ctx->comm_rank == 0 || !vg_sharded(ctx); }
+// Whether this rank sweeps a trace of h rows in a machine-wide report (*run: its rows): its run if the trace is split, else rank 0 only.
+inline bool vg_reports_trace(const vgpu_ctx* ctx, uint64_t h, VgRun* run) { *run = vg_trace_run(ctx, h); return run->split || vg_reports_replicated(ctx); }
+// m's word at stored row `row`, column col, when this rank reports it (holds the row in its shard, or is rank 0 of a whole m); else null
+inline const uint32_t* vg_reported_word(const vgpu_ctx* ctx, const vgpu_dmat* m, uint64_t row, uint64_t col) {
+    const bool mine = m->dist == VG_ROWS ? (row >= m->row0 && row < m->row0 + m->h) : vg_reports_replicated(ctx);
+    return mine ? m->d + col * m->col_stride + (row - m->row0) : nullptr;
+}
 // The part of a gh x gw matrix this rank holds: its run of stored rows when `split` (VG_ROWS), else all of it (VG_FULL).
 // symm: taken from the symmetric heap (peers store into it and read it); such a shard has the column stride vg_run_max on every rank,
 // so that every rank's allocation, and a column's place in it, is the same.

@@ -31,14 +31,18 @@ uint32_t vg_perm_totals_ranks(const vgpu_ctx* ctx);
 // the cumulative sum (Montgomery) from the n per-rank totals ([rank][limb]) vg_perm_trace_enqueue left for a chip
 void vg_perm_totals_fold(const uint32_t* totals, uint32_t n, uint32_t out[5]);
 
+uint32_t vg_chip_base_constraints(uint32_t chip_id);   // quotient.cu
+// every constraint of a chip in eval order: Air::eval's assertions (vg_chip_base_constraints), one per interaction, the 3 LogUp ones
+inline uint32_t vg_chip_constraints(const vgpu_chip_desc* chip) { return vg_chip_base_constraints(chip->chip_id) + chip->n_interactions + 3; }
+// a description of one of the machine's chips with no more interactions than a DevChip holds
+inline bool vg_chip_ok(const vgpu_chip_desc* chip) { return chip && chip->chip_id < VGPU_NUM_CHIPS && chip->n_interactions <= VGPU_MAX_INTERACTIONS; }
 // The preprocessed trace of machine chip i (prep[0] / prep[1]: chips 1 / 12), null for the others.
 inline const vgpu_dmat* vg_machine_prep(const vgpu_dmat* const prep[2], int i) { return i == 1 ? prep[0] : i == 12 ? prep[1] : nullptr; }
 // check.cu — refuses, before anything is enqueued and alike on every rank, what the check sweep cannot read (perm may be null;
 // shards: this rank's row shards are accepted)
 int32_t vg_check_shapes(vgpu_ctx* ctx, const vgpu_chip_desc* chip, const vgpu_dmat* main, const vgpu_dmat* prep, const vgpu_dmat* perm, bool shards);
-// check.cu — one CTA (vgpu_check_failures' scan): off[j] = the exclusive prefix sum of the m per-CTA counts, *total their sum, *end = 1 +
-// the last CTA with a count that starts below cap (0: none)
-int32_t vg_cta_scan(vgpu_ctx* ctx, const uint32_t* count, uint32_t m, uint64_t cap, unsigned long long* off, unsigned long long* total, uint32_t* end);
+// check.cu — the same for the 14 + 2 traces of a machine witness (their permutation traces not yet built); `what` names the call
+int32_t vg_check_machine(vgpu_ctx* ctx, const char* what, const vgpu_dmat* const main[VGPU_NUM_CHIPS], const vgpu_dmat* const prep[2]);
 
 // check.cu — the permutation traces of a machine witness (14 chips, prep[0] / prep[1] the preprocessed traces of chips 1 / 12) and,
 // when `check`, check_constraints of every chip on this rank's run: vgpu_check_witness and prove's debug mode.  perm(i) enqueues

@@ -11,6 +11,7 @@
 // Words are compared as stored (Montgomery); only the reported words are made canonical.
 #include "ctx.h"
 #include "devchip.h"
+#include "lists.cuh"
 #include "witness.h"
 #include "host/vmlog.h"
 #include <algorithm>
@@ -58,7 +59,6 @@ __device__ __forceinline__ void row_diffs(const DParams& p, uint64_t i, F&& f) {
 
 __global__ void __launch_bounds__(DIFF_THREADS) diff_count_kernel(const __grid_constant__ DParams p) {
     __shared__ uint32_t hist[DIFF_MAX_COLS];
-    __shared__ uint32_t warp_total[DIFF_WARPS];
     __shared__ uint32_t low;                                 // the CTA's lowest thread with a difference
     for (uint32_t t = threadIdx.x; t < p.width; t += blockDim.x) hist[t] = 0;
     if (threadIdx.x == 0) low = 0xffffffffu;
@@ -67,12 +67,7 @@ __global__ void __launch_bounds__(DIFF_THREADS) diff_count_kernel(const __grid_c
     uint32_t mine = 0;
     if (i < p.n) row_diffs(p, i, [&](uint32_t c, uint32_t, uint32_t) { atomicAdd(&hist[c], 1u); mine++; });
     if (mine) atomicMin(&low, threadIdx.x);
-    const uint32_t s = __reduce_add_sync(0xffffffffu, mine);
-    if ((threadIdx.x & 31) == 0) warp_total[threadIdx.x >> 5] = s;
-    __syncthreads();
-    uint32_t total = 0;
-#pragma unroll
-    for (int w = 0; w < DIFF_WARPS; w++) total += warp_total[w];
+    const uint32_t total = vg_cta_total<DIFF_WARPS>(mine);
     if (threadIdx.x == 0) p.cta_count[blockIdx.x] = total;
     if (!total) return;
     if (threadIdx.x == 0) atomicMin(p.first, (unsigned long long)(p.g0 + (uint64_t)blockIdx.x * blockDim.x + low));
@@ -88,18 +83,7 @@ __global__ void __launch_bounds__(DIFF_THREADS) diff_write_kernel(const __grid_c
     uint32_t mine = 0;
     if (i < p.n) row_diffs(p, i, [&](uint32_t, uint32_t, uint32_t) { mine++; });
     // the thread's first entry: the differences of the CTA's lower threads
-    __shared__ uint32_t warp_total[DIFF_WARPS];
-    const uint32_t lane = threadIdx.x & 31;
-    uint32_t x = mine;
-#pragma unroll
-    for (int d = 1; d < 32; d <<= 1) {
-        const uint32_t y = __shfl_up_sync(0xffffffffu, x, d);
-        if (lane >= (uint32_t)d) x += y;
-    }
-    if (lane == 31) warp_total[threadIdx.x >> 5] = x;
-    __syncthreads();
-    uint32_t pos = x - mine;
-    for (uint32_t w = 0; w < (threadIdx.x >> 5); w++) pos += warp_total[w];
+    uint32_t pos = vg_cta_exclusive<DIFF_WARPS>(mine);
     const uint32_t end = (uint32_t)min((unsigned long long)total, p.cap - base);
     if (!mine || pos >= end) return;
     vgpu_cell_diff* out = p.out + base;
@@ -133,10 +117,7 @@ extern "C" int32_t vgpu_diff_witness(vgpu_ctx* ctx, const vgpu_vmlog* log, const
     if (!ctx) return -1;
     if (!log || !main || !prep) VG_FAIL(ctx, "diff_witness: null argument");
     if (!n_out || !total || !summary || (cap && !out)) VG_FAIL(ctx, "diff_witness: null output");
-    for (int i = 0; i < VGPU_NUM_CHIPS; i++) {
-        if (!main[i]) VG_FAIL(ctx, "diff_witness: chip %d has no trace", i);
-        VG_TRY(vg_check_shapes(ctx, vgpu_basic_machine_chip(i), main[i], vg_machine_prep(prep, i), nullptr, true));
-    }
+    VG_TRY(vg_check_machine(ctx, "diff_witness", main, prep));
     const VgVmLogs& L = *vg_vmlog_view(log);
     if (!L.n_cpu) VG_FAIL(ctx, "diff_witness: the run has no cycles");
     VG_TRY(vg_enter(ctx));
@@ -153,21 +134,18 @@ extern "C" int32_t vgpu_diff_witness(vgpu_ctx* ctx, const vgpu_vmlog* log, const
     VG_CUDA(ctx, cudaMemsetAsync(mine + VGPU_NUM_CHIPS, 0, ncol * 8, ctx->stream));
     // this rank's first min(its cells, cap) entries: straight into out on a lone context, else gathered below
     std::vector<vgpu_cell_diff> local;
-    vgpu_cell_diff* dst = gather ? nullptr : out;
     uint64_t listed = 0;
     // Compares this rank's run of one trace of chip c with generate_trace's (cb: its first per-column count), then lists its
     // differences while the list has room.
     auto compare = [&](int c, uint32_t trace, const vgpu_dmat* have, const vgpu_dmat* want, const VgRun& run, uint64_t cb) -> int32_t {
         VG_TRY(vg_dmat_materialize(ctx, have));
         if (!run.count) return 0;
-        // first row of the run: a shard starts there, a whole matrix is entered at run.begin
-        auto rows_of = [&](const vgpu_dmat* m) -> const uint32_t* { return m->d + (m->dist == VG_ROWS ? 0 : run.begin); };
         const unsigned grid = blocks_of(run.count);
         VgBuf cta(ctx);
         VG_TRY(cta.alloc((size_t)grid * 4));
         DParams p{};
-        p.have = rows_of(have); p.hcs = have->col_stride;
-        p.want = rows_of(want); p.wcs = want->col_stride;
+        p.have = vg_run_rows(have, run); p.hcs = have->col_stride;
+        p.want = vg_run_rows(want, run); p.wcs = want->col_stride;
         p.g0 = run.begin; p.n = run.count;
         p.width = (uint32_t)have->gw; p.chip = (uint32_t)c; p.trace = trace;
         p.cta_count = cta.as<uint32_t>(); p.cols = mine + VGPU_NUM_CHIPS + cb; p.first = mine + c;
@@ -194,7 +172,7 @@ extern "C" int32_t vgpu_diff_witness(vgpu_ctx* ctx, const vgpu_vmlog* log, const
             VG_LAUNCH_CHECK(ctx);
         }
         if (gather) local.resize(listed + k);
-        VG_CUDA(ctx, cudaMemcpyAsync((gather ? local.data() : dst) + listed, ents.p, k * sizeof(vgpu_cell_diff), cudaMemcpyDeviceToHost, ctx->stream));
+        VG_CUDA(ctx, cudaMemcpyAsync((gather ? local.data() : out) + listed, ents.p, k * sizeof(vgpu_cell_diff), cudaMemcpyDeviceToHost, ctx->stream));
         VG_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
         listed += k;
         return 0;
@@ -202,8 +180,8 @@ extern "C" int32_t vgpu_diff_witness(vgpu_ctx* ctx, const vgpu_vmlog* log, const
     for (int c = 0; c < VGPU_NUM_CHIPS; c++) {
         const uint64_t h = wb.height(c);
         if (h != main[c]->gh) continue;                      // reported in the summary, not compared
-        const VgRun run = vg_trace_run(ctx, h);
-        if (!run.split && !vg_reports_replicated(ctx)) continue;
+        VgRun run;
+        if (!vg_reports_trace(ctx, h, &run)) continue;
         VgMat want;                                          // back to the cache once its comparison is done
         VG_TRY(wb.main(c, &want));
         VG_TRY(compare(c, VGPU_TRACE_MAIN, main[c], want.get(), run, column_base(c)));
@@ -221,26 +199,22 @@ extern "C" int32_t vgpu_diff_witness(vgpu_ctx* ctx, const vgpu_vmlog* log, const
     std::vector<uint64_t> per_rank(N, 0), cols(ncol, 0);
     unsigned long long first[VGPU_NUM_CHIPS];
     std::fill(first, first + VGPU_NUM_CHIPS, ~0ull);
+    uint64_t all = 0;
     for (uint32_t r = 0; r < N; r++) {
         const unsigned long long* b = hc.data() + (size_t)r * words;
         for (int c = 0; c < VGPU_NUM_CHIPS; c++) first[c] = std::min(first[c], b[c]);
         for (uint64_t j = 0; j < ncol; j++) { cols[j] += b[VGPU_NUM_CHIPS + j]; per_rank[r] += b[VGPU_NUM_CHIPS + j]; }
+        all += per_rank[r];
     }
-    uint64_t all = 0, block = 0;
-    for (uint32_t r = 0; r < N; r++) { all += per_rank[r]; block = std::max(block, std::min<uint64_t>(per_rank[r], cap)); }
-    if (gather && block) {                                   // alike on every rank: from the gathered counts
-        VgBuf ents(ctx);
-        VG_TRY(ents.alloc((size_t)N * block * sizeof(vgpu_cell_diff)));
-        vgpu_cell_diff* blocks = ents.as<vgpu_cell_diff>();
-        if (listed) VG_CUDA(ctx, cudaMemcpyAsync(blocks + (uint64_t)me * block, local.data(), listed * sizeof(vgpu_cell_diff), cudaMemcpyHostToDevice, ctx->stream));
-        VG_TRY(vg_comm_allgather_inplace(ctx, ents.as<uint32_t>(), block * sizeof(vgpu_cell_diff) / 4));
-        std::vector<vgpu_cell_diff> every((size_t)N * block);
-        VG_CUDA(ctx, cudaMemcpyAsync(every.data(), blocks, every.size() * sizeof(vgpu_cell_diff), cudaMemcpyDeviceToHost, ctx->stream));
-        VG_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
+    if (gather) {
         // each rank's list is ascending; the first cap of the union are among the ranks' first cap
         std::vector<vgpu_cell_diff> merged;
-        for (uint32_t r = 0; r < N; r++)
-            merged.insert(merged.end(), every.begin() + (size_t)r * block, every.begin() + (size_t)r * block + std::min<uint64_t>(per_rank[r], cap));
+        for (uint64_t x : per_rank) merged.resize(merged.size() + std::min(x, cap));
+        uint64_t gathered = 0;
+        VG_TRY(vg_gather_lists(ctx, true, per_rank, cap, [&](vgpu_cell_diff* slot) -> int32_t {
+            if (listed) VG_CUDA(ctx, cudaMemcpyAsync(slot, local.data(), listed * sizeof(vgpu_cell_diff), cudaMemcpyHostToDevice, ctx->stream));
+            return 0;
+        }, merged.data(), merged.size(), &gathered));
         std::sort(merged.begin(), merged.end(), [](const vgpu_cell_diff& a, const vgpu_cell_diff& b) {
             return std::tie(a.chip, a.trace, a.row, a.column) < std::tie(b.chip, b.trace, b.row, b.column);
         });

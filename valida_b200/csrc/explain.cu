@@ -140,7 +140,7 @@ const NameTable& names() {
 }
 
 const char* column_name(const vgpu_chip_desc* chip, int32_t trace, uint32_t column) {
-    if (!chip || chip->chip_id >= VGPU_NUM_CHIPS || chip->n_interactions > VGPU_MAX_INTERACTIONS) return nullptr;
+    if (!vg_chip_ok(chip)) return nullptr;
     const NameTable& t = names();
     if (trace == VGPU_TRACE_MAIN || trace == VGPU_TRACE_PREPROCESSED) {
         const std::vector<std::string>& v = trace == VGPU_TRACE_MAIN ? t.main[chip->chip_id] : t.prep[chip->chip_id];
@@ -210,8 +210,6 @@ bool constraint_cells(const vgpu_chip_desc* chip, uint32_t c, const char** label
     return true;
 }
 
-bool chip_ok(const vgpu_chip_desc* chip) { return chip && chip->chip_id < VGPU_NUM_CHIPS && chip->n_interactions <= VGPU_MAX_INTERACTIONS; }
-
 }  // namespace
 
 extern "C" const char* vgpu_chip_column_name(const vgpu_chip_desc* chip, int32_t trace, uint32_t column) {
@@ -220,7 +218,7 @@ extern "C" const char* vgpu_chip_column_name(const vgpu_chip_desc* chip, int32_t
 
 extern "C" int32_t vgpu_chip_constraint_cells(const vgpu_chip_desc* chip, uint32_t constraint, const char** label, vgpu_cell* cells,
                                               uint32_t cap, uint32_t* n) {
-    if (!chip_ok(chip) || !label || !n || (cap && !cells)) return -1;
+    if (!vg_chip_ok(chip) || !label || !n || (cap && !cells)) return -1;
     std::vector<vgpu_cell> v;
     if (!constraint_cells(chip, constraint, label, &v)) return -1;
     for (uint32_t i = 0; i < v.size() && i < cap; i++) cells[i] = v[i];
@@ -236,7 +234,7 @@ extern "C" int32_t vgpu_explain_failures(vgpu_ctx* ctx, const vgpu_chip_desc* ch
     if (chip->n_interactions > VGPU_MAX_INTERACTIONS) VG_FAIL(ctx, "explain_failures: %u interactions exceed %d", chip->n_interactions, VGPU_MAX_INTERACTIONS);
     VG_TRY(vg_check_shapes(ctx, chip, main, prep_or_null, perm_or_null, true));
     const uint64_t h = main->gh;
-    const uint32_t total = vg_chip_base_constraints(chip->chip_id) + chip->n_interactions + 3;
+    const uint32_t total = vg_chip_constraints(chip);
     // every item's cells, in catalogue order; refused alike on every rank (the list and the global shapes only)
     std::vector<std::vector<vgpu_cell>> cat(total);
     std::vector<bool> have(total, false);
@@ -272,10 +270,8 @@ extern "C" int32_t vgpu_explain_failures(vgpu_ctx* ctx, const vgpu_chip_desc* ch
         for (const vgpu_cell& c : cat[items[i].constraint]) {
             const vgpu_dmat* m = mats[c.trace];
             if (!m) { slot[j++] = ~0ull; continue; }
-            const uint64_t g = c.next ? (row + 1) % h : row;
-            const bool mine = m->dist == VG_ROWS ? (g >= m->row0 && g < m->row0 + m->h) : vg_reports_replicated(ctx);
             slot[j++] = ptrs.size();
-            ptrs.push_back(mine ? m->d + (uint64_t)c.column * m->col_stride + (g - m->row0) : nullptr);
+            ptrs.push_back(vg_reported_word(ctx, m, c.next ? (row + 1) % h : row, c.column));
         }
         first[i + 1] = j;
     }

@@ -264,8 +264,7 @@ int32_t open_multi_batches(vgpu_ctx* ctx, const std::vector<OpenRound>& rounds, 
             uint64_t bidx = index >> (log_max - lg);
             for (auto* m : rd.pd->ldes) {
                 const uint64_t row = bidx >> (lg - log2u(m->gh));
-                const bool mine = m->dist == VG_ROWS ? (row >= m->row0 && row < m->row0 + m->h) : vg_reports_replicated(ctx);
-                for (uint64_t c = 0; c < m->w; c++) *o++ = mine ? m->d + c * m->col_stride + (row - m->row0) : nullptr;
+                for (uint64_t c = 0; c < m->w; c++) *o++ = vg_reported_word(ctx, m, row, c);
             }
             push_path(layers.size() + r);
         }

@@ -16,6 +16,5 @@ int32_t vg_reduced_opening_accumulate(vgpu_ctx* ctx, const vgpu_dmat* lde, const
 int32_t vg_fri_fold(vgpu_ctx* ctx, const uint32_t* cur, uint64_t ccs, uint64_t n, uint64_t i0, uint64_t count, const bb::E5& beta,
                     const uint32_t* add_v, uint64_t acs, uint32_t* out_v, uint64_t ocs);
 int32_t vg_gather_words(vgpu_ctx* ctx, const std::vector<const uint32_t*>& ptrs, std::vector<uint32_t>* out);
-uint32_t vg_chip_base_constraints(uint32_t chip_id);
 namespace vgh { struct Challenger; }
 int32_t vg_pow_grind(vgpu_ctx* ctx, vgh::Challenger& ch, int bits, uint32_t* witness_monty);   // pow.cu

@@ -240,14 +240,12 @@ int32_t vg_perm_trace_enqueue(vgpu_ctx* ctx, const vgpu_chip_desc* chip, const v
     const VgRun run = vg_trace_run(ctx, main->gh);
     const bool split = run.split;
     if (!split && main->dist != VG_FULL) VG_FAIL(ctx, "perm_trace: the trace is a shard but too short to be split");
-    const uint64_t h = run.count, row0 = run.begin;          // rows swept here
+    const uint64_t h = run.count;                            // rows swept here
     uint32_t k = chip->n_interactions;
     VgMat perm;
     VG_TRY(vg_dmat_alloc_run(ctx, main->gh, 5 * (k + 1), split, false, &perm));
-    // first swept row of a matrix: a shard starts there, a whole trace is entered at row0
-    auto rows_of = [&](const vgpu_dmat* m) { return m->d + (m->dist == VG_ROWS ? 0 : row0); };
-    const uint32_t* md = rows_of(main);
-    const uint32_t* pd = prep_or_null ? rows_of(prep_or_null) : nullptr;
+    const uint32_t* md = vg_run_rows(main, run);
+    const uint32_t* pd = vg_run_rows(prep_or_null, run);
     uint64_t pcs = prep_or_null ? prep_or_null->col_stride : 0;
     unsigned blocks = (unsigned)((h + 255) / 256);
     uint32_t* phi = perm->d + (uint64_t)(5 * k) * perm->col_stride;

@@ -198,7 +198,7 @@ extern "C" int32_t vgpu_quotient(vgpu_ctx* ctx, const vgpu_chip_desc* chip, uint
     const bool split = main_lde->dist == VG_ROWS;
     if ((perm_lde->dist == VG_ROWS) != split || (prep_lde && (prep_lde->dist == VG_ROWS) != split)) VG_FAIL(ctx, "quotient: the LDEs are not distributed alike");
     // alpha powers for N = base + k + 3 constraints
-    const uint32_t N = vg_chip_base_constraints(chip->chip_id) + chip->n_interactions + 3;
+    const uint32_t N = vg_chip_constraints(chip);
     if (N > Q_MAX_CONSTRAINTS) { VG_FAIL(ctx, "quotient: %u constraints exceed the parameter table (%u)", N, Q_MAX_CONSTRAINTS); }
     auto pp = std::make_unique<QParams>();
     QParams& p = *pp;
