@@ -503,6 +503,34 @@ int32_t vgpu_diff_witness(vgpu_ctx* ctx, const vgpu_vmlog* log, const vgpu_dmat*
                           uint64_t cap, vgpu_cell_diff* out, uint64_t* n_out, uint64_t* total,
                           vgpu_diff_summary summary[VGPU_NUM_CHIPS], uint64_t* per_column_or_null);
 
+/* ---- which cells of a witness no check pins ------------------------------------------------------------------------------------
+ * One main-trace cell that no constraint and no bus event depends on. */
+typedef struct vgpu_free_cell {
+    int64_t row;                /* global row */
+    uint32_t column;            /* main-trace column */
+} vgpu_free_cell;
+/* Every FREE main-trace cell (row r, column c) of one chip's witness: a cell such that
+ *   - every assertion of the chip's Air::eval keeps its value whatever the cell holds, on row r (the cell as the local row's column c)
+ *     and on row (r - 1) mod h with that row's own selectors (the cell as the next row's column c; on a one-row chip the cell is both
+ *     of the one evaluation).  Every constraint has degree <= 3, so this is decided exactly from the cell + 0, + 1, + 2 and + 3;
+ *   - no interaction's count gives column c a non-zero summed weight, and, on a row where an interaction's count is not 0, none of
+ *     its fields does (so no bus event of the row changes with the cell).
+ * Changing one free cell of a witness that passes vgpu_check_witness to any value gives a witness that still passes (its permutation
+ * trace rebuilt), so a proof of it verifies; changing a pinned cell at random is caught by the AIR or unbalances a bus tuple.  Only
+ * single cells are judged.  Preprocessed and permutation cells are not.  Writes:
+ *   - out[0, *n_out): the first min(cap, *total) free cells, in ascending (row, column) order;
+ *   - rows_per_column (may be NULL, else chip->width entries): the free rows of each column.
+ * Takes what vgpu_check_failures takes without perm and the challenges (whole matrices, or this rank's row shards; uploaded, imported
+ * or borrowed, with any column stride) and refuses the same traces, a matrix stored with bit-reversed rows, a row shard that is not
+ * this context's run, out == NULL with cap > 0 and a null n_out or total, before anything is enqueued and alike on every rank.  One
+ * thread per row evaluates the AIR with 4-lane values for each column the AIR reads; a second pass, in the parts of the trace whose
+ * cells fall below cap only, writes.  Collective on a split context, with byte-identical output on every rank: a split chip is swept
+ * over this rank's run, whose edge rows come from one all-gather of each rank's first and last main rows; one all-gather brings the
+ * per-rank counts and, when something is free and cap > 0, one more each rank's first min(count, cap) cells.  A chip too short to
+ * be split is swept whole by every rank.  Synchronises. */
+int32_t vgpu_free_cells(vgpu_ctx* ctx, const vgpu_chip_desc* chip, const vgpu_dmat* main, const vgpu_dmat* prep_or_null,
+                        uint64_t cap, vgpu_free_cell* out, uint64_t* n_out, uint64_t* total, uint64_t* rows_per_column);
+
 /* fib_program of basic/tests/test_prover.rs:35-188 with `imm32 -8(fp)` = n; returns the instruction count (23). */
 uint64_t vgpu_fib_program(uint32_t n, int32_t* out_words /* >= 23*6 */);
 

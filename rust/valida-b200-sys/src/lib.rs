@@ -196,6 +196,16 @@ pub struct vgpu_diff_summary {
     pub first_row: i64,
 }
 
+/// One main-trace cell that no constraint and no bus event depends on ([`vgpu_free_cells`]).
+#[repr(C)]
+#[derive(Clone, Copy, Debug, Default, PartialEq, Eq)]
+pub struct vgpu_free_cell {
+    /// Global row.
+    pub row: i64,
+    /// Main-trace column.
+    pub column: u32,
+}
+
 extern "C" {
     // ---- context ----
     pub fn vgpu_ctx_create(device: i32, cuda_stream: *mut c_void, out: *mut *mut vgpu_ctx) -> i32;
@@ -301,5 +311,6 @@ extern "C" {
     pub fn vgpu_vmlog_free(log: *mut vgpu_vmlog);
     pub fn vgpu_witness_column_count() -> u64;
     pub fn vgpu_diff_witness(ctx: *mut vgpu_ctx, log: *const vgpu_vmlog, main: *const *const vgpu_dmat, prep: *const *const vgpu_dmat, cap: u64, out: *mut vgpu_cell_diff, n_out: *mut u64, total: *mut u64, summary: *mut vgpu_diff_summary, per_column_or_null: *mut u64) -> i32;
+    pub fn vgpu_free_cells(ctx: *mut vgpu_ctx, chip: *const vgpu_chip_desc, main: *const vgpu_dmat, prep_or_null: *const vgpu_dmat, cap: u64, out: *mut vgpu_free_cell, n_out: *mut u64, total: *mut u64, rows_per_column: *mut u64) -> i32;
     pub fn vgpu_fib_program(n: u32, out_words: *mut i32) -> u64;
 }

@@ -71,6 +71,8 @@ CELL_ABSENT = 0xFFFFFFFF      # vgpu_explain_failures' word for a permutation ce
 # vgpu_cell_diff / vgpu_diff_summary (include/valida_b200.h)
 CELL_DIFF_DTYPE = np.dtype([("chip", "<u4"), ("trace", "<u4"), ("column", "<u4"), ("row", "<i8"), ("have", "<u4"), ("want", "<u4")], align=True)
 DIFF_SUMMARY_DTYPE = np.dtype([("height_have", "<u8"), ("height_want", "<u8"), ("cells", "<u8"), ("first_row", "<i8")])
+# vgpu_free_cell (include/valida_b200.h): one main-trace cell no check pins
+FREE_CELL_DTYPE = np.dtype([("row", "<i8"), ("column", "<u4")], align=True)
 
 
 def _load():
@@ -163,6 +165,7 @@ def _load():
         "vgpu_witness_column_count": (u64, []),
         "vgpu_diff_witness": (C.c_int32, [vp, vp, C.POINTER(vp), C.POINTER(vp), u64, vp, C.POINTER(u64), C.POINTER(u64), vp, C.POINTER(u64)]),
         "vgpu_vmlog_free": (None, [vp]),
+        "vgpu_free_cells": (C.c_int32, [vp, vp, vp, vp, u64, vp, C.POINTER(u64), C.POINTER(u64), C.POINTER(u64)]),
     }
     for name, (res, args) in sig.items():
         f = getattr(L, name)
@@ -852,6 +855,34 @@ def diff_witness(ctx, log, main, prep, cap=1 << 16):
                       int(e["row"]), int(e["have"]), int(e["want"])) for e in out[:n.value]]
     chips = [ChipDiff(c, CHIP_NAMES[c], int(x["height_have"]), int(x["height_want"]), int(x["cells"]), int(x["first_row"])) for c, x in enumerate(summ)]
     return WitnessDiff(cells, int(total.value), n.value == total.value, chips, per)
+
+
+FreeCell = collections.namedtuple("FreeCell", "row column column_name")
+FreeCells = collections.namedtuple("FreeCells", "cells total complete per_column")
+
+
+def free_cells(ctx, chip_id, main, prep, cap=1 << 16):
+    """Every main-trace cell of one chip's witness that no check pins: no assertion of the chip's Air::eval changes with the cell (on
+    its row, and on the row before as that row's next row), and no bus event does (no interaction's count reads its column, and on a
+    row where an interaction's count is not 0 none of its fields does).  Changing one such cell of a witness that passes check_witness
+    leaves it passing, so its proof still verifies: the cells are the chip's AIR gaps on this witness.  Takes what check_failures
+    takes without perm and challenges (whole matrices, or on a split context this rank's row shards; collective there, with the same
+    result on every rank).  Returns FreeCells(cells, total, complete, per_column): the first min(cap, total) FreeCell(row, column,
+    column_name) in ascending (row, column) order, the number of free cells, whether cells holds them all, and per column name its
+    number of free rows."""
+    cap = int(cap)
+    chip = lib().vgpu_basic_machine_chip(chip_id)
+    if not chip:
+        raise VgpuError("free_cells: unknown chip id %r" % (chip_id,))
+    width = C.cast(chip, C.POINTER(_ChipDesc)).contents.width
+    out = np.zeros(cap, dtype=FREE_CELL_DTYPE)
+    per = np.zeros(width, dtype=np.uint64)
+    n, total = C.c_uint64(), C.c_uint64()
+    ctx.check(lib().vgpu_free_cells(ctx._h, chip, main._h, _h(prep), cap, out.ctypes.data_as(C.c_void_p) if cap else None, C.byref(n),
+                                    C.byref(total), per.ctypes.data_as(C.POINTER(C.c_uint64))))
+    names = [column_name(chip_id, TRACE_MAIN, c) for c in range(width)]
+    cells = [FreeCell(int(e["row"]), int(e["column"]), names[int(e["column"])]) for e in out[:n.value]]
+    return FreeCells(cells, int(total.value), n.value == total.value, {names[c]: int(per[c]) for c in range(width)})
 
 
 class StarkConfig:

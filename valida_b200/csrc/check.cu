@@ -517,6 +517,13 @@ int32_t vg_cta_scan(vgpu_ctx* ctx, const uint32_t* count, uint32_t m, uint64_t c
     return 0;
 }
 
+int32_t vg_copy_segments(vgpu_ctx* ctx, const VgCopySeg* segs, int n) {
+    if (n > COPY_SEGS) VG_FAIL(ctx, "copy_segments: %d segments exceed %d", n, COPY_SEGS);
+    CopyList l{};
+    for (int i = 0; i < n; i++) l.s[i] = {segs[i].src, segs[i].scs, segs[i].dst, segs[i].dcs, segs[i].n};
+    return copy_segments(ctx, l, n);
+}
+
 bool vg_sums_cancel(const vgpu_check_report report[VGPU_NUM_CHIPS]) {
     for (int l = 0; l < 5; l++) {
         uint64_t s = 0;

@@ -41,6 +41,12 @@ inline const vgpu_dmat* vg_machine_prep(const vgpu_dmat* const prep[2], int i) {
 // check.cu — refuses, before anything is enqueued and alike on every rank, what the check sweep cannot read (perm may be null;
 // shards: this rank's row shards are accepted)
 int32_t vg_check_shapes(vgpu_ctx* ctx, const vgpu_chip_desc* chip, const vgpu_dmat* main, const vgpu_dmat* prep, const vgpu_dmat* perm, bool shards);
+// check.cu — n <= 7 strided copies of n words each, (src, scs) -> (dst, dcs), in one launch of the check's boundary-row copy kernel
+struct VgCopySeg { const uint32_t* src; uint64_t scs; uint32_t* dst; uint64_t dcs; uint32_t n; };
+int32_t vg_copy_segments(vgpu_ctx* ctx, const VgCopySeg* segs, int n);
+// explain.cu — the main columns chip_id's Air::eval reads on the local row and on the next row (bit c % 64 of word c / 64): the unions
+// of the constraint catalogue's cells
+void vg_air_reads(uint32_t chip_id, uint64_t local[2], uint64_t next[2]);
 // check.cu — the same for the 14 + 2 traces of a machine witness (their permutation traces not yet built); `what` names the call
 int32_t vg_check_machine(vgpu_ctx* ctx, const char* what, const vgpu_dmat* const main[VGPU_NUM_CHIPS], const vgpu_dmat* const prep[2]);
 

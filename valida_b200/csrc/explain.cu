@@ -212,6 +212,12 @@ bool constraint_cells(const vgpu_chip_desc* chip, uint32_t c, const char** label
 
 }  // namespace
 
+void vg_air_reads(uint32_t chip_id, uint64_t local[2], uint64_t next[2]) {
+    Cells u{};
+    for (const AirEntry& e : air_entries(chip_id)) u = u | e.cells;
+    for (int w = 0; w < 2; w++) { local[w] = u.l[w]; next[w] = u.n[w]; }
+}
+
 extern "C" const char* vgpu_chip_column_name(const vgpu_chip_desc* chip, int32_t trace, uint32_t column) {
     return column_name(chip, trace, column);
 }
