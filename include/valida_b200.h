@@ -531,6 +531,41 @@ typedef struct vgpu_free_cell {
 int32_t vgpu_free_cells(vgpu_ctx* ctx, const vgpu_chip_desc* chip, const vgpu_dmat* main, const vgpu_dmat* prep_or_null,
                         uint64_t cap, vgpu_free_cell* out, uint64_t* n_out, uint64_t* total, uint64_t* rows_per_column);
 
+/* One main-trace cell that some constraint depends on and that the constraints would accept at other values. */
+typedef struct vgpu_cell_alternative {
+    int64_t row;                /* global row */
+    uint32_t column;            /* main-trace column */
+    uint32_t value;             /* the cell's current word, canonical */
+    uint32_t n_values;          /* 1..3 */
+    uint32_t values[3];         /* the other common roots, canonical, ascending; unused entries 0 */
+    uint32_t bus;               /* 1 when a bus event reads the cell */
+    uint32_t reserved;          /* 0 */
+} vgpu_cell_alternative;
+/* Every main-trace cell (row r, column c) of one chip's witness, holding x0, that the chip's Air::eval assertions would also accept
+ * at another value.  S is the set of assertions whose value depends on the cell: those of row r (the cell as the local row's column
+ * c) and of row (r - 1) mod h with that row's own selectors (the cell as the next row's column c; on a one-row chip the cell is both
+ * of the one evaluation).  Every constraint has degree <= 3, so each assertion of S is a polynomial of degree <= 3 in the cell,
+ * decided exactly from the cell + 0, + 1, + 2 and + 3.  The cell is listed when S is not empty and its polynomials share a root
+ * v != x0 in F_p; its values are all such v (at most 3).  A cell with S empty is not listed: it is vgpu_free_cells' when no bus event
+ * reads it either.  `bus` is vgpu_free_cells' bus rule: some interaction's count gives column c a non-zero summed weight, or an
+ * interaction's count is not 0 on row r and one of its fields gives c a non-zero weight.  Setting one listed cell with bus = 0 of a
+ * witness that passes vgpu_check_witness to one of its values gives a witness that still passes it and vgpu_check_buses, so a proof
+ * of it verifies; a cell with bus = 1 set so leaves the chip's AIR satisfied and unbalances a bus tuple.  On a witness with one wrong
+ * cell that S depends on, the cell's right value is among its values.  Only single cells are judged.  Preprocessed and permutation
+ * cells are not.  Writes:
+ *   - out[0, *n_out): the first min(cap, *total) listed cells, in ascending (row, column) order;
+ *   - *total_bus_free: the listed cells with bus = 0;
+ *   - per_column_or_null (may be NULL, else 2 * chip->width entries): the listed rows of each column, then the bus-free ones.
+ * Takes and refuses what vgpu_free_cells takes and refuses (a null total_bus_free too), before anything is enqueued and alike on every
+ * rank.  One thread per row folds, for each column the AIR reads, the assertions of its row's evaluation and then the previous row's
+ * (4-lane values) into their gcd by pseudo-remainders, and finds its roots in F_p (gcd with t^p - t, then a deterministic split); a
+ * second pass, in the parts of the trace whose cells fall below cap only, writes.  Fails, naming the cell, if a cubic with three roots
+ * is not split in 32 tries (no such cell is known).  Collective on a split context, with byte-identical output on every rank and the
+ * all-gathers of vgpu_free_cells.  Synchronises. */
+int32_t vgpu_cell_alternatives(vgpu_ctx* ctx, const vgpu_chip_desc* chip, const vgpu_dmat* main, const vgpu_dmat* prep_or_null,
+                               uint64_t cap, vgpu_cell_alternative* out, uint64_t* n_out, uint64_t* total, uint64_t* total_bus_free,
+                               uint64_t* per_column_or_null);
+
 /* fib_program of basic/tests/test_prover.rs:35-188 with `imm32 -8(fp)` = n; returns the instruction count (23). */
 uint64_t vgpu_fib_program(uint32_t n, int32_t* out_words /* >= 23*6 */);
 

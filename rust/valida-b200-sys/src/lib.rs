@@ -206,6 +206,27 @@ pub struct vgpu_free_cell {
     pub column: u32,
 }
 
+/// One main-trace cell that some constraint depends on and that the constraints would accept at other values
+/// ([`vgpu_cell_alternatives`]).
+#[repr(C)]
+#[derive(Clone, Copy, Debug, Default, PartialEq, Eq)]
+pub struct vgpu_cell_alternative {
+    /// Global row.
+    pub row: i64,
+    /// Main-trace column.
+    pub column: u32,
+    /// The cell's current word, canonical.
+    pub value: u32,
+    /// 1..3.
+    pub n_values: u32,
+    /// The other common roots, canonical, ascending; unused entries 0.
+    pub values: [u32; 3],
+    /// 1 when a bus event reads the cell.
+    pub bus: u32,
+    /// 0.
+    pub reserved: u32,
+}
+
 extern "C" {
     // ---- context ----
     pub fn vgpu_ctx_create(device: i32, cuda_stream: *mut c_void, out: *mut *mut vgpu_ctx) -> i32;
@@ -312,5 +333,6 @@ extern "C" {
     pub fn vgpu_witness_column_count() -> u64;
     pub fn vgpu_diff_witness(ctx: *mut vgpu_ctx, log: *const vgpu_vmlog, main: *const *const vgpu_dmat, prep: *const *const vgpu_dmat, cap: u64, out: *mut vgpu_cell_diff, n_out: *mut u64, total: *mut u64, summary: *mut vgpu_diff_summary, per_column_or_null: *mut u64) -> i32;
     pub fn vgpu_free_cells(ctx: *mut vgpu_ctx, chip: *const vgpu_chip_desc, main: *const vgpu_dmat, prep_or_null: *const vgpu_dmat, cap: u64, out: *mut vgpu_free_cell, n_out: *mut u64, total: *mut u64, rows_per_column: *mut u64) -> i32;
+    pub fn vgpu_cell_alternatives(ctx: *mut vgpu_ctx, chip: *const vgpu_chip_desc, main: *const vgpu_dmat, prep_or_null: *const vgpu_dmat, cap: u64, out: *mut vgpu_cell_alternative, n_out: *mut u64, total: *mut u64, total_bus_free: *mut u64, per_column_or_null: *mut u64) -> i32;
     pub fn vgpu_fib_program(n: u32, out_words: *mut i32) -> u64;
 }

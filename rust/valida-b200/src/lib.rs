@@ -432,6 +432,28 @@ impl Context {
         Ok((out, total, per))
     }
 
+    /// Every main-trace cell of one chip's witness that the chip's `Air::eval` assertions would also accept at another value (the
+    /// assertions that depend on the cell share a root other than its value), with those values: the first `min(cap, total)` in
+    /// ascending (row, column) order, the total, the number whose `bus` is 0, and per column the listed rows followed by the bus-free
+    /// ones (`2 * width` entries).  Takes what [`Context::free_cells`] takes and refuses the same traces; collective on a split
+    /// context, with the same result on every rank.  Synchronises.
+    pub fn cell_alternatives(&self, chip_id: u32, main: &DMat<'_>, prep: Option<&DMat<'_>>, cap: usize) -> Result<(Vec<sys::vgpu_cell_alternative>, u64, u64, Vec<u64>)> {
+        let chip = unsafe { sys::vgpu_basic_machine_chip(chip_id) };
+        if chip.is_null() {
+            return Err(Error { code: -1, message: format!("cell_alternatives: unknown chip id {chip_id}") });
+        }
+        let width = unsafe { (*chip).width } as usize;
+        let prep_ptr = prep.map_or(ptr::null(), |m| m.as_ptr());
+        let mut out = vec![sys::vgpu_cell_alternative::default(); cap];
+        let mut per = vec![0u64; 2 * width];
+        let (mut n, mut total, mut bus_free) = (0u64, 0u64, 0u64);
+        self.check(unsafe {
+            sys::vgpu_cell_alternatives(self.raw, chip, main.as_ptr(), prep_ptr, cap as u64, out.as_mut_ptr(), &mut n, &mut total, &mut bus_free, per.as_mut_ptr())
+        })?;
+        out.truncate(n as usize);
+        Ok((out, total, bus_free, per))
+    }
+
     /// The witness check of the reference's debug builds (`check_constraints` of every chip + `check_cumulative_sums`,
     /// `derive/src/lib.rs:246-253,376-377`) without a proof, with the caller's 15 challenge words: one report per chip and whether
     /// the cumulative sums cancel.  `main` / `prep` are whole traces or, on a [`LocalGroup`] rank, its row shards; every rank of a

@@ -73,6 +73,9 @@ CELL_DIFF_DTYPE = np.dtype([("chip", "<u4"), ("trace", "<u4"), ("column", "<u4")
 DIFF_SUMMARY_DTYPE = np.dtype([("height_have", "<u8"), ("height_want", "<u8"), ("cells", "<u8"), ("first_row", "<i8")])
 # vgpu_free_cell (include/valida_b200.h): one main-trace cell no check pins
 FREE_CELL_DTYPE = np.dtype([("row", "<i8"), ("column", "<u4")], align=True)
+# vgpu_cell_alternative (include/valida_b200.h): one cell the constraints would accept at other values
+CELL_ALTERNATIVE_DTYPE = np.dtype([("row", "<i8"), ("column", "<u4"), ("value", "<u4"), ("n_values", "<u4"), ("values", "<u4", 3),
+                                   ("bus", "<u4"), ("reserved", "<u4")], align=True)
 
 
 def _load():
@@ -166,6 +169,7 @@ def _load():
         "vgpu_diff_witness": (C.c_int32, [vp, vp, C.POINTER(vp), C.POINTER(vp), u64, vp, C.POINTER(u64), C.POINTER(u64), vp, C.POINTER(u64)]),
         "vgpu_vmlog_free": (None, [vp]),
         "vgpu_free_cells": (C.c_int32, [vp, vp, vp, vp, u64, vp, C.POINTER(u64), C.POINTER(u64), C.POINTER(u64)]),
+        "vgpu_cell_alternatives": (C.c_int32, [vp, vp, vp, vp, u64, vp, C.POINTER(u64), C.POINTER(u64), C.POINTER(u64), C.POINTER(u64)]),
     }
     for name, (res, args) in sig.items():
         f = getattr(L, name)
@@ -883,6 +887,38 @@ def free_cells(ctx, chip_id, main, prep, cap=1 << 16):
     names = [column_name(chip_id, TRACE_MAIN, c) for c in range(width)]
     cells = [FreeCell(int(e["row"]), int(e["column"]), names[int(e["column"])]) for e in out[:n.value]]
     return FreeCells(cells, int(total.value), n.value == total.value, {names[c]: int(per[c]) for c in range(width)})
+
+
+CellAlternative = collections.namedtuple("CellAlternative", "row column column_name value values bus")
+CellAlternatives = collections.namedtuple("CellAlternatives", "cells total bus_free complete per_column")
+
+
+def cell_alternatives(ctx, chip_id, main, prep, cap=1 << 16):
+    """Every main-trace cell of one chip's witness that the chip's Air::eval assertions would also accept at another value: S, the
+    assertions whose value depends on the cell (on its row, and on the row before as that row's next row), is not empty and its
+    polynomials in the cell share a root other than the cell's value.  Those roots are the cell's values.  bus: a bus event reads the
+    cell (free_cells' rule).  Setting one such cell with bus False of a witness that passes check_witness to one of its values leaves
+    the witness passing check_witness and check_buses, so its proof still verifies; on a witness with one wrong cell that an assertion
+    reads, the right value is among that cell's values.  Takes what free_cells takes (collective on a split context, with the same
+    result on every rank).  Returns CellAlternatives(cells, total, bus_free, complete, per_column): the first min(cap, total)
+    CellAlternative(row, column, column_name, value, values, bus) in ascending (row, column) order (value and values canonical, values
+    ascending), the number of listed cells and of those with bus False, whether cells holds them all, and per column name
+    (listed, bus_free) rows."""
+    cap = int(cap)
+    chip = lib().vgpu_basic_machine_chip(chip_id)
+    if not chip:
+        raise VgpuError("cell_alternatives: unknown chip id %r" % (chip_id,))
+    width = C.cast(chip, C.POINTER(_ChipDesc)).contents.width
+    out = np.zeros(cap, dtype=CELL_ALTERNATIVE_DTYPE)
+    per = np.zeros(2 * width, dtype=np.uint64)
+    n, total, bus_free = C.c_uint64(), C.c_uint64(), C.c_uint64()
+    ctx.check(lib().vgpu_cell_alternatives(ctx._h, chip, main._h, _h(prep), cap, out.ctypes.data_as(C.c_void_p) if cap else None,
+                                           C.byref(n), C.byref(total), C.byref(bus_free), per.ctypes.data_as(C.POINTER(C.c_uint64))))
+    names = [column_name(chip_id, TRACE_MAIN, c) for c in range(width)]
+    cells = [CellAlternative(int(e["row"]), int(e["column"]), names[int(e["column"])], int(e["value"]),
+                             tuple(int(v) for v in e["values"][:int(e["n_values"])]), bool(e["bus"])) for e in out[:n.value]]
+    return CellAlternatives(cells, int(total.value), int(bus_free.value), n.value == total.value,
+                            {names[c]: (int(per[c]), int(per[width + c])) for c in range(width)})
 
 
 class StarkConfig:

@@ -17,49 +17,17 @@
 // is in (row, column) order.  A split chip's run needs the row before its first row and the row after its last: each rank packs its
 // first and last main rows into a small block (check_copy_kernel) and one all-gather exchanges them (no peer pointers: a borrowed
 // shard is caller memory).
-#include "ctx.h"
-#include "devchip.h"
-#include "airs.cuh"
-#include "logup.cuh"
+#include "cells.cuh"
 #include "lists.cuh"
 
 namespace {
 
-constexpr int FREE_THREADS = 128, FREE_WARPS = FREE_THREADS / 32, FREE_MAX_COLS = 128;
+constexpr int FREE_THREADS = 128, FREE_WARPS = FREE_THREADS / 32, FREE_MAX_COLS = CELLS_MAX_COLS;
 static_assert(sizeof(vgpu_free_cell) == 16, "vgpu_free_cell is 4 words");
 
-// one expression's value with the cell under test at +0, +1, +2 and +3 (Montgomery)
-struct F4 {
-    uint32_t v[4];
-};
-BB_HD F4 operator+(const F4& a, const F4& b) { return F4{{bb::add(a.v[0], b.v[0]), bb::add(a.v[1], b.v[1]), bb::add(a.v[2], b.v[2]), bb::add(a.v[3], b.v[3])}}; }
-BB_HD F4 operator-(const F4& a, const F4& b) { return F4{{bb::sub(a.v[0], b.v[0]), bb::sub(a.v[1], b.v[1]), bb::sub(a.v[2], b.v[2]), bb::sub(a.v[3], b.v[3])}}; }
-BB_HD F4 operator*(const F4& a, const F4& b) { return F4{{bb::mul(a.v[0], b.v[0]), bb::mul(a.v[1], b.v[1]), bb::mul(a.v[2], b.v[2]), bb::mul(a.v[3], b.v[3])}}; }
-
-}  // namespace
-
-namespace air {
-template <> struct Lift<F4> { static BB_HD F4 from_monty_word(uint32_t m) { return F4{{m, m, m, m}}; } };
-}  // namespace air
-
-namespace {
-
-struct LaneBuilder {
-    using V = F4;
-    const uint32_t* lrow; uint64_t lcs;             // the evaluated row and its next row, each with its column stride
-    const uint32_t* nrow; uint64_t ncs;
-    V first, last, trans;
-    int tl, tn;                                     // the column under test as L(c) / as N(c) (-1: none)
+struct LaneBuilder : VgLanes {
     bool dep;                                       // some assertion's value changed with the cell
-    __device__ __forceinline__ static V at(uint32_t x, bool test) {
-        if (!test) return V{{x, x, x, x}};
-        const uint32_t x1 = bb::add(x, bb::R1), x2 = bb::add(x1, bb::R1);
-        return V{{x, x1, x2, bb::add(x2, bb::R1)}};
-    }
-    __device__ __forceinline__ V L(int c) const { return at(__ldg(lrow + (uint64_t)c * lcs), c == tl); }
-    __device__ __forceinline__ V N(int c) const { return at(__ldg(nrow + (uint64_t)c * ncs), c == tn); }
     __device__ __forceinline__ void z(const V& x) { dep |= (x.v[1] != x.v[0]) | (x.v[2] != x.v[0]) | (x.v[3] != x.v[0]); }
-    __device__ __forceinline__ void section(const char*) {}
 };
 
 struct MParams {
@@ -70,9 +38,7 @@ struct MParams {
     uint64_t g0, n, h;                              // global row of local row 0; rows swept; global height
     uint64_t air_l[2], air_n[2];                    // columns the AIR text reads on the local / next row (bit c % 64 of word c / 64)
     uint64_t cols[2];                               // the chip's columns
-    uint64_t bus_count[2];                          // columns some interaction's count gives a non-zero weight
-    uint64_t bus_fields[VGPU_MAX_INTERACTIONS][2];  // columns interaction m's fields give a non-zero weight
-    DevPairCol count[VGPU_MAX_INTERACTIONS];
+    VgBusMasks bus;
     uint32_t k, width;
     uint32_t* cta_count;                            // free cells of each CTA
     unsigned long long* per_col;                    // mask pass: free cells per column
@@ -84,11 +50,11 @@ struct MParams {
 template <int CHIP>
 __device__ __forceinline__ void free_mask(const MParams& p, uint64_t i, uint64_t& f0, uint64_t& f1) {
     const uint32_t* row = p.main + i;
-    uint64_t pin0 = p.bus_count[0], pin1 = p.bus_count[1];
+    uint64_t pin0 = p.bus.count_cols[0], pin1 = p.bus.count_cols[1];
     for (uint32_t m = 0; m < p.k; m++)
-        if (logup::pair_col(p.count[m], row, p.mcs, p.prep ? p.prep + i : nullptr, p.pcs) != 0) {
-            pin0 |= p.bus_fields[m][0];
-            pin1 |= p.bus_fields[m][1];
+        if (logup::pair_col(p.bus.count[m], row, p.mcs, p.prep ? p.prep + i : nullptr, p.pcs) != 0) {
+            pin0 |= p.bus.fields[m][0];
+            pin1 |= p.bus.fields[m][1];
         }
     const uint64_t g = p.g0 + i, one_row = p.h == 1;
     LaneBuilder b;
@@ -174,16 +140,6 @@ __global__ void __launch_bounds__(FREE_THREADS, 1) free_write_kernel(const __gri
         }
 }
 
-// the main columns a VirtualPairCol gives a non-zero summed weight (preprocessed terms are the verifier's)
-void weighted_columns(const vgpu_pair_col& pc, uint64_t mask[2]) {
-    uint64_t sum[FREE_MAX_COLS] = {};
-    for (uint32_t t = 0; t < pc.n_terms && t < VGPU_MAX_TERMS; t++)
-        if (!pc.terms[t].is_preprocessed && pc.terms[t].column < FREE_MAX_COLS)
-            sum[pc.terms[t].column] = (sum[pc.terms[t].column] + pc.terms[t].weight % bb::P) % bb::P;
-    for (uint32_t c = 0; c < FREE_MAX_COLS; c++)
-        if (sum[c]) mask[c >> 6] |= 1ull << (c & 63);
-}
-
 }  // namespace
 
 extern "C" int32_t vgpu_free_cells(vgpu_ctx* ctx, const vgpu_chip_desc* chip, const vgpu_dmat* main, const vgpu_dmat* prep_or_null,
@@ -209,17 +165,7 @@ extern "C" int32_t vgpu_free_cells(vgpu_ctx* ctx, const vgpu_chip_desc* chip, co
     p->g0 = run.begin; p->n = run.count; p->h = h; p->width = w; p->k = chip->n_interactions;
     vg_air_reads(chip->chip_id, p->air_l, p->air_n);
     for (uint32_t c = 0; c < w; c++) p->cols[c >> 6] |= 1ull << (c & 63);
-    {
-        auto dev = std::make_unique<DevChip>();
-        const uint32_t no_challenges[15] = {};
-        VG_TRY(vg_build_devchip(ctx, chip, no_challenges, dev.get()));
-        for (uint32_t m = 0; m < p->k; m++) {
-            const vgpu_interaction& it = chip->interactions[m];
-            weighted_columns(it.count, p->bus_count);
-            for (uint32_t f = 0; f < it.n_fields; f++) weighted_columns(it.fields[f], p->bus_fields[m]);
-            p->count[m] = dev->interactions[m].count;
-        }
-    }
+    VG_TRY(vg_bus_masks(ctx, chip, &p->bus));
     VgBuf counts(ctx), cta(ctx), off(ctx), endb(ctx), edges(ctx);
     VG_TRY(counts.alloc(N * words * 8));
     VG_TRY(cta.alloc(ctas * 4ull));
@@ -228,19 +174,7 @@ extern "C" int32_t vgpu_free_cells(vgpu_ctx* ctx, const vgpu_chip_desc* chip, co
     unsigned long long* mine = counts.as<unsigned long long>() + (uint64_t)me * words;
     VG_CUDA(ctx, cudaMemsetAsync(mine, 0, words * 8, ctx->stream));
     VG_CUDA(ctx, cudaMemsetAsync(cta.p, 0, ctas * 4ull, ctx->stream));
-    if (run.split) {
-        // per rank [first row | last row] of its run; the row before ours is the previous rank's last, the row after the next's first
-        VG_TRY(edges.alloc((size_t)N * 2 * w * 4));
-        uint32_t* blk = edges.as<uint32_t>() + (uint64_t)me * 2 * w;
-        const VgCopySeg segs[2] = {{p->main, p->mcs, blk, 1, w}, {p->main + run.count - 1, p->mcs, blk + w, 1, w}};
-        VG_TRY(vg_copy_segments(ctx, segs, 2));
-        VG_TRY(vg_comm_allgather_inplace(ctx, edges.as<uint32_t>(), 2 * (uint64_t)w));
-        p->before = edges.as<uint32_t>() + (uint64_t)((me + N - 1) % N) * 2 * w + w; p->bcs = 1;
-        p->after = edges.as<uint32_t>() + (uint64_t)((me + 1) % N) * 2 * w; p->acs = 1;
-    } else {
-        p->before = p->main + h - 1; p->bcs = p->mcs;
-        p->after = p->main; p->acs = p->mcs;
-    }
+    VG_TRY(vg_edge_rows(ctx, run, p->main, p->mcs, h, w, edges, &p->before, &p->bcs, &p->after, &p->acs));
     p->cta_count = cta.as<uint32_t>(); p->per_col = mine + 1;
     {
         KScope ks(ctx, KC_CHECK, 4.0 * (double)run.count * w);
