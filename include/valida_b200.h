@@ -353,6 +353,37 @@ int32_t vgpu_check_buses(vgpu_ctx* ctx, const vgpu_dmat* const main[VGPU_NUM_CHI
                          vgpu_bus_imbalance* tuples, uint64_t* n_tuples,
                          vgpu_bus_event* events, uint64_t* n_events, uint64_t* unexamined);
 
+/* One item's answer of vgpu_bus_links. */
+typedef struct vgpu_bus_link {
+    uint32_t bus;
+    uint32_t fields[VGPU_MAX_FIELDS];  /* the item's tuple on its row, canonical, zero-padded */
+    uint32_t multiplicity;             /* the item's own count on its row, canonical; 0: the item is not an event */
+    uint32_t sends, receives;          /* summed multiplicities of ALL events carrying the tuple, canonical */
+    uint64_t n_events;                 /* number of events carrying the tuple, exact */
+    uint64_t first_event;              /* events[first_event, first_event + n_events) when listed, else UINT64_MAX */
+} vgpu_bus_link;
+/* Every event of a machine witness that carries the tuple of each of n items, on both sides of its bus: the CPU cycle behind an ALU
+ * row is the CPU row whose general-bus send carries the ALU row's tuple, and so on.  An item is (chip, interaction, row) given as a
+ * vgpu_bus_event whose multiplicity and is_send are ignored, so vgpu_check_buses' events and this call's own are items as they are.
+ * Writes:
+ *   - links[i]: item i's tuple on its row, its own count, and, over the whole witness, the summed send and receive multiplicities and
+ *     the number of the events carrying the tuple (exact whatever cap is), and where they are listed;
+ *   - events[0, *n_events): the events of the listed tuples.  The distinct tuples of the items are ordered ascending by (bus, fields);
+ *     each one's events are listed once, in ascending (chip, row, interaction) order, and items with the same tuple share that range;
+ *   - *unlisted: the distinct tuples whose events did not fit: the listed ones are the longest prefix whose events fit in cap.
+ * For a tuple vgpu_check_buses reports, the events are its events and sends - receives is its net.  Takes what vgpu_check_buses takes
+ * (whole matrices, or this rank's row shards; uploaded, imported or borrowed, with any column stride) and refuses what it refuses, an
+ * item whose chip is not below 14, whose interaction is not below the chip's interactions or whose row is outside the chip's trace
+ * (naming the item), and null outputs (events only when cap > 0), before anything is enqueued and alike on every rank.  Each item's
+ * words are read by the rank that holds its row (rank 0 of a whole matrix); one sweep of every row of this rank's run counts each
+ * tuple's events through a hash table of the items' tuples, and a second, only when a listed tuple has events, writes them.
+ * Collective on a split context, with byte-identical output on every rank: one all-gather of the items' words (summed), one of the
+ * per-rank counts and sums, and, when a listed tuple has events, one of each rank's listed events.  Synchronises; the traces are left
+ * untouched. */
+int32_t vgpu_bus_links(vgpu_ctx* ctx, const vgpu_dmat* const main[VGPU_NUM_CHIPS], const vgpu_dmat* const prep[2],
+                       const vgpu_bus_event* items, uint64_t n, vgpu_bus_link* links /* n */,
+                       uint64_t cap, vgpu_bus_event* events, uint64_t* n_events, uint64_t* unlisted);
+
 /* ---- Fiat-Shamir transcript owned by the context (DuplexChallenger; config.challenger() clone) ------
  * reset() restores the initial sponge of vgpu_set_challenger; values are canonical words. */
 int32_t vgpu_challenger_reset(vgpu_ctx* ctx);

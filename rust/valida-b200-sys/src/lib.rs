@@ -166,6 +166,24 @@ pub struct vgpu_bus_imbalance {
     pub n_events: u64,
 }
 
+/// One item's answer of [`vgpu_bus_links`]: its tuple, its own count, and the events of the whole witness that carry the tuple.
+#[repr(C)]
+#[derive(Clone, Copy, Debug, Default, PartialEq, Eq)]
+pub struct vgpu_bus_link {
+    pub bus: u32,
+    /// The item's tuple on its row, canonical, zero-padded.
+    pub fields: [u32; VGPU_MAX_FIELDS],
+    /// The item's own count on its row, canonical; 0: the item is not an event.
+    pub multiplicity: u32,
+    /// Summed multiplicities of all events carrying the tuple, canonical.
+    pub sends: u32,
+    pub receives: u32,
+    /// Number of events carrying the tuple, exact.
+    pub n_events: u64,
+    /// `events[first_event..first_event + n_events]` when listed, else `u64::MAX`.
+    pub first_event: u64,
+}
+
 /// One cell of a caller's witness that differs from what `Chip::generate_trace` writes for the run ([`vgpu_diff_witness`]).
 #[repr(C)]
 #[derive(Clone, Copy, Debug, Default, PartialEq, Eq)]
@@ -287,6 +305,7 @@ extern "C" {
     pub fn vgpu_explain_failures(ctx: *mut vgpu_ctx, chip: *const vgpu_chip_desc, main: *const vgpu_dmat, prep_or_null: *const vgpu_dmat, perm_or_null: *const vgpu_dmat, items: *const vgpu_check_failure, n: u64, first: *mut u64, values: *mut u32, cap: u64, n_values: *mut u64) -> i32;
     pub fn vgpu_check_witness(ctx: *mut vgpu_ctx, main: *const *const vgpu_dmat, prep: *const *const vgpu_dmat, challenges: *const u32, report: *mut vgpu_check_report, sums_cancel: *mut i32) -> i32;
     pub fn vgpu_check_buses(ctx: *mut vgpu_ctx, main: *const *const vgpu_dmat, prep: *const *const vgpu_dmat, challenges: *const u32, cap: u64, tuples: *mut vgpu_bus_imbalance, n_tuples: *mut u64, events: *mut vgpu_bus_event, n_events: *mut u64, unexamined: *mut u64) -> i32;
+    pub fn vgpu_bus_links(ctx: *mut vgpu_ctx, main: *const *const vgpu_dmat, prep: *const *const vgpu_dmat, items: *const vgpu_bus_event, n: u64, links: *mut vgpu_bus_link, cap: u64, events: *mut vgpu_bus_event, n_events: *mut u64, unlisted: *mut u64) -> i32;
 
     // ---- transcript ----
     pub fn vgpu_challenger_reset(ctx: *mut vgpu_ctx) -> i32;

@@ -485,6 +485,27 @@ impl Context {
         Ok((tuples, events, unexamined))
     }
 
+    /// Every event of the witness that carries each item's bus tuple, sends and receives alike (the items' `multiplicity` and
+    /// `is_send` are ignored, so the events of [`Context::check_buses`] and of this call are items as they are): one link per item
+    /// (its tuple, its own count, the summed send and receive multiplicities and the number of events carrying the tuple, exact), the
+    /// events of the listed tuples (tuple order ascending by (bus, fields), each tuple's events ascending by (chip, row, interaction),
+    /// shared by the items with that tuple; an unlisted tuple's `first_event` is `u64::MAX`) and the number of distinct tuples whose
+    /// events did not fit under `cap`.  Takes what [`Context::check_buses`] takes; collective on a split context, with the same result
+    /// on every rank.  Synchronises.
+    pub fn bus_links(&self, main: &[&DMat<'_>; sys::VGPU_NUM_CHIPS], prep: &[&DMat<'_>; 2], items: &[sys::vgpu_bus_event], cap: usize)
+                     -> Result<(Vec<sys::vgpu_bus_link>, Vec<sys::vgpu_bus_event>, u64)> {
+        let (main_raw, prep_raw) = Self::witness_ptrs(main, prep);
+        let mut links = vec![sys::vgpu_bus_link::default(); items.len()];
+        let mut events = vec![sys::vgpu_bus_event::default(); cap];
+        let (mut ne, mut unlisted) = (0u64, 0u64);
+        self.check(unsafe {
+            sys::vgpu_bus_links(self.raw, main_raw.as_ptr(), prep_raw.as_ptr(), items.as_ptr(), items.len() as u64, links.as_mut_ptr(), cap as u64,
+                                events.as_mut_ptr(), &mut ne, &mut unlisted)
+        })?;
+        events.truncate(ne as usize);
+        Ok((links, events, unlisted))
+    }
+
     /// The values of the cells each `(row, constraint)` item reads (the items' `value` fields are ignored: [`Context::check_failures`]'
     /// list as it is; a bus event of [`Context::check_buses`] is `(row, air_constraints + interaction)`), per item in
     /// [`constraint_cells`] order, canonical; a next-row cell is read at `(row + 1) mod h`.  Without `perm` the permutation cells are

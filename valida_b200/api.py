@@ -61,6 +61,9 @@ CHECK_FAILURE_DTYPE = np.dtype([("row", "<i8"), ("constraint", "<u4"), ("value",
 # vgpu_bus_event / vgpu_bus_imbalance (include/valida_b200.h)
 BUS_EVENT_DTYPE = np.dtype([("chip", "<u4"), ("interaction", "<u4"), ("row", "<i8"), ("multiplicity", "<u4"), ("is_send", "<u4")])
 BUS_IMBALANCE_DTYPE = np.dtype([("bus", "<u4"), ("fields", "<u4", (14,)), ("net", "<u4"), ("first_event", "<u8"), ("n_events", "<u8")], align=True)
+# vgpu_bus_link (include/valida_b200.h): one item's tuple, its own count, and the events that carry its tuple
+BUS_LINK_DTYPE = np.dtype([("bus", "<u4"), ("fields", "<u4", (14,)), ("multiplicity", "<u4"), ("sends", "<u4"), ("receives", "<u4"),
+                           ("n_events", "<u8"), ("first_event", "<u8")], align=True)
 # BasicMachine's chips and buses (basic/src/lib.rs:151-166, 1190-1212), by id
 CHIP_NAMES = ("cpu", "program", "memory", "add", "sub", "mul", "div", "shift", "lt", "com", "bitwise", "output", "range", "static_data")
 BUS_NAMES = ("general", "program", "memory", "range")
@@ -132,6 +135,7 @@ def _load():
         "vgpu_explain_failures": (C.c_int32, [vp, vp, vp, vp, vp, vp, u64, C.POINTER(u64), u32p, u64, C.POINTER(u64)]),
         "vgpu_check_witness": (C.c_int32, [vp, C.POINTER(vp), C.POINTER(vp), u32p, C.POINTER(_CheckReport), C.POINTER(C.c_int32)]),
         "vgpu_check_buses": (C.c_int32, [vp, C.POINTER(vp), C.POINTER(vp), u32p, u64, vp, C.POINTER(u64), vp, C.POINTER(u64), C.POINTER(u64)]),
+        "vgpu_bus_links": (C.c_int32, [vp, C.POINTER(vp), C.POINTER(vp), vp, u64, vp, u64, vp, C.POINTER(u64), C.POINTER(u64)]),
         "vgpu_ctx_set_debug_checks": (C.c_int32, [vp, C.c_int32]),
         "vgpu_set_challenger": (C.c_int32, [vp, u32p, u32p]),
         "vgpu_ctx_set_merkle_hash": (C.c_int32, [vp, C.c_int32]),
@@ -815,6 +819,96 @@ def check_buses(ctx, main, prep, challenges, cap=1 << 16):
         out.append(BusImbalance(int(t["bus"]), BUS_NAMES[int(t["bus"])] if t["bus"] < len(BUS_NAMES) else "bus %d" % t["bus"], fields,
                                 net - BABYBEAR_P if net > BABYBEAR_P // 2 else net, events))
     return BusCheck(out, un.value == 0, int(un.value))
+
+
+BusLink = collections.namedtuple("BusLink", "bus bus_name fields multiplicity sends receives n_events events")
+BusLinks = collections.namedtuple("BusLinks", "links complete unlisted")
+Cycles = collections.namedtuple("Cycles", "cycles complete")
+
+
+def _bus_name(bus):
+    return BUS_NAMES[bus] if bus < len(BUS_NAMES) else "bus %d" % bus
+
+
+def bus_links(ctx, main, prep, items, cap=1 << 16):
+    """Every event of the witness that carries each item's bus tuple, sends and receives alike: the CPU cycle whose general-bus send
+    carries an ALU row's tuple, the memory row that receives a CPU channel's operation, the add and sub rows that send a range row's
+    byte.  items: a BUS_EVENT_DTYPE array, check_buses' BusEvents or (chip, interaction, row) triples (multiplicity and direction are
+    ignored, so an answer's events are items as they are).  Takes what check_buses takes (whole traces, or this rank's row shards on a
+    split context, where every rank calls it with the same items and gets the same answer).  Returns BusLinks(links, complete,
+    unlisted), one BusLink(bus, bus_name, fields trimmed of trailing zeros, multiplicity, sends, receives, n_events, events) per item:
+    its tuple on its row, its own count (0: the item is no event), the summed send and receive multiplicities and the number of all
+    events carrying the tuple (exact whatever cap is), and those events as BusEvents in ascending (chip, row, interaction) order, or
+    None when its tuple was not listed.  Distinct tuples are listed in ascending (bus, fields) order while their events fit in cap;
+    unlisted counts the others."""
+    if isinstance(items, np.ndarray) and items.dtype == BUS_EVENT_DTYPE:
+        arr = np.ascontiguousarray(items)
+    else:
+        triples = [(x.chip, x.interaction, x.row) if isinstance(x, BusEvent) else tuple(x) for x in items]
+        arr = np.zeros(len(triples), dtype=BUS_EVENT_DTYPE)
+        for i, (chip, m, row) in enumerate(triples):
+            arr[i]["chip"], arr[i]["interaction"], arr[i]["row"] = chip, m, row
+    n, cap = len(arr), int(cap)
+    links = np.zeros(max(n, 1), dtype=BUS_LINK_DTYPE)
+    ev = np.zeros(max(cap, 1), dtype=BUS_EVENT_DTYPE)
+    ne, un = C.c_uint64(), C.c_uint64()
+    ctx.check(lib().vgpu_bus_links(ctx._h, *_witness_handles(main, prep), arr.ctypes.data_as(C.c_void_p) if n else None, n,
+                                   links.ctypes.data_as(C.c_void_p), cap, ev.ctypes.data_as(C.c_void_p) if cap else None,
+                                   C.byref(ne), C.byref(un)))
+    evs = [BusEvent(chip, CHIP_NAMES[chip], m, row, mult, bool(send)) for chip, m, row, mult, send in ev[:ne.value].tolist()]
+    out = []
+    for bus, fields, mult, sends, receives, k, e0 in links[:n].tolist():
+        fields = fields.tolist()
+        while fields and fields[-1] == 0:
+            fields.pop()
+        events = evs[e0:e0 + k] if e0 != 0xFFFFFFFFFFFFFFFF else None
+        out.append(BusLink(bus, _bus_name(bus), fields, mult, sends, receives, k, events))
+    return BusLinks(out, un.value == 0, int(un.value))
+
+
+def _neighbours(ctx, main, prep, nodes, cap):
+    """For each (chip, row) node, the nodes that carry an event of a tuple it carries an event of (itself left out), by one
+    bus_links call over every interaction of every node; and whether every tuple was listed."""
+    nodes = sorted(set(nodes))
+    items = [(chip, m, row) for chip, row in nodes for m in range(_interaction_count(chip))]
+    res = bus_links(ctx, main, prep, items, cap)
+    out = {node: set() for node in nodes}
+    for (chip, _, row), link in zip(items, res.links):
+        if link.multiplicity and link.events is not None:
+            out[(chip, row)].update((e.chip, e.row) for e in link.events)
+    for node in nodes:
+        out[node].discard(node)
+    return out, res.complete
+
+
+def _interaction_count(chip):
+    return C.cast(lib().vgpu_basic_machine_chip(chip), C.POINTER(_ChipDesc)).contents.n_interactions
+
+
+def cycles_of(ctx, main, prep, chip, rows, cap=1 << 16):
+    """The cycles behind rows of one chip: in the graph whose nodes are (chip, row) and whose edges join two nodes that each carry an
+    event of the same bus tuple, the CPU rows (cycles) at the least distance from the row, searching up to distance 2.  A CPU row is
+    its own cycle; an ALU or memory row is at distance 1 from the cycles that send it its tuple; a range row reaches cycles through the
+    add and sub rows that send it its byte.  Empty when no CPU row is that close: a static-initial memory row, a row without events,
+    a row whose tuple no CPU row sends.  Two bus_links calls at most (so collective on a split context, as bus_links is).  Returns
+    Cycles(cycles, complete): per row, its cycles ascending, and whether cap let every tuple consulted list its events."""
+    rows = [int(r) for r in rows]
+    if chip == 0:
+        h = main[0].shape[0]
+        bad = [r for r in rows if not 0 <= r < h]
+        if bad:
+            raise VgpuError("cycles_of: row %d is outside the CPU trace of height %d" % (bad[0], h))
+        return Cycles([[r] for r in rows], True)
+    near, complete = _neighbours(ctx, main, prep, [(chip, r) for r in rows], cap)
+    far_nodes = {x for r in rows if not any(c == 0 for c, _ in near[(chip, r)]) for x in near[(chip, r)]}
+    far, done = _neighbours(ctx, main, prep, far_nodes, cap) if far_nodes else ({}, True)
+    cycles = []
+    for r in rows:
+        hit = sorted(x for c, x in near[(chip, r)] if c == 0)
+        if not hit:
+            hit = sorted({x for node in near[(chip, r)] for c, x in far[node] if c == 0})
+        cycles.append(hit)
+    return Cycles(cycles, complete and done)
 
 
 CellDiff = collections.namedtuple("CellDiff", "chip chip_name trace column column_name row have want")

@@ -11,10 +11,8 @@
 //   2. count: the events of each candidate (all-gathered); the longest prefix of candidates whose events fit in cap is examined.
 //   3. write: the events of the examined candidates with their tuple words (all-gathered).
 // The host groups the events by exact tuple, drops the balanced ones that shared a bucket with an unbalanced one, and sorts.
-#include "ctx.h"
-#include "devchip.h"
+#include "bus_events.cuh"
 #include "lists.cuh"
-#include "logup.cuh"
 #include <array>
 #include <map>
 #include <memory>
@@ -22,60 +20,7 @@
 
 namespace {
 
-constexpr uint32_t BUS_NONE = 0xffffffffu;
 constexpr int BUS_LOG_BUCKETS_MIN = 10, BUS_LOG_BUCKETS_MAX = 20;   // B = 2^10 .. 2^20 buckets
-
-// one event as the write pass leaves it, canonical words (22 words: all-gathered as such)
-struct BusEventRec {
-    uint32_t chip, interaction;
-    uint64_t row;
-    uint32_t multiplicity, is_send, bus, fields[VGPU_MAX_FIELDS], pad;
-};
-static_assert(sizeof(BusEventRec) == 88, "BusEventRec is 22 words");
-
-struct BParams {
-    const uint32_t* main; uint64_t mcs;            // at local row 0 of the rows swept
-    const uint32_t* prep; uint64_t pcs;            // null without a preprocessed trace
-    uint64_t g0, n;                                // global row of local row 0; rows swept
-    uint32_t z;                                    // the weights' pole (Montgomery)
-    uint32_t log_b;
-    uint32_t bus[VGPU_MAX_INTERACTIONS];
-    unsigned long long* acc;                       // bucket pass: B sums of +-mult * weight, each term < p
-    const uint32_t* cand;                          // count / write passes: candidate number of each bucket, BUS_NONE if none
-    uint32_t* count;                               // count pass: events per candidate
-    uint32_t examined;                             // write pass: the events of candidates below it are written ...
-    unsigned long long* wpos; BusEventRec* out;    // ... at out[atomicAdd(wpos, 1)]
-    DevChip chip;
-};
-
-// the bucket of a tuple: a fixed 64-bit mix of the bus and the 14 padded field words (Montgomery), alike on every rank
-__device__ __forceinline__ uint32_t bucket_of(uint32_t bus, const uint32_t (&f)[VGPU_MAX_FIELDS], uint32_t log_b) {
-    uint64_t x = 0x9e3779b97f4a7c15ull * (bus + 1);
-#pragma unroll
-    for (int k = 0; k < VGPU_MAX_FIELDS; k++) {
-        x = (x ^ f[k]) * 0xff51afd7ed558ccdull;
-        x ^= x >> 32;
-    }
-    x *= 0xc4ceb9fe1a85ec53ull;
-    x ^= x >> 33;
-    return (uint32_t)(x >> (64 - log_b));
-}
-
-// Calls f(m, mult, fields) for every event of local row i (interaction m, Montgomery words).
-template <class F>
-__device__ __forceinline__ void row_events(const BParams& p, uint64_t i, F&& f) {
-    const uint32_t* ml = p.main + i;
-    const uint32_t* pl = p.prep ? p.prep + i : nullptr;
-    for (uint32_t m = 0; m < p.chip.n_interactions; m++) {
-        const DevInteraction& it = p.chip.interactions[m];
-        const uint32_t mult = logup::pair_col(it.count, ml, p.mcs, pl, p.pcs);
-        if (!mult) continue;
-        uint32_t fv[VGPU_MAX_FIELDS];
-#pragma unroll
-        for (int k = 0; k < VGPU_MAX_FIELDS; k++) fv[k] = (uint32_t)k < it.n_fields ? logup::pair_col(it.fields[k], ml, p.mcs, pl, p.pcs) : 0u;
-        f(m, mult, fv);
-    }
-}
 
 __global__ void __launch_bounds__(256) bus_bucket_kernel(const __grid_constant__ BParams p) {
     const uint64_t i = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
